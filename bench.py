@@ -1,30 +1,32 @@
 #!/usr/bin/env python
-"""bench.py — BASELINE.json metric: "GenRe shapes/sec @128^3 voxel, 1/2/4/8 GPU; cam_bp HBM GB/s vs peak".
+"""bench.py — GenRe's 3D hot path at 128^3 voxels, shapes/s on H100s, with cam_bp HBM GB/s against the HBM peak.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            this repo (one rank per GPU, torchrun for N > 1)
-    python bench.py --impl reference [...]                         the reference's CPU path (rank 0 only)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   this repo (one rank per GPU, torchrun for N > 1)
+    python bench.py --impl reference [...]                                      the reference's CPU path (needs $GENRE_REF)
 
-Workload = BASELINE configs[2]: GenRe full_model inference, batch 16 per GPU, through the reference's FROZEN caller
-``models/genre_full_model.py:116-132 Net.forward`` (an unmodified copy staged in baseline/_ref) on top of this package's
-drop-in toolbox / networks: net1 (2D U-ResNet18, reference code on cuDNN) -> cam_bp -> render_spherical -> sph_pad ->
-net2 (2D inpainting U-ResNet18) -> spherical back-projection -> Unet_3D refiner.  Random-init weights (no checkpoints
-offline; genre_shapehd_b200/synth_genre.py), synthetic rgb / silhouette inputs.  A "step" is one Net.forward over a batch.
+Workload: the 3D half of GenRe full_model inference (models/genre_full_model.py Net.forward of GenRe-ShapeHD), batch 16 per
+GPU, every op on this package's kernels: absolute depth [B,1,256,256] -> camera back-projection to a 128^3 TDF ->
+spherical render (stop-probability scan) -> sph_pad -> spherical back-projection of the padded map -> cat with the clamped
+TDF -> Unet_3D refiner -> pred_voxel [B,1,128,128,128].  The two 2D U-ResNet18 nets of the full model (depth estimation and
+spherical inpainting) are the reference's own code and are not part of this repository: the depth maps are synthetic
+(genre_shapehd_b200/synth.py: spheres and random-depth masks) and the rendered spherical map stands in for the inpainted one.
+Unet_3D has PyTorch's default random initialisation under torch.manual_seed(0).  A "step" is one forward over a batch.
 
 One JSON line on stdout (rank 0):
   value        whole-job shapes/s, inputs resident in HBM, device-timed, max over ranks
-  e2e          the same through predict()+pack_output()'s data flow (netinterface.py:340-350, genre_full_model.py:188-200):
-               pinned host rgb+silhou -> H2D -> Net.forward -> D2H of pred_voxel, every step, double-buffered over streams
-  roofline     the metric's second clause, cam_bp: algorithmic bytes B*(4*H*W + 4*R^3) / whole-op time (project + splat)
-               against the measured HBM peak; `clauses` adds the splat kernel alone, render_spherical, spherical
-               back-projection (HBM) and the Unet_3D refiner (tensor pipe: useful FLOP/s against the measured dense peak)
-  cpu_baseline the reference arm (below) on a bounded sample, run as a sub-process on rank 0 at N = 1
-  secondary    BASELINE configs[1] (cam_bp batch 32) and the same GenRe step with single-pass fp16 conv operands
-  secondary_ddp  BASELINE configs[3] and [4]: ShapeHD fine-tune step and WGAN-GP critic step (batch 8 per GPU), GenRe end-to-end
-               fine-tune + Chamfer (batch 4 per GPU), frozen model classes, DDP over NCCL for N > 1 with the exposed all-reduce time
+  e2e          the same with pinned host depth maps -> H2D -> forward -> D2H of pred_voxel, every step, double-buffered
+  roofline     cam_bp: algorithmic bytes B*(4*H*W + 4*R^3) / whole-op time (project + splat) against the HBM peak;
+               `clauses` adds the splat kernel alone, render_spherical, spherical back-projection (HBM) and the Unet_3D
+               refiner (tensor pipe: useful FLOP/s against the dense peak)
+  cpu_baseline the reference arm (below) on a bounded sample, run as a sub-process on rank 0 at N = 1 (only with $GENRE_REF)
+  secondary    cam_bp at batch 32 and the same step with single-pass fp16 conv operands
 
---impl reference: the same frozen Net.forward on the host CPU: toolbox ops = the CPU oracle port (the reference's ops are
-CUDA-only), networks = the reference's own networks/*.py on torch CPU, every host thread.
-The oracle is only executed by that arm (and therefore by the cpu_baseline sub-process).
+--dump-outputs DIR: after the timed steps, DIR/pred_voxel_0.npy (shape 0 of the last timed step, float32 [128,128,128]) and
+DIR/pred_voxel_sample.npy (4 Mi values of the last step's whole pred_voxel at fixed seeded positions, float32); the inputs
+are the same on every run, so two builds can be compared output for output.
+
+--impl reference: the reference's frozen Net.forward on the host CPU (toolbox ops = the CPU oracle port, networks = the
+reference's own networks/*.py on torch CPU); it needs a GenRe-ShapeHD checkout ($GENRE_REF).
 """
 import argparse
 import json
@@ -45,7 +47,7 @@ if REPO not in sys.path:
 H = W = 256
 RES = 128
 FL, CAM_DIST = 418.3, 2.2
-METRIC = "GenRe shapes/sec @128^3 voxel (full_model inference); cam_bp HBM GB/s vs peak"
+METRIC = "GenRe shapes/sec @128^3 voxel (3D hot path: cam_bp, render, sph_bp, Unet_3D); cam_bp HBM GB/s vs peak"
 UNIT = "shapes/s"
 UNET3D_GFLOP = 78.0          # per shape, forward (SURVEY 8a a12 / Appendix A)
 
@@ -57,22 +59,24 @@ def parse():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=16, help="shapes per GPU per step (BASELINE configs[2]: 16)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/*.npy (float32)")
     ap.add_argument("--no-graph", action="store_true", help="launch steps from Python instead of replaying a CUDA graph")
     ap.add_argument("--cpu-seconds", type=float, default=25.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--cpu-budget", type=float, default=150.0, help="--impl reference: wall-clock budget of the whole run (s)")
     ap.add_argument("--skip", default=os.environ.get("GENRE_B200_BENCH_SKIP", ""),
-                    help="comma list of legs to skip: e2e,roofline,cpu,secondary,ddp")
+                    help="comma list of legs to skip: e2e,roofline,cpu,secondary")
     return ap.parse_args()
 
 
 def config(args, n_gpus, extra=None):
-    c = {"workload": "GenRe full_model inference (depth + sph-inpaint + voxel refine), batch=%d per GPU (BASELINE configs[2]), "
-                     "frozen models/genre_full_model.py Net.forward on the drop-in toolbox/networks" % args.batch,
+    c = {"workload": "GenRe 3D hot path (cam_bp -> render_spherical -> sph_pad -> spherical back-projection -> Unet_3D), "
+                     "batch=%d per GPU, synthetic depth maps" % args.batch,
          "batch_per_gpu": args.batch, "global_batch": args.batch * n_gpus, "rgb_hw": [H, W], "voxel_res": RES,
-         "weights": "random init (PyTorch defaults; min/max-depth head biased to the dataset depth range so cam_bp hits the grid)",
+         "weights": "Unet_3D: random init (PyTorch defaults, torch.manual_seed(0))",
          "parallelism": "replicas x%d (batch-sharded, no collective)" % n_gpus,
          "l2": "no explicit flush: one step streams > 1 GB of activations (Unet_3D enc1 output alone is 336 MB at batch 16) "
-               "through the 126 MB L2; inputs rotate over 2 buffers"}
+               "through the 50 MB L2; inputs rotate over 2 buffers"}
     if extra:
         c.update(extra)
     return c
@@ -213,7 +217,12 @@ def run_reference(args):
     value = sample * steps / dt
     line = {"impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": steps,
             "warmup": warmup, "ms_per_step": 1e3 * dt / steps, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config(args, args.gpus),
+            "vs_baseline": None, "dtype": "f32", "data": "synthetic",
+            "config": config(args, args.gpus, {"workload": "GenRe full_model inference (depth + sph-inpaint + voxel refine), batch=%d "
+                                                           "(BASELINE configs[2]), frozen models/genre_full_model.py Net.forward on "
+                                                           "the host CPU" % args.batch,
+                                               "weights": "random init (PyTorch defaults; min/max-depth head biased to the dataset "
+                                                          "depth range so cam_bp hits the grid)"}),
             "cpu_baseline": {"value": value, "unit": UNIT, "cores": cores, "kind": "port",
                              "sample": "%d of the %d shapes of a batch per step; frozen Net.forward on CPU: toolbox ops = oracle/genre_oracle.c "
                                        "over a thread pool (the reference's ops are CUDA-only), 2D/3D networks = the reference's "
@@ -228,7 +237,7 @@ def run_reference(args):
 # helpers of our arm
 # ----------------------------------------------------------------------------------------------------
 def measured_peaks():
-    hbm, tens, src = 6650.0, 1500.0, "fallback (B200_PROFILING.md)"
+    hbm, tens, src = 3350.0, 989.0, "H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W)"
     pk = os.path.join(REPO, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         try:
@@ -290,14 +299,47 @@ def graph_of(torch, fn, warm=2):
 # ----------------------------------------------------------------------------------------------------
 # our arm
 # ----------------------------------------------------------------------------------------------------
+def build_3d_path(torch, dev):
+    """(glue, refiner, forward): forward(depth [B,1,256,256]) -> pred_voxel [B,1,128,128,128]"""
+    import networks.networks as nets
+    from genre_shapehd_b200.fused import GenRe3DGlue
+    torch.manual_seed(0)
+    glue = GenRe3DGlue().to(dev)
+    refine = nets.Unet_3D().to(dev).eval()
+
+    def forward(depth):
+        with torch.no_grad():
+            proj, sph_in = glue.project_and_render(depth, FL, CAM_DIST)
+            return refine(glue.refine_input(proj, sph_in))
+    return glue, refine, forward
+
+
+def depth_inputs(torch, B, dev, seed):
+    """seed 0: synth.bench_depth_batch(B); seed 1: the same maps mirrored left-right"""
+    from genre_shapehd_b200.synth import bench_depth_batch
+    d = torch.from_numpy(bench_depth_batch(B))
+    if seed % 2:
+        d = d.flip(-1).contiguous()
+    return d.to(dev) if dev is not None else d
+
+
+def dump_outputs(out_dir, pred):
+    """shape 0 whole, plus 4 Mi values of the whole batch at positions drawn by a fixed seed"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    v = pred.detach().float().cpu().numpy()
+    np.save(os.path.join(out_dir, "pred_voxel_0.npy"), v[0, 0])
+    flat = v.reshape(-1)
+    idx = np.random.RandomState(0).randint(0, flat.size, size=min(flat.size, 1 << 22))
+    np.save(os.path.join(out_dir, "pred_voxel_sample.npy"), flat[idx])
+
+
 def run_b200(args):
     import torch
 
-    from genre_shapehd_b200 import compat
-    compat.bootstrap()                       # frozen callers from baseline/_ref; toolbox / networks.networks from this package
+    import genre_shapehd_b200
+    genre_shapehd_b200.install()
     from genre_shapehd_b200 import _lib, dist_util, ops_conv
-    from genre_shapehd_b200.synth_genre import genre_inputs, genre_opt, init_genre_net_for_bench
-    import models.genre_full_model as gfm
 
     skip = set(x for x in args.skip.split(",") if x)
     world, rank, local = dist_util.env_world()
@@ -310,20 +352,7 @@ def run_b200(args):
     _lib.load()
 
     B, K, Wm = args.batch, args.steps, max(args.warmup, 3)
-    torch.manual_seed(0)
-    net = gfm.Net(genre_opt(), gfm.Model)
-    init_genre_net_for_bench(net)
-    net = net.to(dev).eval()
-    # the two 2D U-ResNet18 nets are the reference's own code (outside the hot path, SURVEY 8f-2); their one cheap win here is the
-    # memory format of the module instances (a deployment choice of the caller, no file of the reference is touched)
-    nets2d = os.environ.get("GENRE_B200_BENCH_2D_FORMAT", "channels_last")
-    if nets2d == "channels_last":
-        net.depth_and_inpaint.net1.to(memory_format=torch.channels_last)
-        net.depth_and_inpaint.net2.to(memory_format=torch.channels_last)
-    folded = 0
-    if os.environ.get("GENRE_B200_BENCH_2D_FOLD_BN", "1") != "0":     # eval-mode BatchNorm2d folded into the preceding (transposed) conv
-        folded = compat.fold_batchnorm2d_eval(net.depth_and_inpaint.net1) + compat.fold_batchnorm2d_eval(net.depth_and_inpaint.net2)
-    nets2d += ", %d eval BatchNorm2d folded into their convolutions" % folded
+    glue, refine, forward = build_3d_path(torch, dev)
     conv_mode = ops_conv.describe_mode()
 
     def barrier():
@@ -334,13 +363,9 @@ def run_b200(args):
 
     # ---- leg 1: inputs resident in HBM --------------------------------------------------------------
     n_in = 2
-    inputs = [genre_inputs(B, dev, seed=10 * rank + i) for i in range(n_in)]
+    inputs = [depth_inputs(torch, B, dev, seed=i) for i in range(n_in)]
 
-    def forward(x):
-        with torch.no_grad():
-            return net(x)["pred_voxel"]
-
-    # launches of THIS library per step (eager, counted by the binding); cuDNN / aten kernels of the 2D nets are not ours
+    # launches of this library per step (eager, counted by the binding)
     forward(inputs[0])
     torch.cuda.synchronize()
     n0 = _lib.launch_count
@@ -354,7 +379,7 @@ def run_b200(args):
         try:
             for x in inputs:
                 replays.append(graph_of(torch, lambda x=x: forward(x)))
-        except Exception as e:       # e.g. an op of the frozen 2D nets that cannot be captured: launch from Python instead
+        except Exception as e:       # an op that cannot be captured: launch from Python instead
             graph_note = "capture failed: " + repr(e)[:160]
             use_graph, replays = False, []
             torch.cuda.synchronize()
@@ -362,8 +387,8 @@ def run_b200(args):
     def step(i):
         if use_graph:
             replays[i % n_in][0]()
-        else:
-            forward(inputs[i % n_in])
+            return replays[i % n_in][1]
+        return forward(inputs[i % n_in])
 
     for i in range(Wm):
         step(i)
@@ -373,21 +398,17 @@ def run_b200(args):
         time.sleep(0.25)
     barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    prof_range = os.environ.get("GENRE_B200_BENCH_PROFILE_RANGE") == "1"    # `ncu --profile-from-start off`: the timed steps only
-    if prof_range:
-        torch.cuda.synchronize()
-        torch.cuda.profiler.start()
     t_wall0 = time.time()
     e0.record()
+    last = None
     for i in range(K):
-        step(i)
+        last = step(i)
     e1.record()
     barrier()
     t_wall1 = time.time()
-    if prof_range:
-        torch.cuda.synchronize()
-        torch.cuda.profiler.stop()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last)
     t_load1 = t_wall1
     try:    # keep the same step running (untimed) so that nvidia-smi's 100 ms samples describe this kernel mix under load
         n_load = min(2000, max(K, int(0.6 / max(ms_total / K * 1e-3, 1e-6))))
@@ -400,12 +421,13 @@ def run_b200(args):
     clocks = sampler.stop(t_wall0, t_load1) if rank == 0 else None
     if clocks is not None:
         clocks["window"] = "timed region + %.2f s untimed replay of the same step" % (t_load1 - t_wall1)
+        clocks["gpu"] = torch.cuda.get_device_name(dev)
     value = world * B * K / (ms_total * 1e-3)
 
     # ---- leg 2: end to end with host buffers, double-buffered over three streams ----------------------
     e2e = None
     if "e2e" not in skip:
-        e2e = e2e_leg(torch, net, dev, B, K, rank, world, barrier, max_over_ranks, use_graph, genre_inputs)
+        e2e = e2e_leg(torch, forward, dev, B, K, rank, world, barrier, max_over_ranks, use_graph)
         if e2e is not None and numa is not None:
             e2e["host_affinity"] = numa
 
@@ -413,74 +435,56 @@ def run_b200(args):
     roofline = None
     if rank == 0 and "roofline" not in skip:
         try:
-            roofline = roofline_leg(torch, net, dev, B, inputs[0])
+            roofline = roofline_leg(torch, glue, refine, dev, B, inputs[0])
         except Exception as e:
             roofline = {"error": repr(e)[:300]}
 
     # ---- leg 4: CPU baseline (rank 0, N = 1): the reference arm on a bounded sample, own process --------
     cpu = None
     if rank == 0 and world == 1 and "cpu" not in skip:
-        cpu = cpu_baseline_leg(args)
+        from genre_shapehd_b200 import compat
+        cpu = cpu_baseline_leg(args) if compat.find_reference() else {"skipped": "no GenRe-ShapeHD checkout ($GENRE_REF)"}
 
-    # ---- secondary: configs[1] and the fast conv mode (rank 0, N = 1) ----------------------------------
+    # ---- secondary: cam_bp at batch 32 and the fast conv mode (rank 0, N = 1) ---------------------------
     secondary = None
     if rank == 0 and world == 1 and "secondary" not in skip:
         try:
-            secondary = secondary_leg(torch, net, dev, B, forward, inputs)
+            secondary = secondary_leg(torch, glue, dev, B, forward, inputs)
         except Exception as e:
             secondary = {"error": repr(e)[:300]}
-
-    # ---- secondary_ddp: configs[3] training steps under DDP (every N) ----------------------------------
-    ddp = None
-    if "ddp" not in skip:
-        try:
-            sys.path.insert(0, os.path.join(REPO, "profiles"))
-            import bench_train_ddp
-            ddp = {}
-            for which in ("shapehd", "wgan", "genre"):      # one at a time: a failing workload must not hide the others
-                try:
-                    ddp.update(bench_train_ddp.run(dev, world, rank, local, batch=8, steps=6, warmup=3, which=(which,)))
-                except Exception as e:
-                    ddp[which + "_error"] = repr(e)[:300]
-                torch.cuda.empty_cache()
-        except Exception as e:
-            ddp = {"error": repr(e)[:300]}
 
     if rank == 0:
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": Wm,
                 "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f32", "data": "synthetic",
-                "config": config(args, world, {"conv_mode": conv_mode, "nets2d": "reference uresnet.py modules on cuDNN (TF32 allowed, PyTorch default), %s" % nets2d}),
+                "config": config(args, world, {"conv_mode": conv_mode}),
                 "e2e": e2e, "gpu_launches": own_per_step * K,
                 "launch_mode": "cuda_graph" if use_graph else "python" + ("; " + graph_note if graph_note else ""),
                 "own_kernel_launches_per_step": own_per_step,
-                "roofline": roofline, "cpu_baseline": cpu, "clocks": clocks, "secondary": secondary, "secondary_ddp": ddp}
+                "roofline": roofline, "cpu_baseline": cpu, "clocks": clocks, "secondary": secondary}
         print(json.dumps(line), flush=True)
     dist_util.finalize()
 
 
-def e2e_leg(torch, net, dev, B, K, rank, world, barrier, max_over_ranks, use_graph, genre_inputs):
-    """pinned rgb+silhou -> H2D -> Net.forward -> D2H(pred_voxel), every step; two slots so that step i's result copy and step
-    i+1's input copy overlap compute.  Mirrors NetInterface.predict + Model.pack_output of the reference."""
-    import types
+def e2e_leg(torch, forward, dev, B, K, rank, world, barrier, max_over_ranks, use_graph):
+    """pinned depth -> H2D -> forward -> D2H(pred_voxel), every step; two slots so that step i's result copy and step
+    i+1's input copy overlap compute."""
     Ke = max(4, min(K, 20))
     s_in, s_cmp, s_out = torch.cuda.Stream(), torch.cuda.Stream(), torch.cuda.Stream()
     slots = []
     for s in range(2):
-        host = genre_inputs(B, None, seed=100 + 10 * rank + s, pin=True)
-        d_in = types.SimpleNamespace(rgb=torch.empty((B, 3, H, W), device=dev), silhou=torch.empty((B, 1, H, W), device=dev))
+        host = depth_inputs(torch, B, None, seed=s).pin_memory()
+        d_in = torch.empty((B, 1, H, W), device=dev)
         slots.append({"host": host, "dev": d_in, "pin_out": torch.empty((B, 1, RES, RES, RES), dtype=torch.float32).pin_memory(),
                       "in_done": torch.cuda.Event(), "cmp_done": torch.cuda.Event(), "out_done": torch.cuda.Event(), "run": None,
                       "out": None})
 
     def fwd(slot):
-        with torch.no_grad():
-            return net(slot["dev"])["pred_voxel"]
+        return forward(slot["dev"])
 
     torch.cuda.synchronize()
     for slot in slots:
-        slot["dev"].rgb.copy_(slot["host"].rgb)
-        slot["dev"].silhou.copy_(slot["host"].silhou)
+        slot["dev"].copy_(slot["host"])
         if use_graph:
             try:
                 replay, out = graph_of(torch, lambda slot=slot: fwd(slot))
@@ -497,8 +501,7 @@ def e2e_leg(torch, net, dev, B, K, rank, world, barrier, max_over_ranks, use_gra
         slot = slots[i % 2]
         with torch.cuda.stream(s_in):
             s_in.wait_event(slot["cmp_done"])                 # the previous forward of this slot has consumed its inputs
-            slot["dev"].rgb.copy_(slot["host"].rgb, non_blocking=True)
-            slot["dev"].silhou.copy_(slot["host"].silhou, non_blocking=True)
+            slot["dev"].copy_(slot["host"], non_blocking=True)
             slot["in_done"].record(s_in)
         with torch.cuda.stream(s_cmp):
             s_cmp.wait_event(slot["in_done"])
@@ -530,35 +533,29 @@ def e2e_leg(torch, net, dev, B, K, rank, world, barrier, max_over_ranks, use_gra
     e1.record(cur)
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
-    bytes_in, bytes_out = B * 4 * H * W * 4, B * RES ** 3 * 4
+    bytes_in, bytes_out = B * H * W * 4, B * RES ** 3 * 4
     return {"value": world * B * Ke / (ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": bytes_in, "d2h_bytes_per_step": bytes_out,
             "steps": Ke, "ms_per_step": ms / Ke, "result_checksum": float(slots[0]["pin_out"].double().abs().sum()),
             "d2h_GBps_per_rank_if_serial": bytes_out / (ms / Ke * 1e-3) / 1e9,
-            "pipeline": "2 slots x 3 streams (H2D | Net.forward%s | D2H)" % (" as a CUDA graph" if slots[0]["run"] is not None else "")}
+            "pipeline": "2 slots x 3 streams (H2D | forward%s | D2H)" % (" as a CUDA graph" if slots[0]["run"] is not None else "")}
 
 
-def roofline_leg(torch, net, dev, B, x):
-    """Each hot-path op of the step, alone, at the step's batch and ON THE STEP'S OWN TENSORS (one real forward is run first and
-    its intermediates captured): CUDA events around a CUDA-graph replay of the public call (so that launch gaps are not billed
-    to the kernels), algorithmic bytes / flops from SURVEY 8(d)."""
+def roofline_leg(torch, glue, refine, dev, B, depth):
+    """Each hot-path op of the step, alone, at the step's batch and on the step's own tensors: CUDA events around a CUDA-graph
+    replay of the public call (so that launch gaps are not billed to the kernels), algorithmic bytes / flops from SURVEY 8(d)."""
     from genre_shapehd_b200 import _lib, ops_conv
     from toolbox.cam_bp.cam_bp.functions import SphericalBackProjection
     from toolbox.spherical_proj import gen_sph_grid
     hbm, tens, src = measured_peaks()
-    layer = net.proj_depth
-    cap = {}
-    h1 = net.depth_and_inpaint.proj_depth.register_forward_pre_hook(lambda m, a: cap.__setitem__("depth", a[0].detach().clone()))
-    h2 = net.depth_and_inpaint.render_spherical.register_forward_pre_hook(lambda m, a: cap.__setitem__("vox", a[0].detach().clone()))
-    h3 = net.refine_net.register_forward_pre_hook(lambda m, a: cap.__setitem__("refine_in", a[0].detach().clone()))
+    layer = glue.proj_depth
     with torch.no_grad():
-        out = net(x)
-    for h in (h1, h2, h3):
-        h.remove()
-    depth, vox, refine_in = cap["depth"], cap["vox"], cap["refine_in"]     # depth: the permuted + flipped view the caller passes
+        proj, sph_in = glue.project_and_render(depth, FL, CAM_DIST)
+        vox = torch.clamp(proj * glue.scale, glue.lo, glue.hi)
+        refine_in = glue.refine_input(proj, sph_in)
     reps = 30
     with torch.no_grad():
         # cam_bp whole op (memset node + project + splat)
-        run, proj = graph_of(torch, lambda: layer(depth))
+        run, _ = graph_of(torch, lambda: layer(depth, FL, CAM_DIST))
         ms_cam = time_cuda(torch, run, reps)
         cam_bytes = B * (4 * H * W + 4 * RES ** 3)
         # splat kernel alone (the HBM-bound kernel of the op)
@@ -572,39 +569,24 @@ def roofline_leg(torch, net, dev, B, x):
         ms_splat = time_cuda(torch, lambda: _lib.call("genre_b200_voxelize_stage_splat", B, H * W, RES, tdf.data_ptr(), None, 1.0,
                                                       -1.0 / 16777216.0, 0.0, ws.data_ptr(), nbytes, st), reps)
         # render_spherical on the volume the caller hands it: clamp(proj * 50, 1e-5, 1 - 1e-5) (depth_pred_with_sph_inpaint.py:124)
-        rend = net.depth_and_inpaint.render_spherical
+        rend = glue.render
         run, sph = graph_of(torch, lambda: rend(vox))
         ms_rend = time_cuda(torch, run, reps)
         rend_bytes = B * (4 * RES ** 3 + 4 * 128 * 128)
-        # spherical back-projection (tdf + cnt out) of the inpainted map (genre_full_model.py:134-143)
+        # spherical back-projection (tdf + cnt out) of the padded map (genre_full_model.py:134-143)
         grid = gen_sph_grid().to(dev).expand(B, -1, -1, -1, -1)
-        sph_in = (1 - out["pred_sph_full"][:, :, 16:144, 16:144]).contiguous()
-        run, _ = graph_of(torch, lambda: SphericalBackProjection.apply(sph_in, grid, RES))
+        sph_crop = (1 - sph_in[:, :, 16:144, 16:144]).contiguous()
+        run, _ = graph_of(torch, lambda: SphericalBackProjection.apply(sph_crop, grid, RES))
         ms_sbp = time_cuda(torch, run, reps)
         sbp_bytes = B * (4 * 128 * 128 + 8 * RES ** 3)
         # the refiner on its real input
-        run, _ = graph_of(torch, lambda: net.refine_net(refine_in))
+        run, _ = graph_of(torch, lambda: refine(refine_in))
         ms_unet = time_cuda(torch, run, 10)
     tf_useful = UNET3D_GFLOP * 1e9 * B / (ms_unet * 1e-3) / 1e12
-    ncu = None
-    f = os.path.join(REPO, "profiles", "r02_tensor_pipe.json")
-    if os.path.exists(f):
-        try:
-            ncu = json.load(open(f))
-        except Exception:
-            pass
-    traffic = None
-    f = os.path.join(REPO, "profiles", "splat_traffic.json")
-    if os.path.exists(f):
-        try:
-            traffic = json.load(open(f))
-        except Exception:
-            pass
     gbs = lambda nbytes, ms: nbytes / (ms * 1e-3) / 1e9
     occ_frac = float((vox > 1e-5).float().mean())
     return {"bound": "hbm", "kernel": "cam_bp whole op: cam_project_kernel + vox_splat_kernel (+ counter memset), batch %d, the step's own depth maps" % B,
             "achieved": gbs(cam_bytes, ms_cam), "peak": hbm, "unit": "GB/s", "frac": gbs(cam_bytes, ms_cam) / hbm,
-            "traffic": (traffic or {}).get("dram_bytes_per_launch_b16"), "traffic_source": "ncu --set full capture, profiles/splat_traffic.json (static: needs a profiler)",
             "peak_source": src, "algorithmic_bytes_per_launch": cam_bytes, "op_us": ms_cam * 1e3,
             "clauses": {
                 "vox_splat_kernel": {"bound": "hbm", "us": ms_splat * 1e3, "achieved": gbs(cam_bytes, ms_splat), "frac": gbs(cam_bytes, ms_splat) / hbm,
@@ -617,8 +599,7 @@ def roofline_leg(torch, net, dev, B, x):
                 "unet3d_refiner": {"bound": "tensor", "ms": ms_unet, "achieved": tf_useful, "peak": tens, "unit": "TFLOP/s (useful: 78.0 GFLOP/shape)",
                                    "frac": tf_useful / tens, "conv_mode": ops_conv.describe_mode(),
                                    "note": "useful flops of the reference layers; the hi/lo-split mode issues 2 MMAs per useful one and merged-parity "
-                                           "layers carry structural zeros, so this understates tensor-pipe activity",
-                                   "ncu_tensor_pipe": ncu}}}
+                                           "layers carry structural zeros, so this understates tensor-pipe activity"}}}
 
 
 def cpu_baseline_leg(args):
@@ -639,7 +620,7 @@ def cpu_baseline_leg(args):
         return {"error": repr(e)[:300]}
 
 
-def secondary_leg(torch, net, dev, B, forward, inputs):
+def secondary_leg(torch, glue, dev, B, forward, inputs):
     from genre_shapehd_b200 import ops_conv
     from genre_shapehd_b200.synth import bench_depth_batch
     hbm, _, _ = measured_peaks()
@@ -647,31 +628,20 @@ def secondary_leg(torch, net, dev, B, forward, inputs):
     with torch.no_grad():
         # BASELINE configs[1]: cam_bp 256x256 -> 128^3, batch 32
         depth = torch.from_numpy(bench_depth_batch(32)).to(dev)
-        run, _ = graph_of(torch, lambda: net.proj_depth(depth))
+        run, _ = graph_of(torch, lambda: glue.proj_depth(depth, FL, CAM_DIST))
         ms = time_cuda(torch, run, 50)
         nbytes = 32 * (4 * H * W + 4 * RES ** 3)
         out["cam_bp_b32"] = {"workload": "BASELINE configs[1]: cam_bp 256x256 depth -> 128^3, batch 32", "us": ms * 1e3,
                              "shapes_per_s": 32 / ms * 1e3, "whole_op_GBps": nbytes / (ms * 1e-3) / 1e9,
                              "whole_op_frac": nbytes / (ms * 1e-3) / 1e9 / hbm}
-        # the same GenRe step with single-pass fp16 operands in the 3D convolutions (10-bit mantissa, tested at 4e-3 per layer)
+        # the same step with single-pass fp16 operands in the 3D convolutions (10-bit mantissa, tested at 4e-3 per layer)
         with ops_conv.precision("f16"):
             ms_fast = time_cuda(torch, lambda: forward(inputs[0]), 5)
-        out["genre_fast_conv_mode"] = {"conv_mode": "f16 single pass (10-bit operand mantissa; NOT the 1e-4 parity mode)",
-                                       "ms_per_step_python_launch": ms_fast, "shapes_per_s": B / ms_fast * 1e3}
+        out["fast_conv_mode"] = {"conv_mode": "f16 single pass (10-bit operand mantissa; NOT the 1e-4 parity mode)",
+                                 "ms_per_step_python_launch": ms_fast, "shapes_per_s": B / ms_fast * 1e3}
         ms_exact = time_cuda(torch, lambda: forward(inputs[0]), 5)
-        out["genre_default_mode_python_launch"] = {"conv_mode": ops_conv.describe_mode(), "ms_per_step": ms_exact,
-                                                   "shapes_per_s": B / ms_exact * 1e3}
-        # the 3D hot path alone (2D nets excluded), fused glue (genre_shapehd_b200/fused.py)
-        from genre_shapehd_b200.fused import GenRe3DGlue
-        glue = GenRe3DGlue().to(dev)
-        d16 = depth[:B]
-        sph_full = torch.rand(B, 1, 160, 160, device=dev) * 0.4 + 0.3
-
-        def path3d():
-            pd, sph = glue.project_and_render(d16)
-            return net.refine_net(glue.refine_input(pd, sph_full))
-        ms3 = time_cuda(torch, path3d, 5)
-        out["genre_3d_path_fused_glue"] = {"ms_per_batch": ms3, "shapes_per_s": B / ms3 * 1e3, "conv_mode": ops_conv.describe_mode()}
+        out["default_mode_python_launch"] = {"conv_mode": ops_conv.describe_mode(), "ms_per_step": ms_exact,
+                                             "shapes_per_s": B / ms_exact * 1e3}
     return out
 
 

@@ -1,4 +1,4 @@
-"""genre_shapehd_b200 — B200-native (sm_100a) hot path of GenRe / ShapeHD.
+"""genre_shapehd_b200 — H100-native (sm_90a) hot path of GenRe / ShapeHD.
 
 The product is ``lib/libgenre_b200.so`` (hand-written CUDA behind a C ABI, ``include/genre_b200.h``)
 plus thin Python packages that mirror the reference's import surface so the reference's frozen

@@ -165,7 +165,7 @@ def stream_ptr(t):
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("genre_shapehd_b200 ops are CUDA-only (sm_100a); got a %s tensor. "
+            raise RuntimeError("genre_shapehd_b200 ops are CUDA-only (sm_90a); got a %s tensor. "
                                "There is no CPU fallback." % t.device)
 
 

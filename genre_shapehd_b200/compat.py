@@ -39,8 +39,8 @@ def _unavailable(what):
 
 
 def find_reference():
-    """the frozen callers: $GENRE_REF, else the staged copy <repo>/baseline/_ref (travels to the GPU box), else /root/reference"""
-    for root in (os.environ.get("GENRE_REF"), os.path.join(genre_shapehd_b200.REPO_ROOT, "baseline", "_ref"), "/root/reference"):
+    """the frozen callers: $GENRE_REF, else the copy __graft_entry__.build() staged into <repo>/baseline/_ref"""
+    for root in (os.environ.get("GENRE_REF"), os.path.join(genre_shapehd_b200.REPO_ROOT, "baseline", "_ref")):
         if root and os.path.isdir(os.path.join(root, "models")):
             return root
     return None
@@ -49,8 +49,8 @@ def find_reference():
 def bootstrap(reference_root=None, offline_resnet=True):
     root = reference_root or find_reference()
     if root is None or not os.path.isdir(os.path.join(root, "models")):
-        raise FileNotFoundError("no GenRe-ShapeHD checkout at %r (searched $GENRE_REF, <repo>/baseline/_ref, /root/reference; "
-                                "`python -c 'import __graft_entry__ as g; g.build()'` stages baseline/_ref)" % root)
+        raise FileNotFoundError("no GenRe-ShapeHD checkout at %r (searched $GENRE_REF and <repo>/baseline/_ref, which "
+                                "`python -c 'import __graft_entry__ as g; g.build()'` stages from a checkout)" % root)
     os.environ["GENRE_REF"] = root
     genre_shapehd_b200.install(root)
     stub_optional_modules(offline_resnet)

@@ -198,8 +198,8 @@ static int bn_shape(int64_t B, int64_t C, int64_t S, BnShape *sh) {
   sh->B = (int)B;
   sh->C = (int)C;
   sh->S = S;
-  // enough CTAs for ~4 waves of the 148 SMs, at least ~4096 float4 per CTA and batch row
-  long long want = (148ll * 4 + C - 1) / C;
+  // enough CTAs for ~4 waves of the SMs, at least ~4096 float4 per CTA and batch row
+  long long want = ((long long)sm_count() * 4 + C - 1) / C;
   const long long n4 = S / 4;
   long long cap = (n4 + 1023) / 1024;
   long long ns = want < cap ? want : cap;

@@ -8,7 +8,7 @@
 // Bit-exactness of the voxel index: every fp32 operation below is written with an explicit
 // round-to-nearest intrinsic in the order nvcc 12.9 emits for the reference source when it is built
 // with its own flags (default --fmad=true, IEEE div/sqrt; toolbox/cam_bp/setup.sh:25-29), read off
-// the sm_100a SASS of oracle/_ref/libref_cam_bp.so:
+// the SASS of oracle/_ref/libref_cam_bp.so:
 //     imind   = fma(size-1, -0.5, idx)                      (exact for image sizes < 2^23)
 //     norm^2  = fma(fl, fl, fma(imind_w, imind_w, imind_h*imind_h))
 //     cos     = fl / sqrt(norm^2)                           (IEEE sqrt, IEEE div)
@@ -444,7 +444,8 @@ extern "C" int genre_b200_surface_mask(const float *depth, int64_t N, int64_t C,
   const bool vec = (res % 4 == 0) && aligned16(cnt) && aligned16(mask);
   const long long work = vec ? nvox / 4 : nvox;
   unsigned gx = (unsigned)((work + 255) / 256);
-  if (gx > 148u * 16u) gx = 148u * 16u;
+  const unsigned gcap = (unsigned)sm_count() * 16u;   // grid-stride beyond ~16 CTAs per SM
+  if (gx > gcap) gx = gcap;
   dim3 grid(gx, (unsigned)(N * C));
   surface_mask_kernel<<<grid, 256, 0, as_stream(stream)>>>(depth, (int)C, (int)H, (int)W, sN, sC, sH, sW, fl, fN, fC,
                                                            camdist, dN, dC, cnt, mask, res, nvox, vec);

@@ -26,6 +26,18 @@ int check_launch(const char *what) {
   return (int)e;
 }
 const char *last_error() { return g_err; }
+
+int sm_count() {
+  static int cached[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  int &n = cached[dev & 63];
+  if (n <= 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+    cudaGetLastError();
+    n = 0;
+  }
+  return n > 0 ? n : 1;
+}
 }  // namespace gb
 
 extern "C" const char *genre_b200_last_error(void) { return gb::last_error(); }

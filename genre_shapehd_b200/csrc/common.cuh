@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libgenre_b200 (sm_100a only; no torch, no CPU fallback).
+// common.cuh — shared helpers for libgenre_b200 (sm_90a only; no torch, no CPU fallback).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,6 +14,9 @@ void set_error(const char *fmt, ...);
 int fail_arg(int code, const char *fmt, ...);
 int check_launch(const char *what);  // cudaPeekAtLastError -> 0 or the cudaError_t (message recorded)
 const char *last_error();
+
+// streaming multiprocessors of the current device (cached per device): grid sizes that aim at whole waves use it
+int sm_count();
 
 #define GB_REQUIRE(cond, code, ...)                      \
   do {                                                   \

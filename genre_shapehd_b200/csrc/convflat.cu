@@ -1,4 +1,4 @@
-// convflat.cu — the stride-2 3D convolutions of the SMALL volumes (<= 8^3 on the coarse side) as a tcgen05 implicit GEMM over a
+// convflat.cu — the stride-2 3D convolutions of the SMALL volumes (<= 8^3 on the coarse side) as a wgmma implicit GEMM over a
 // flattened, zero-separated volume.
 //
 // Reference layers: networks/networks.py:157-165 (Unet_3D.enc4, enc5 = Conv3d(k 4, s 2, p 1) -> BatchNorm3d -> LeakyReLU on
@@ -21,14 +21,17 @@
 // OP 1: fp16 operands; OP 2: the fp32-accurate fp16 hi/lo split of convt3d.cu (2 MMAs per K step, see ConvTCfg there).
 // CTA = MT M-tiles of 128 positions x NPAD output channels (x 2 accumulator halves in OP 2) of one class; warps 0-3:
 // warp 0 lane 0 issues the bulk copies, then all four run the epilogue (scale/shift = bias + folded BatchNorm, LeakyReLU,
-// NCDHW fp32 store); warp 4: TMEM allocation + MMA issue.  A stage = one K step (16 channels) x 8 taps.
+// NCDHW fp32 store) from a shared-memory image of the accumulators; warps 4-11: two consumer warpgroups, warpgroup wg
+// issuing the m64 wgmma of rows [64 wg, 64 wg + 64) of every M-tile with its accumulators in registers (MT * NACC <= 256).
+// A stage = one K step (16 channels) x 8 taps.
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
 namespace gb {
 
-constexpr int CF_THREADS = 160;
+constexpr int CF_THREADS = 384;
+constexpr int CF_CONSUMER_WARPS = 8;
 constexpr int CF_TAPS = 8;
 constexpr int CF_MAX_STAGES = 6;
 
@@ -49,21 +52,8 @@ struct ConvFlatParams {
   float slope;
   float *out;           // NCDHW fp32 [B][Cout][Do][Ho][Wo]
   int Cout;
-  int stages, a_cg_stride, stage_bytes;   // shared-memory plan (host)
+  int stages, a_cg_stride, stage_bytes, ring_bytes;   // shared-memory plan (host)
 };
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 template <int NPAD, int MT, int OP>
 __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatParams p) {
@@ -72,15 +62,13 @@ __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatP
   constexpr int NACC = PARTS * NPAD;
   constexpr int B_TAP_BYTES = 2 * (NACC / 8) * 128;
   constexpr int B_BYTES = CF_TAPS * B_TAP_BYTES;
-  constexpr int TMEM_COLS = MT * NACC <= 32 ? 32 : MT * NACC <= 64 ? 64 : MT * NACC <= 128 ? 128 : MT * NACC <= 256 ? 256 : 512;
-  constexpr float LO_SCALE = 1.0f / 2048.0f;
-  static_assert(MT * NACC <= 512 && NACC <= 256 && NPAD % 16 == 0, "accumulator shape");
+  constexpr int ACC_LD = NPAD + 4;   // accumulator image [MT][128 rows][ACC_LD] fp32, over the drained ring
+  static_assert(MT * NACC <= 256 && NACC <= 256 && NPAD % 16 == 0, "accumulator shape");
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *stages = smem;
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)p.stages * p.stage_bytes);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)p.ring_bytes);
   uint64_t *empty = full + CF_MAX_STAGES;
-  uint64_t *accum_full = empty + CF_MAX_STAGES;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(accum_full + 1);
+  float *acc_img = reinterpret_cast<float *>(smem);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long q0 = (long long)blockIdx.x * (128 * MT);   // first position of this CTA
@@ -91,20 +79,11 @@ __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatP
   if (tid == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], CF_CONSUMER_WARPS);
     }
-    mbar_init(accum_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
     if (tid == 0) {
@@ -126,9 +105,49 @@ __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatP
         }
       }
     }
+  } else {
+    // ===================== consumers ============================================================================
+    const int wg = (warp - 4) >> 2;
+    float acc[MT][NACC / 2];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int j = 0; j < NACC / 2; ++j) acc[mt][j] = 0.0f;
+    for (int ks = 0; ks < p.ksteps; ++ks) {
+      const int s = ks % p.stages, use = ks / p.stages;
+      mbar_wait(&full[s], use & 1);
+      wgmma_fence();
+      const uint32_t sa = smem_u32(stages + (size_t)s * p.stage_bytes);
+      const uint32_t sb = sa + a_bytes;
+      const int grp = p.cgs_per_group ? ((ks * 2) / p.cgs_per_group) & 7 : cls;
+#pragma unroll
+      for (int t = 0; t < CF_TAPS; ++t) {
+        const uint64_t bdesc = gmma_desc(sb + t * B_TAP_BYTES, (NACC / 8) * 128, 128);
+        const int sh = p.shift[grp][t];
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const uint32_t a0 = sa + (uint32_t)((p.halo + sh + 128 * mt + 64 * wg) * 16);
+          const uint64_t adesc = gmma_desc(a0, p.a_cg_stride, 128);
+          wgmma_f16<NACC>(acc[mt], adesc, bdesc);
+          if constexpr (X2) {
+            const uint64_t adesc_lo = gmma_desc(a0 + 2 * p.a_cg_stride, p.a_cg_stride, 128);
+            wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc_lo, bdesc);
+          }
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    // every stage has been consumed: the ring becomes the accumulator image
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // ... by BOTH consumer warpgroups: the other one may still be reading it
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) store_acc_tile<NPAD, X2>(acc[mt], acc_img + ((size_t)mt * 128 + 64 * wg) * ACC_LD, ACC_LD);
+  }
+  __syncthreads();
+  if (warp < 4) {
     // ===================== epilogue ===========================================================================
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
     const int Wp = p.W + 1, Hp = p.H + 1, Dp = p.D + 1;
     const int Do = p.up ? 2 * p.D : p.D, Ho = p.up ? 2 * p.H : p.H, Wo = p.up ? 2 * p.W : p.W;
     const int pz = p.up ? (cls >> 2) & 1 : 0, py = p.up ? (cls >> 1) & 1 : 0, px = p.up ? cls & 1 : 0;
@@ -144,18 +163,12 @@ __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatP
       const bool valid = q < p.M && x < p.W && y < p.H && z < p.D;
       const int oz = p.up ? 2 * z + pz : z, oy = p.up ? 2 * y + py : y, ox = p.up ? 2 * x + px : x;
       float *orow = p.out + (size_t)b * p.Cout * ovol + ((size_t)oz * Ho + oy) * Wo + ox;
-      const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(mt * NACC);
+      const float *arow = acc_img + ((size_t)mt * 128 + warp * 32 + lane) * ACC_LD;
 #pragma unroll 1
       for (int nb = 0; nb < NPAD / 16; ++nb) {
-        float v[16];
-        tmem_ld16(trow + (uint32_t)(nb * 16), v);     // warp-collective: every lane takes part, valid or not
-        if constexpr (X2) {
-          float l[16];
-          tmem_ld16(trow + (uint32_t)(NPAD + nb * 16), l);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaf(l[i], LO_SCALE, v[i]);
-        }
         if (valid) {
+          float v[16];
+          ld_row<16>(arow + nb * 16, v);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             const int n = ntile * NPAD + nb * 16 + i;
@@ -167,41 +180,6 @@ __global__ void __launch_bounds__(CF_THREADS, 1) convflat_kernel(const ConvFlatP
         }
       }
     }
-    tc_fence_before();
-  } else if (lane == 0) {
-    // ===================== MMA issuer ===========================================================================
-    constexpr uint32_t idesc = umma_idesc_f16(128, NACC);
-    constexpr uint32_t idesc_lo = umma_idesc_f16(128, NPAD);
-    for (int ks = 0; ks < p.ksteps; ++ks) {
-      const int s = ks % p.stages, use = ks / p.stages;
-      mbar_wait(&full[s], use & 1);
-      tc_fence_after();
-      const uint32_t sa = smem_u32(stages + (size_t)s * p.stage_bytes);
-      const uint32_t sb = sa + a_bytes;
-      const int grp = p.cgs_per_group ? ((ks * 2) / p.cgs_per_group) & 7 : cls;
-#pragma unroll
-      for (int t = 0; t < CF_TAPS; ++t) {
-        const uint64_t bdesc = umma_desc(sb + t * B_TAP_BYTES, (NACC / 8) * 128, 128);
-        const int sh = p.shift[grp][t];
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt) {
-          const uint32_t a0 = sa + (uint32_t)((p.halo + sh + 128 * mt) * 16);
-          const uint64_t adesc = umma_desc(a0, p.a_cg_stride, 128);
-          umma_f16(tmem_base + mt * NACC, adesc, bdesc, idesc, (ks | t) != 0);
-          if constexpr (X2) {
-            const uint64_t adesc_lo = umma_desc(a0 + 2 * p.a_cg_stride, p.a_cg_stride, 128);
-            umma_f16(tmem_base + mt * NACC + NPAD, adesc_lo, bdesc, idesc_lo, true);
-          }
-        }
-      }
-      umma_commit(&empty[s]);
-    }
-    umma_commit(accum_full);
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
   }
 }
 
@@ -254,29 +232,35 @@ flat_pack_kernel(const float *__restrict__ src, int C, int B, int D, int H, int 
 template <int NPAD, int MT, int OP>
 static int launch_convflat(ConvFlatParams &p, int classes, cudaStream_t st) {
   constexpr int PARTS = OP == 2 ? 2 : 1, NACC = PARTS * NPAD;
-  constexpr int B_BYTES = CF_TAPS * 2 * (NACC / 8) * 128;
-  const int a_cg_bytes = (128 * MT + 2 * p.halo) * 16;
-  p.a_cg_stride = (a_cg_bytes + 127) / 128 * 128;
-  p.stage_bytes = PARTS * 2 * p.a_cg_stride + B_BYTES;
-  int stages = (224 * 1024) / p.stage_bytes;
-  if (stages > CF_MAX_STAGES) stages = CF_MAX_STAGES;
-  if (stages > p.ksteps) stages = p.ksteps < 1 ? 1 : p.ksteps;
-  GB_REQUIRE(stages >= 2 || p.ksteps == 1, GENRE_B200_EINVAL, "convflat: a stage of %d bytes does not fit twice", p.stage_bytes);
-  p.stages = stages;
-  const size_t smem = (size_t)stages * p.stage_bytes + 256;
-  auto kern = convflat_kernel<NPAD, MT, OP>;
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!configured[dev & 63]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return check_launch("convflat: cudaFuncSetAttribute");
-    configured[dev & 63] = true;
+  if constexpr (MT > 1 && MT * NACC > 256) {   // register budget of the consumers
+    return launch_convflat<NPAD, MT / 2, OP>(p, classes, st);
+  } else {
+    const int acc_bytes = MT * 128 * (NPAD + 4) * 4;
+    constexpr int B_BYTES = CF_TAPS * 2 * (NACC / 8) * 128;
+    const int a_cg_bytes = (128 * MT + 2 * p.halo) * 16;
+    p.a_cg_stride = (a_cg_bytes + 127) / 128 * 128;
+    p.stage_bytes = PARTS * 2 * p.a_cg_stride + B_BYTES;
+    int stages = (224 * 1024) / p.stage_bytes;
+    if (stages > CF_MAX_STAGES) stages = CF_MAX_STAGES;
+    if (stages > p.ksteps) stages = p.ksteps < 1 ? 1 : p.ksteps;
+    GB_REQUIRE(stages >= 2 || p.ksteps == 1, GENRE_B200_EINVAL, "convflat: a stage of %d bytes does not fit twice", p.stage_bytes);
+    p.stages = stages;
+    p.ring_bytes = stages * p.stage_bytes > acc_bytes ? stages * p.stage_bytes : acc_bytes;
+    const size_t smem = (size_t)p.ring_bytes + 256;
+    auto kern = convflat_kernel<NPAD, MT, OP>;
+    static bool configured[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (!configured[dev & 63]) {
+      if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+        return check_launch("convflat: cudaFuncSetAttribute");
+      configured[dev & 63] = true;
+    }
+    const long long mtiles = (p.M + 128 * MT - 1) / (128 * MT);
+    dim3 grid((unsigned)mtiles, (unsigned)p.ntiles, (unsigned)classes);
+    kern<<<grid, CF_THREADS, smem, st>>>(p);
+    return check_launch("convflat kernel");
   }
-  const long long mtiles = (p.M + 128 * MT - 1) / (128 * MT);
-  dim3 grid((unsigned)mtiles, (unsigned)p.ntiles, (unsigned)classes);
-  kern<<<grid, CF_THREADS, smem, st>>>(p);
-  return check_launch("convflat kernel");
 }
 
 }  // namespace gb

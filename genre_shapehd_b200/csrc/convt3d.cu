@@ -1,4 +1,4 @@
-// convt3d.cu — stride-2 ConvTranspose3d forward as a tcgen05 (5th-gen tensor core) implicit GEMM, TF32 in / FP32 out.
+// convt3d.cu — stride-2 ConvTranspose3d forward as a wgmma (Hopper warpgroup tensor core) implicit GEMM, TF32 in / FP32 out.
 //
 // Reference layers: networks/networks.py:162-167 (Unet_3D.dec2..dec6 = Deconv3d_skip: cat(x, skip) ->
 // ConvTranspose3d(k, s=2, p) [-> BatchNorm3d -> LeakyReLU]), :253-256,:40-57 (VoxelDecoder / VoxelGenerator
@@ -8,7 +8,7 @@
 // the taps k = k0 + 2 t, t < T = K/2, at input positions i = j + base - t: a stride-1 T^3-tap convolution.
 //     GEMM per class:  M = B * D*H*W positions,  N = Cout (padded to NPAD),  K = T^3 * Cin
 // Activations are kept channel-BLOCKED: [B*D][C/4][H][W][4] (16 bytes per position and channel group), so
-//   * a shared-memory halo [cg][y][x][4] is exactly tcgen05's canonical K-major NO-SWIZZLE operand layout
+//   * a shared-memory halo [cg][y][x][4] is exactly wgmma's canonical K-major NO-SWIZZLE operand layout
 //     (core matrix = 8 consecutive x positions x 16 B; next y row = SBO; next channel group = LBO), and
 //   * the operand of ANY tap is the same halo at a different 16-byte-aligned start address: one halo load feeds
 //     T*T (y,x) taps and MT M-tiles, which is what keeps the kernel off the L2 bandwidth wall at N = 20.
@@ -16,10 +16,14 @@
 // materialised).  Weights are pre-packed on the host into the exact shared-memory image of each (parity, z-tap,
 // K-chunk) stage and arrive with ONE cp.async.bulk per stage.
 //
-// CTA = one (b, z, 16 y-rows, full W) output slab of one parity class: MT = W/8 M-tiles of 128 rows, accumulators
-// MT x NPAD fp32 columns in TMEM.  Warps 0-3: halo producers (cp.async 16 B, zero-fill = padding), then epilogue
-// (tcgen05.ld -> scale/shift/LeakyReLU -> blocked store).  Warp 4: TMEM allocation + single-thread MMA issue.
-// Pipeline: STAGES-deep ring of (halo chunk, weight chunk) with full/empty mbarriers; tcgen05.commit frees a slot.
+// CTA = one (b, z, 16 y-rows, 8*MT x-columns) output slab of one parity class: MT M-tiles of 128 rows.  Warps 0-3: halo
+// producers (cp.async 16 B, zero-fill = padding, or one thread issuing tensor copies), then epilogue (shared-memory
+// accumulator image -> scale/shift/LeakyReLU -> blocked store).  Warps 4-11: two consumer warpgroups, each issuing the
+// m64 wgmma of one half (8 y-rows) of every M-tile and holding its MT x NACC / 2 fp32 accumulators in registers, so
+// MT * NACC <= 256 (launch_convt_impl narrows the x tile until it fits).  After the last K step they store the
+// accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.
+// Pipeline: STAGES-deep ring of (halo chunk, weight chunk) with full/empty mbarriers; every consumer warp arrives on a slot's
+// empty barrier once its wgmma that read the slot have completed.
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (the entry point is resolved through the runtime: no -lcuda)
 #include <cstdlib>
 #include <cstring>
@@ -28,7 +32,9 @@
 
 namespace gb {
 
-constexpr int CT_THREADS = 160;       // 4 producer/epilogue warps + 1 MMA warp
+constexpr int CT_THREADS = 384;       // 4 producer/epilogue warps + 2 consumer warpgroups
+constexpr int CT_CONSUMER_WARPS = 8;
+constexpr int CT_ACC_COLS = 256;      // accumulator columns per CTA (MT * NACC): 128 fp32 registers per consumer thread
 constexpr int CT_PRODUCERS = 128;
 constexpr int CT_BY = 16;             // y rows per CTA (16 core-matrix groups of 8 x positions = M 128)
 constexpr int CT_KCG = 2;             // channel groups (of 4) per stage = one K=8 TF32 MMA per tap and M-tile
@@ -54,8 +60,8 @@ struct ConvTParams {
 // T: taps per dimension of a parity class (K/2: 2 for k=4, 4 for k=8); NPAD: padded Cout (32 or 64); MT = W/8.
 // X2: the fp32-accurate fp16 hi/lo operand split.  Activations arrive as [B*D][2 parts: hi, lo'][cg][H][W][8 fp16] with
 // lo' = (a - hi) * 2^11, weights as [W_hi | W_lo'] side by side along N (lo' = (w - hi) * 2^11).  Per K step and tap:
-//     A_hi  x [W_hi | W_lo']  ->  TMEM columns [0, 2*NPAD)         (one MMA, N = 2*NPAD)
-//     A_lo' x  W_hi           ->  TMEM columns [NPAD, 2*NPAD)      (one MMA, N = NPAD)
+//     A_hi  x [W_hi | W_lo']  ->  accumulator columns [0, 2*NPAD)      (one MMA, N = 2*NPAD)
+//     A_lo' x  W_hi           ->  accumulator columns [NPAD, 2*NPAD)   (one MMA, N = NPAD)
 // so the hi*hi products and the 2^11-scaled cross terms keep separate accumulators (the tensor core's fp32 accumulator
 // truncates: a step's error scales with the partial sum it joins, and the cross terms would otherwise ride on the big one),
 // and the epilogue returns acc_hi + 2^-11 * acc_cross.  2 MMAs per K step instead of the 3 of a K-expanded split.
@@ -86,18 +92,18 @@ struct ConvTCfg {
   static constexpr int ROWS = (T + YS - 1) / YS;
   static constexpr int B_BYTES = ROWS * T * B_TAP_BYTES;
   static constexpr int STAGE_BYTES = stage_bytes(YS);
-  static constexpr int TMEM_COLS = MT * NACC <= 32 ? 32 : MT * NACC <= 64 ? 64 : MT * NACC <= 128 ? 128 : MT * NACC <= 256 ? 256 : 512;
-  // Two CTAs per SM whenever TMEM (<= 256 columns each) and shared memory (<= ~112 KB each) allow: one CTA's prologue
-  // (TMEM alloc, pipeline fill) and epilogue (TMEM drain, stores) then overlap the other's MMA stream.
-  static constexpr int S_ALONE = (218 * 1024) / STAGE_BYTES > 6 ? 6 : (218 * 1024) / STAGE_BYTES;
-  static constexpr int S_PAIR = (112 * 1024) / STAGE_BYTES > 6 ? 6 : (112 * 1024) / STAGE_BYTES;
-  static constexpr bool PAIR = TMEM_COLS <= 256 && S_PAIR >= 2;
-  static constexpr int STAGES = PAIR ? S_PAIR : S_ALONE;
+  // one CTA per SM (the accumulators take half the register file): the whole 227 KB of shared memory serves the ring
+  static constexpr int STAGES = (218 * 1024) / STAGE_BYTES > 6 ? 6 : (218 * 1024) / STAGE_BYTES;
   static constexpr int POS = PY * PX;
   static constexpr int POS_PER_THREAD = (POS + CT_PRODUCERS - 1) / CT_PRODUCERS;
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 256;
+  // epilogue image of the accumulators, [128 rows][MT * NPAD (+ 4 pad) columns] fp32, over the drained ring
+  static constexpr int ACC_LD = MT * NPAD + 4;
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
+  static constexpr size_t SMEM = (size_t)RING_BYTES + 256;
   static_assert(STAGES >= 2, "stage too large");
-  static_assert(MT * NACC <= 512, "accumulators exceed TMEM");
+  static_assert(MT * NACC <= CT_ACC_COLS, "accumulators exceed the register budget");
+  static_assert(SMEM <= 227 * 1024, "shared memory");
   static_assert(NACC <= 256 && NACC % 16 == 0 && NPAD % 16 == 0 || !X2, "X2: MMA N must be a multiple of 16, at most 256");
 };
 
@@ -123,14 +129,12 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   constexpr bool F16 = OP != 0, X2 = OP == 2;
   using Cfg = ConvTCfg<T, NPAD, MT, X2, TMA>;
   constexpr int NACC = Cfg::NACC;
-  constexpr float LO_SCALE = 1.0f / 2048.0f;   // the cross-term accumulators hold 2^11 x their value
   constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *stages = smem;
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)Cfg::RING_BYTES);
   uint64_t *empty = full + Cfg::STAGES;
-  uint64_t *accum_full = empty + Cfg::STAGES;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(accum_full + 1);
+  float *acc_img = reinterpret_cast<float *>(smem);   // after the main loop: [128 rows][ACC_LD]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int par = blockIdx.y;  // parity class: bit 2 = z, bit 1 = y, bit 0 = x
@@ -177,22 +181,12 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], TMA ? 1 : CT_PRODUCERS + 1);  // cp.async path: 128 producer arrivals + the expect_tx arrival of the
                                                         // weight copy; TMA path: the one expect_tx arrival (halo + weight bytes)
-      mbar_init(&empty[s], ncl);              // one tcgen05.commit per CTA of the cluster
+      mbar_init(&empty[s], ncl * CT_CONSUMER_WARPS);   // every consumer warp of every CTA of the cluster
     }
-    mbar_init(accum_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {  // TMEM allocation is warp-wide
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
   if (ncl > 1) cluster_sync_all();   // every CTA's barriers exist before a peer's multicast can signal them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // weights of one stage: this CTA's slice, to every CTA of the cluster
   auto load_weights = [&](uint8_t *dst, const float *wsrc, uint32_t bytes, uint64_t *bar) {
     if (ncl == 1) {
@@ -304,27 +298,81 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     for (int e = 0; e < LAG; ++e) publish();  // drain: empty groups push the last real ones through
 
     }
-    // ===================== epilogue: TMEM -> registers -> act(acc*scale+shift) -> blocked global store =========
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
-    const int m = warp * 32 + lane;  // accumulator row = TMEM lane
+  } else {
+    // ===================== consumers: warpgroup wg issues the wgmma of rows [64 wg, 64 wg + 64) of every M-tile ===========
+    const int wg = (warp - 4) >> 2;
+    float acc[MT][NACC / 2];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int j = 0; j < NACC / 2; ++j) acc[mt][j] = 0.0f;
+    int it = 0;
+    for (int q = 0; q < n_q; ++q) {
+      int tz, kc, ys, bz, by, bx;
+      const bool valid = stage_of(q, tz, kc, ys, bz, by, bx);
+      if (!valid && ncl == 1) continue;
+      const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
+      ++it;
+      mbar_wait(&full[s], use & 1);
+      if (valid) {
+      wgmma_fence();
+      const uint32_t sa = smem_u32(stages + (size_t)s * Cfg::STAGE_BYTES);
+      const uint32_t sb = sa + Cfg::A_BYTES;
+      const int ty0 = ys * Cfg::ROWS;
+#pragma unroll
+      for (int r = 0; r < Cfg::ROWS; ++r) {
+        const int ty = ty0 + r;
+        if (ty >= T) break;
+#pragma unroll
+        for (int tx = 0; tx < T; ++tx) {
+          const uint64_t bdesc = gmma_desc(sb + (r * T + tx) * Cfg::B_TAP_BYTES, (NACC / 8) * 128, 128);
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt) {
+            // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x; this warpgroup's
+            // 64 rows are y = 8 wg .. 8 wg + 7
+            const uint32_t a0 = sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
+            const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+            if constexpr (F16) wgmma_f16<NACC>(acc[mt], adesc, bdesc);
+            else wgmma_tf32<NACC>(acc[mt], adesc, bdesc);
+            if constexpr (X2) {   // A_lo' x W_hi: the first NPAD columns of the same B tile
+              const uint64_t adesc_lo = gmma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+              wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc_lo, bdesc);
+            }
+          }
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      }
+      // frees the slot (in every CTA of the cluster): this warp's wgmma that read it are done
+      __syncwarp();
+      if (lane == 0) {
+        if (ncl == 1) mbar_arrive(&empty[s]);
+        else
+          for (uint32_t c = 0; c < ncl; ++c) mbar_arrive_cluster(&empty[s], c);
+      }
+    }
+    // every stage has been consumed, so no copy can still land in the ring: it becomes the accumulator image
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // ... by BOTH consumer warpgroups: the other one may still be reading it
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+      store_acc_tile<NPAD, X2>(acc[mt], acc_img + (size_t)(64 * wg) * Cfg::ACC_LD + mt * NPAD, Cfg::ACC_LD);
+  }
+  __syncthreads();
+  if (warp < 4) {
+    // ===================== epilogue: accumulator image -> act(acc*scale+shift) -> blocked global store ===============
+    const int m = warp * 32 + lane;  // accumulator row
+    const float *arow = acc_img + (size_t)m * Cfg::ACC_LD;
     const int yy = m >> 3, xx = m & 7;
     constexpr bool UP = PAR || MERGE || MERGE8 || C1;
     const int Ho = UP ? 2 * p.H : p.H, Wo = UP ? 2 * p.W : p.W, Do = UP ? 2 * p.D : p.D;
     const int oz_plain = UP ? 2 * zj + pz : zj, oy = PAR ? 2 * (y0 + yy) + py : y0 + yy;
     if constexpr (C1) {
-      const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
       const float bias = __ldg(p.shift);
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt) {
         float v[8];
-        tmem_ld8(trow + (uint32_t)(mt * NACC), v);
-        if constexpr (X2) {
-          float l[8];
-          tmem_ld8(trow + (uint32_t)(mt * NACC + NPAD), l);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = fmaf(l[i], LO_SCALE, v[i]);
-        }
+        ld_row<8>(arow + mt * NPAD, v);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           v[i] += bias;
@@ -341,7 +389,6 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       constexpr int NZ = MERGE8 ? 2 : 1;      // z classes held by this CTA's accumulators
       constexpr int CP = NPAD / (4 * NZ);     // output channels per class
       static_assert(CP % 4 == 0, "merged classes must be whole channel groups");
-      const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt) {
         const int oxb = 2 * (x0 + 8 * mt + xx);
@@ -353,16 +400,13 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
           for (int cgo = 0; cgo < CP / 4; ++cgo) {
             if (cgo >= p.cgo) continue;  // uniform across the CTA
-            float v[8];
-            tmem_ld4x2(trow + (uint32_t)(mt * NACC + (qzy * 2) * CP + cgo * 4),
-                       trow + (uint32_t)(mt * NACC + (qzy * 2 + 1) * CP + cgo * 4), v);
-            if constexpr (X2) {
-              float l[8];
-              tmem_ld4x2(trow + (uint32_t)(mt * NACC + NPAD + (qzy * 2) * CP + cgo * 4),
-                         trow + (uint32_t)(mt * NACC + NPAD + (qzy * 2 + 1) * CP + cgo * 4), l);
+            float v[8], v4[4];
+            ld_row<4>(arow + mt * NPAD + (qzy * 2) * CP + cgo * 4, v4);
 #pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = fmaf(l[i], LO_SCALE, v[i]);
-            }
+            for (int i = 0; i < 4; ++i) v[i] = v4[i];
+            ld_row<4>(arow + mt * NPAD + (qzy * 2 + 1) * CP + cgo * 4, v4);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[4 + i] = v4[i];
             float4 o[2];
 #pragma unroll
             for (int qx = 0; qx < 2; ++qx) {
@@ -387,13 +431,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
       for (int nb = 0; nb < NPAD / 32; ++nb) {
         float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(mt * NACC + nb * 32), v);
-        if constexpr (X2) {
-          float l[32];
-          tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(mt * NACC + NPAD + nb * 32), l);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaf(l[i], LO_SCALE, v[i]);
-        }
+        ld_row<32>(arow + mt * NPAD + nb * 32, v);
 #pragma unroll
         for (int g4 = 0; g4 < 8; ++g4) {
           const int cgo = nb * 8 + g4;
@@ -413,62 +451,10 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       }
     }
     }
-    tc_fence_before();
-  } else if (lane == 0) {
-    // ===================== MMA issuer (one thread) =============================================================
-    constexpr uint32_t idesc = F16 ? umma_idesc_f16(128, NACC) : umma_idesc_tf32(128, NACC);
-    constexpr uint32_t idesc_lo = umma_idesc_f16(128, NPAD);   // X2: A_lo' x W_hi, the first NPAD columns of the same B tile
-    bool first = true;
-    int it = 0;
-    for (int q = 0; q < n_q; ++q) {
-      int tz, kc, ys, bz, by, bx;
-      const bool valid = stage_of(q, tz, kc, ys, bz, by, bx);
-      if (!valid && ncl == 1) continue;
-      const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-      ++it;
-      mbar_wait(&full[s], use & 1);
-      tc_fence_after();
-      if (valid) {
-      const uint32_t sa = smem_u32(stages + (size_t)s * Cfg::STAGE_BYTES);
-      const uint32_t sb = sa + Cfg::A_BYTES;
-      const int ty0 = ys * Cfg::ROWS;
-#pragma unroll
-      for (int r = 0; r < Cfg::ROWS; ++r) {
-        const int ty = ty0 + r;
-        if (ty >= T) break;
-#pragma unroll
-        for (int tx = 0; tx < T; ++tx) {
-          const uint64_t bdesc = umma_desc(sb + (r * T + tx) * Cfg::B_TAP_BYTES, (NACC / 8) * 128, 128);
-#pragma unroll
-          for (int mt = 0; mt < MT; ++mt) {
-            // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x
-            const uint32_t a0 = sa + (((T - 1 - ty) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
-            const uint64_t adesc = umma_desc(a0, Cfg::A_CG_STRIDE, Cfg::PX * 16);
-            const bool acc = !first || (r | tx);
-            if (F16) umma_f16(tmem_base + mt * NACC, adesc, bdesc, idesc, acc);
-            else umma_tf32(tmem_base + mt * NACC, adesc, bdesc, idesc, acc);
-            if constexpr (X2) {
-              const uint64_t adesc_lo = umma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, Cfg::PX * 16);
-              umma_f16(tmem_base + mt * NACC + NPAD, adesc_lo, bdesc, idesc_lo, true);
-            }
-          }
-        }
-      }
-      first = false;
-      }
-      // frees the slot (in every CTA of the cluster) when the MMAs that read it are done (implies fence::before_thread_sync)
-      if (ncl == 1) umma_commit(&empty[s]);
-      else umma_commit_multicast(&empty[s], cmask);
-    }
-    umma_commit(accum_full);
   }
-  __syncthreads();
   if (ncl > 1) cluster_sync_all();   // no CTA leaves while a peer may still signal its barriers
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS) : "memory");
-  }
 }
+
 
 // ---- tensor maps of the activation operands (host) ------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -573,18 +559,21 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
 
 template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
 static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
-  if (conv_use_tma()) return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, true>(p, st);
-  return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, false>(p, st);
+  // narrower x tiles (more CTAs, each with fewer M-tiles) until the accumulators fit the consumers' registers
+  if constexpr (MT > 1 && MT * (OP == 2 ? 2 : 1) * NPAD > CT_ACC_COLS) {
+    return launch_convt_impl<TZ, T, NPAD, MT / 2, MODE, OP>(p, st);
+  } else {
+    if (conv_use_tma()) return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, true>(p, st);
+    return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, false>(p, st);
+  }
 }
 
 static thread_local int g_conv_op = 0;  // operand type of the next launch (set by the C ABI entry points): 0 TF32, 1 fp16, 2 fp16 hi/lo
-// X2 doubles the accumulator columns: halve the M-tiles per CTA until MT * 2 * NPAD fits the 512 TMEM columns
+// X2 doubles the accumulator columns (launch_convt_impl narrows the tile to fit them)
 template <int TZ, int T, int NPAD, int MT, int MODE>
 static int launch_convt_x2(const ConvTParams &p, cudaStream_t st) {
   if constexpr (NPAD % 16 != 0 || 2 * NPAD > 256) {
     return fail_arg(GENRE_B200_EINVAL, "convt3d: the fp16 hi/lo mode needs N = %d to be a multiple of 16, at most 128", NPAD);
-  } else if constexpr (MT * 2 * NPAD > 512) {
-    return launch_convt_x2<TZ, T, NPAD, MT / 2, MODE>(p, st);
   } else {
     return launch_convt_impl<TZ, T, NPAD, MT, MODE, 2>(p, st);
   }
@@ -746,7 +735,7 @@ extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src_, int cg, int6
   p.srcpar_cgs = 0;
   p.base[0] = p.base[1] = 1;  // input cell = j + 1 - t
   // npad 80: the z class moves to blockIdx.y (MODE 2 with 3 z taps per class; wpack [2 qz][3][chunk][9][2][10][8][g]):
-  // twice the MMAs of the 8-class form, but 256 TMEM columns and half the weight bytes per stage let two CTAs share an SM
+  // twice the MMAs of the 8-class form, but half the accumulator columns and weight bytes per stage
   if (npad == 80) return launch_convt_merged<3, 3, 80, 2>(p, as_stream(stream));
   return launch_conv_merged8<3, 160, 2>(p, as_stream(stream));
 }
@@ -814,14 +803,13 @@ extern "C" int genre_b200_conv3d_taps_forward(const void *src0_, int cg0, const 
   p.srcpar_cgs = 0;
   p.base[0] = p.base[1] = base;
   cudaStream_t st = as_stream(stream);
-  // 3 taps, N = 64: Conv3d(1 -> 64, k4, s2, p1) over the 2x space-to-depth input (VoxelDiscriminator's first layer);
-  // 32-wide tiles (256 TMEM columns) so that two CTAs share an SM
+  // 3 taps, N = 64: Conv3d(1 -> 64, k4, s2, p1) over the 2x space-to-depth input (VoxelDiscriminator's first layer)
   if (taps == 3 && npad == 64) {
     if (W % 32 == 0) return launch_convt<3, 64, 4, false>(p, st);
     return launch_convt<3, 64, 2, false>(p, st);
   }
   // 5 taps, N = 96: Conv3d(20 -> 80, k8, s2, p3) over the 2x space-to-depth input = the input gradient of Unet_3D.dec5
-  // (ConvTranspose3d 80 -> 20); 32- or 16-wide tiles (384 / 192 TMEM columns)
+  // (ConvTranspose3d 80 -> 20)
   if (taps == 5 && npad == 96) {
     if (W % 32 == 0) return launch_convt<5, 96, 4, false>(p, st);
     return launch_convt<5, 96, 2, false>(p, st);

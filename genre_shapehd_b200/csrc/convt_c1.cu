@@ -2,7 +2,7 @@
 // (Unet_3D.dec6 networks.py:167-168 = cat(dec5, enc1) -> ConvT(40 -> 1); VoxelDecoder main.17 :57; VoxelGenerator :98).
 //
 // With one output channel this is a 320-MAC stencil per output voxel, not a GEMM: tensor cores have nothing to chew on
-// (N = 1), so it runs on the FP32 pipe.  Inputs arrive in the channel-blocked layout the tcgen05 kernels write
+// (N = 1), so it runs on the FP32 pipe.  Inputs arrive in the channel-blocked layout the wgmma kernels write
 // ([B*D][C/4][H][W][4]), so one 16-byte load brings 4 channels of a position and one 16-byte broadcast load brings the
 // matching 4 weights: 118 loads per 1024 FMAs.  A thread owns 4 input-aligned cells along x = 32 outputs (4 cells x 8
 // parities), needs the 3 x 3 x 6 neighbourhood per channel group, and writes eight 16-byte stores into the NCDHW

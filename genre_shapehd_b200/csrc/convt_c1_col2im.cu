@@ -1,4 +1,4 @@
-// convt_c1_col2im.cu — ConvTranspose3d(Cin -> 1, k 4, s 2, p 1) on 64-wide volumes as a tcgen05 GEMM over the 64 kernel taps
+// convt_c1_col2im.cu — ConvTranspose3d(Cin -> 1, k 4, s 2, p 1) on 64-wide volumes as a wgmma GEMM over the 64 kernel taps
 // followed by a shared-memory col2im: the last layer of every decoder at full size.
 //
 // Reference layers: networks/networks.py:167-168 (Unet_3D.dec6 = cat(dec5, enc1) -> ConvTranspose3d(2 nf -> 1) on 64^3),
@@ -12,10 +12,11 @@
 // The A operand of the GEMM is the channel-blocked activation itself (no halo, no im2col): 128 consecutive positions of one
 // (plane, channel group) are 128 contiguous 16-byte units = the K-major no-swizzle operand, fetched with plain bulk copies.
 //
-// CTA = one (sample, band of 8 input rows), sweeping z.  Per z step: 512 positions (4 M-tiles of 2 rows x 64) x 64 taps are
-// accumulated in TMEM (fp16 operands; OP 2 = the fp32-accurate hi/lo split of convt3d.cu: columns [0,64) hi*hi, [64,128) the
-// 2^11-scaled cross terms), then 16 epilogue warps (one thread per position) add them into a ring of four output planes in
-// shared memory.  Along x the two contributions of an output are summed in registers (warp shuffles; the two lanes at a warp
+// CTA = one (sample, band of 2 input rows), sweeping z.  Per z step: 128 positions (one M-tile of 2 rows x 64) x 64 taps are
+// accumulated in the registers of one consumer warpgroup (fp16 operands; OP 2 = the fp32-accurate hi/lo split of convt3d.cu:
+// columns [0,64) hi*hi, [64,128) the 2^11-scaled cross terms: 128 fp32 registers per thread, which is what bounds the band),
+// which stores hi + 2^-11 cross to a shared-memory image; 4 epilogue warps (one thread per position) then add the image into
+// a ring of four output planes in shared memory while the consumers accumulate the next step.  Along x the two contributions of an output are summed in registers (warp shuffles; the two lanes at a warp
 // seam exchange through a scratch), and the taps are processed in 4 phases (kz>>1, ky>>1): within a phase a position adds one
 // float2 (outputs 2x, 2x+1) to each of 4 (kz, ky) rows and different positions hit different cells, so the adds are race-free
 // without atomics; a barrier separates phases (shared-memory traffic: 1/4 of a per-tap scatter, and conflict-free).  Output
@@ -30,11 +31,12 @@
 namespace gb {
 
 constexpr int CI_W = 64;             // input width (positions per row)
-constexpr int CI_ROWS = 8;           // input rows per band
-constexpr int CI_POS = CI_W * CI_ROWS;   // positions per z step = 4 M-tiles
-constexpr int CI_MT = 4;
-constexpr int CI_EPI_WARPS = 16;          // one warp per (M-tile, TMEM lane quarter): a thread owns one input position per z step
-constexpr int CI_THREADS = (CI_EPI_WARPS + 2) * 32;   // + MMA warp + producer warp
+constexpr int CI_ROWS = 2;           // input rows per band
+constexpr int CI_POS = CI_W * CI_ROWS;   // positions per z step = 1 M-tile
+constexpr int CI_MT = 1;
+constexpr int CI_EPI_WARPS = 4 * CI_MT;   // one warp per (M-tile, 32-row quarter): a thread owns one input position per z step
+constexpr int CI_THREADS = (CI_EPI_WARPS + 5) * 32;   // + consumer warpgroup + producer warp
+constexpr int CI_ACC_LD = 64 + 4;        // accumulator image [CI_POS rows][CI_ACC_LD] fp32
 constexpr int CI_MAX_STAGES = 6;
 constexpr int CI_UY = 2 * CI_ROWS + 2;   // output rows touched by a band
 constexpr int CI_PITCH = 136;            // floats per ring row: column ux + 3 holds output x = ux - 1 (x = 0 is 16-byte aligned)
@@ -52,16 +54,6 @@ struct ColParams {
 
 __device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-// 16 accumulator columns of this thread's row, no wait (tmem_ld_wait() before the registers are read)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                 "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 __device__ __forceinline__ void red_add_v4(float *p, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
@@ -71,21 +63,19 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
   constexpr bool X2 = OP == 2;
   constexpr int PARTS = X2 ? 2 : 1;
   constexpr int NACC = PARTS * 64;
-  constexpr int CG_BYTES = CI_POS * 16;                  // one channel group of one part: 8 rows x 64 positions x 16 B
+  constexpr int CG_BYTES = CI_POS * 16;                  // one channel group of one part: CI_ROWS rows x 64 positions x 16 B
   constexpr int STAGE_BYTES = PARTS * 2 * CG_BYTES;      // one K step (16 channels)
   constexpr int W_KSTEP_BYTES = 2 * (NACC / 8) * 128;
-  constexpr int TMEM_COLS = CI_MT * NACC;                // 256 or 512
-  constexpr float LO_SCALE = 1.0f / 2048.0f;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *stages = smem;
   uint8_t *sw = smem + (size_t)p.stages * STAGE_BYTES;
   float *ring = reinterpret_cast<float *>(sw + (size_t)p.ksteps * W_KSTEP_BYTES);
-  uint64_t *full = reinterpret_cast<uint64_t *>(ring + 4 * CI_PLANE);
+  float *acc_img = ring + 4 * CI_PLANE;
+  uint64_t *full = reinterpret_cast<uint64_t *>(acc_img + CI_POS * CI_ACC_LD);
   uint64_t *empty = full + CI_MAX_STAGES;
   uint64_t *wbar = empty + CI_MAX_STAGES;
-  uint64_t *tmem_full = wbar + 1;
-  uint64_t *tmem_empty = tmem_full + 1;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_empty + 1);
+  uint64_t *acc_full = wbar + 1;     // the consumers have stored step z's accumulators to the image
+  uint64_t *acc_empty = acc_full + 1;   // the epilogue has read them
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int band = blockIdx.x, nbands = gridDim.x, b = blockIdx.y;
@@ -94,23 +84,16 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
   if (tid == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 4);    // the 4 consumer warps
     }
     mbar_init(wbar, 1);
-    mbar_init(tmem_full, 1);
-    mbar_init(tmem_empty, CI_EPI_WARPS * 32);
+    mbar_init(acc_full, 128);
+    mbar_init(acc_empty, CI_EPI_WARPS * 32);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == CI_EPI_WARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == CI_EPI_WARPS + 1) {
+  if (warp == CI_EPI_WARPS + 4) {
     // ===================== producer =============================================================================
     if (lane == 0) {
       mbar_arrive_expect_tx(wbar, (uint32_t)(p.ksteps * W_KSTEP_BYTES));
@@ -138,37 +121,43 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
         }
       }
     }
-  } else if (warp == CI_EPI_WARPS) {
-    // ===================== MMA issuer ===========================================================================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(128, NACC);
-      constexpr uint32_t idesc_lo = umma_idesc_f16(128, 64);
-      mbar_wait(wbar, 0);
-      int it = 0;
-      for (int z = 0; z < p.D; ++z) {
-        if (z > 0) mbar_wait(tmem_empty, (z - 1) & 1);   // the epilogue has read step z-1's accumulators
-        tc_fence_after();
-        for (int ks = 0; ks < p.ksteps; ++ks, ++it) {
-          const int s = it % p.stages, use = it / p.stages;
-          mbar_wait(&full[s], use & 1);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(stages + (size_t)s * STAGE_BYTES);
-          const uint64_t bdesc = umma_desc(smem_u32(sw) + ks * W_KSTEP_BYTES, (NACC / 8) * 128, 128);
+  } else if (warp >= CI_EPI_WARPS) {
+    // ===================== consumers: the two m64 halves of the M-tile, accumulators in registers =====================
+    static_assert(CI_MT == 1, "one consumer warpgroup holds one M-tile");
+    mbar_wait(wbar, 0);
+    int it = 0;
+    for (int z = 0; z < p.D; ++z) {
+      float acc[2][NACC / 2];
 #pragma unroll
-          for (int mt = 0; mt < CI_MT; ++mt) {
-            const uint32_t a0 = sa + mt * 128 * 16;
-            umma_f16(tmem_base + mt * NACC, umma_desc(a0, CG_BYTES, 128), bdesc, idesc, ks > 0);
-            if constexpr (X2) umma_f16(tmem_base + mt * NACC + 64, umma_desc(a0 + 2 * CG_BYTES, CG_BYTES, 128), bdesc, idesc_lo, true);
-          }
-          umma_commit(&empty[s]);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < NACC / 2; ++j) acc[h][j] = 0.0f;
+      for (int ks = 0; ks < p.ksteps; ++ks, ++it) {
+        const int s = it % p.stages, use = it / p.stages;
+        mbar_wait(&full[s], use & 1);
+        wgmma_fence();
+        const uint32_t sa = smem_u32(stages + (size_t)s * STAGE_BYTES);
+        const uint64_t bdesc = gmma_desc(smem_u32(sw) + ks * W_KSTEP_BYTES, (NACC / 8) * 128, 128);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t a0 = sa + h * 64 * 16;
+          wgmma_f16<NACC>(acc[h], gmma_desc(a0, CG_BYTES, 128), bdesc);
+          if constexpr (X2) wgmma_f16<64>(acc[h] + 32, gmma_desc(a0 + 2 * CG_BYTES, CG_BYTES, 128), bdesc);
         }
-        umma_commit(tmem_full);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
       }
+      if (z > 0) mbar_wait(acc_empty, (z - 1) & 1);   // the epilogue has read step z-1's accumulators
+#pragma unroll
+      for (int h = 0; h < 2; ++h) store_acc_tile<64, X2>(acc[h], acc_img + h * 64 * CI_ACC_LD, CI_ACC_LD);
+      mbar_arrive(acc_full);
     }
   } else {
-    // ===================== epilogue: TMEM -> scatter-add into the plane ring -> global ================================
-    const int etid = tid;                                 // 0..511
-    const int quarter = warp & 3, mt = warp >> 2;         // TMEM lane quarter of this warp; its M-tile
+    // ===================== epilogue: accumulator image -> scatter-add into the plane ring -> global ======================
+    const int etid = tid;                                 // 0..CI_EPI_WARPS*32 - 1
+    const int quarter = warp & 3, mt = warp >> 2;         // 32-row quarter of this warp; its M-tile
     const int row = quarter * 32 + lane;                  // accumulator row within the M-tile: input row (row >> 6), x = row & 63
     const int x = row & 63;
     const int yl = 2 * mt + (row >> 6);                   // input row of this thread within the band
@@ -177,12 +166,12 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
     const float bias = __ldg(p.bias);
     const int Ho = 2 * p.H, Do = 2 * p.D;
     constexpr int Wo = 2 * CI_W;
-    const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
+    const float *arow = acc_img + (size_t)(mt * 128 + row) * CI_ACC_LD;
     // ring cell of output column ox = 2x of this thread's two input rows (column ox + 4: even, so an (ox, ox + 1) pair is one float2)
     float *base = ring + (2 * yl) * CI_PITCH + 2 * x + 4;
     const int xhalf = quarter & 1, ysub = quarter >> 1;
     // taps kx = 3 of x = 31 and kx = 0 of x = 32 belong to cells of the neighbouring warp: exchanged through this scratch
-    float *scr = reinterpret_cast<float *>(tmem_slot + 2);   // [2 buffers][4 M-tiles][2 rows][2 directions][4 (rz,ry)]
+    float *scr = reinterpret_cast<float *>(acc_empty + 1);   // [2 buffers][M-tile: 4 slots, CI_MT used][2 rows][2 directions][4 (rz,ry)]
 
     auto flush_plane = [&](int slot, int oz) {   // complete plane -> global, ring slot back to zero
       float *pl = ring + slot * CI_PLANE;
@@ -202,33 +191,21 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
     };
 
     for (int z = 0; z < p.D; ++z) {
-      mbar_wait(tmem_full, z & 1);
-      tc_fence_after();
+      mbar_wait(acc_full, z & 1);
       const int zs = (2 * z) & 3;   // ring slot of tap kz = 0 (output plane 2z - 1); tap kz uses (zs + kz) & 3
       // 4 phases (tz, ty): the 16 taps (rz, ry, kx = 0..3) of a position.  Along x the two contributions of an output are
       // summed in registers first (ox = 2x: kx = 1 of x and kx = 3 of x - 1; ox = 2x + 1: kx = 2 of x and kx = 0 of x + 1, via
       // warp shuffles), so a position adds ONE float2 per (kz, ky) to the ring: distinct cells for distinct positions.
-      // The TMEM read of phase ph + 1 (hi half) is issued before the adds of phase ph: its latency hides behind the
-      // shared-memory work; the 4 ring cells are loaded before any of them is touched (no load-add-store chains).
+      // The 4 ring cells are loaded before any of them is touched (no load-add-store chains).
       float *pb[4];   // this position's cell row in the ring plane of tap kz
 #pragma unroll
       for (int k = 0; k < 4; ++k) pb[k] = base + ((zs + k) & 3) * CI_PLANE;
-      uint32_t rh[16], rl[16];
-      tmem_ld16_nowait(trow + (uint32_t)(mt * NACC), rh);
 #pragma unroll
       for (int ph = 0; ph < 4; ++ph) {
         const int tz = ph >> 1, ty = ph & 1;
-        if constexpr (X2) tmem_ld16_nowait(trow + (uint32_t)(mt * NACC + 64 + ph * 16), rl);
-        tmem_ld_wait();
         float v[16];   // index tx * 8 + rz * 4 + ry * 2 + rx, kx = 2 tx + rx
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = X2 ? fmaf(__uint_as_float(rl[i]), LO_SCALE, __uint_as_float(rh[i])) : __uint_as_float(rh[i]);
-        if (ph < 3) {
-          tmem_ld16_nowait(trow + (uint32_t)(mt * NACC + (ph + 1) * 16), rh);
-        } else {        // the last TMEM read of this step has landed: the MMA warp may overwrite the accumulators
-          tc_fence_before();
-          mbar_arrive(tmem_empty);
-        }
+        ld_row<16>(arow + ph * 16, v);
+        if (ph == 3) mbar_arrive(acc_empty);   // the last read of this step's image: the consumers may overwrite it
         float *sb = scr + (ph & 1) * 64 + (mt * 2 + ysub) * 8;
         if (lane == 31 && xhalf == 0) {
 #pragma unroll
@@ -271,12 +248,6 @@ __global__ void __launch_bounds__(CI_THREADS, 1) convt_c1_col2im_kernel(const Co
     }
     // the last step's tap kz = 2 plane (output 2D - 1) has no later contributor; its kz = 3 plane (output 2D) is dropped
     flush_plane((2 * (p.D - 1) + 2) & 3, Do - 1);
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == CI_EPI_WARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
   }
 }
 
@@ -284,7 +255,8 @@ template <int OP>
 static int launch_col2im(ColParams &p, cudaStream_t st) {
   constexpr int PARTS = OP == 2 ? 2 : 1, NACC = PARTS * 64;
   constexpr int STAGE_BYTES = PARTS * 2 * CI_POS * 16;
-  const int fixed = p.ksteps * 2 * (NACC / 8) * 128 + 4 * CI_PLANE * 4 + 1024;   // weights + plane ring + barriers, TMEM slot, exchange scratch
+  // weights + plane ring + accumulator image + barriers and exchange scratch
+  const int fixed = p.ksteps * 2 * (NACC / 8) * 128 + 4 * CI_PLANE * 4 + CI_POS * CI_ACC_LD * 4 + 1024;
   int stages = (226 * 1024 - fixed) / STAGE_BYTES;
   if (stages > CI_MAX_STAGES) stages = CI_MAX_STAGES;
   GB_REQUIRE(stages >= 2, GENRE_B200_EINVAL, "convt_c1_col2im: %d K steps of weights leave no room for the pipeline", p.ksteps);
@@ -330,11 +302,13 @@ extern "C" int genre_b200_convt_c1_col2im_forward(const void *src0, int cg0, con
   p.bias = bias;
   p.out = out;
   cudaStream_t st = as_stream(stream);
-  // zero the output rows two bands share (rows 16 j - 1, 16 j of every plane: pairs of adjacent rows at a pitch of 16 rows)
+  // zero the output rows two bands share (rows 2 R j - 1, 2 R j of every plane, R = CI_ROWS: pairs of adjacent rows at a pitch
+  // of 2 R rows)
   const int64_t Wo = 2 * W, Ho = 2 * H, Do = 2 * D, nbands = H / CI_ROWS;
   const int64_t pairs = B * Do * nbands - 1;
   if (nbands > 1 && pairs > 0) {
-    if (cudaMemset2DAsync(out + 15 * Wo, (size_t)16 * Wo * sizeof(float), 0, (size_t)2 * Wo * sizeof(float), (size_t)pairs, st) != cudaSuccess)
+    if (cudaMemset2DAsync(out + (2 * CI_ROWS - 1) * Wo, (size_t)2 * CI_ROWS * Wo * sizeof(float), 0, (size_t)2 * Wo * sizeof(float),
+                          (size_t)pairs, st) != cudaSuccess)
       return check_launch("convt_c1_col2im: memset");
   }
   (void)Ho;

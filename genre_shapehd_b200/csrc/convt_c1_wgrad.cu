@@ -14,6 +14,10 @@
 
 namespace gb {
 
+// CTAs of a weight-gradient launch, two per SM: the workspace holds one partial sum per CTA, so its size and the grid
+// come from this one value
+static int wgrad_max_ctas() { return 2 * sm_count(); }
+
 constexpr int WG_THREADS = 256;   // 64 taps x 4 channel lanes
 constexpr int WG_ROWS = 8;        // input rows per slab
 constexpr int WG_MAX_CPT = 16;    // channels per thread (Cin <= 64)
@@ -161,7 +165,7 @@ convt_c1_dgrad_kernel(const float *__restrict__ gy, const float *__restrict__ we
 
 using namespace gb;
 
-extern "C" size_t genre_b200_convt_c1_wgrad_workspace_bytes(int cin) { return (size_t)148 * 2 * (size_t)cin * 64 * sizeof(float); }
+extern "C" size_t genre_b200_convt_c1_wgrad_workspace_bytes(int cin) { return (size_t)wgrad_max_ctas() * (size_t)cin * 64 * sizeof(float); }
 
 // x [B][Cin][D][H][W] fp32 contiguous (the concatenated input), gy [B][1][2D][2H][2W] fp32 contiguous,
 // dW [Cin][1][4][4][4] (fully written).  H % 8 == 0, Cin <= 64, workspace of genre_b200_convt_c1_wgrad_workspace_bytes(Cin).
@@ -177,7 +181,7 @@ extern "C" int genre_b200_convt_c1_wgrad(const float *x, const float *gy, int64_
              (long long)W, (long long)Cin);
   const int64_t n_slabs = B * D * (H / WG_ROWS);
   GB_REQUIRE(n_slabs < (1ll << 31), GENRE_B200_EINVAL, "convt_c1_wgrad: too many slabs");
-  const int grid = (int)(n_slabs < 148 * 2 ? n_slabs : 148 * 2);
+  const int grid = (int)(n_slabs < wgrad_max_ctas() ? n_slabs : wgrad_max_ctas());
   cudaStream_t st = as_stream(stream);
   const int cpt = (int)((Cin + 3) / 4);
 #define GB_WG(CPT)                                                                                                   \
@@ -312,7 +316,7 @@ conv_k8s2_wgrad_reduce_kernel(const float *__restrict__ partial, int n_parts, in
 
 }  // namespace gb
 
-extern "C" size_t genre_b200_conv_k8s2_wgrad_workspace_bytes(void) { return (size_t)148 * 2 * 20480 * sizeof(float); }
+extern "C" size_t genre_b200_conv_k8s2_wgrad_workspace_bytes(void) { return (size_t)wgrad_max_ctas() * 20480 * sizeof(float); }
 
 // x [B][Cin][D][H][W], gy [B][Cout][D/2][H/2][W/2] (fp32, contiguous) -> dW [Cout][Cin][8][8][8] (fully written).
 // Cin <= 2, Cout <= 20, even extents, (H/2) % 8 == 0, W <= 128.
@@ -331,7 +335,7 @@ extern "C" int genre_b200_conv_k8s2_wgrad(const float *x, const float *gy, int64
   GB_REQUIRE(smem <= 200 * 1024, GENRE_B200_EINVAL, "conv_k8s2_wgrad: slab does not fit shared memory");
   const int64_t n_slabs = B * (D / 2) * ((H / 2) / W8_ROWS);
   GB_REQUIRE(n_slabs < (1ll << 31), GENRE_B200_EINVAL, "conv_k8s2_wgrad: too many slabs");
-  const int grid = (int)(n_slabs < 148 * 2 ? n_slabs : 148 * 2);
+  const int grid = (int)(n_slabs < wgrad_max_ctas() ? n_slabs : wgrad_max_ctas());
   cudaStream_t st = as_stream(stream);
   cudaError_t e = cudaFuncSetAttribute(conv_k8s2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail_arg((int)e, "conv_k8s2_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(e));

@@ -1,4 +1,4 @@
-// layout.cu — NCDHW <-> channel-blocked activation layouts for the tcgen05 convolution kernels (convt3d.cu).
+// layout.cu — NCDHW <-> channel-blocked activation layouts for the wgmma convolution kernels (convt3d.cu).
 //
 // The reference's nets (networks/networks.py) exchange NCDHW fp32 tensors; the kernels want 16 bytes per position and
 // channel group ([B*D][C/g][H][W][g], g = 4 fp32 or 8 fp16) so that a tap shift is an address offset.  These are the
@@ -266,7 +266,7 @@ split3_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, int CG, 
 
 static unsigned ly_grid(size_t n) {
   const size_t blocks = (n + LY_THREADS - 1) / LY_THREADS;
-  const size_t cap = 148ull * 8 * 16;  // grid-stride beyond ~16 waves of 8 CTAs per SM
+  const size_t cap = (size_t)sm_count() * 8 * 16;  // grid-stride beyond ~16 waves of 8 CTAs per SM
   return (unsigned)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
 

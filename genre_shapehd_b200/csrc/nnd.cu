@@ -6,18 +6,17 @@
 //   NmDistanceGradKernel :143-162, launcher :163-177 (two cudaMemset + two launches, default stream)
 // Here one launch covers both directions.  The op is bound by the FP32 issue rate (2*B*N*M pairs x 6 fp32 operations + the
 // running minimum), so the kernel spends as few instructions per pair as exact arithmetic allows:
-//   * sm_100a's packed fp32 instructions (add/mul/fma.rn.f32x2: two IEEE-rounded results per issue slot) evaluate TWO
-//     candidates per instruction; each thread carries two queries, so a shared-memory candidate pair (3 x LDS.64 from SoA
-//     tiles) feeds four pairs;
+//   * candidates come in pairs (float2: each lane evaluates two candidates per step; each thread carries two queries, so a
+//     shared-memory candidate pair (3 x LDS.64 from SoA tiles) feeds four pairs);
 //   * only the running MINIMUM is updated per pair (one FMNMX for two candidates); the arg-min is recovered afterwards: each
 //     lane remembers the 16-candidate chunk in which its minimum improved ("<": the earliest chunk wins) and re-evaluates that
 //     one chunk at the end to find the first index whose distance equals the minimum.
-// 19 instructions per 4 pairs instead of 40.  A CTA owns 128 queries; each query is scanned by 4 lanes on interleaved candidate
+// Hopper has no packed fp32 arithmetic, so a pair costs its scalar instructions; the minimum-only update still halves the rest.  A CTA owns 128 queries; each query is scanned by 4 lanes on interleaved candidate
 // pairs and the 4 partial (distance, index) results meet in a 2-step shuffle reduction that keeps the lowest index on ties — the
 // reference's semantics (strict '<' on an ascending scan, nnd_cuda.cu:33,120).
 // The squared distance is rounded exactly as nvcc contracts the reference expression
 // x2*x2+y2*y2+z2*z2 (SASS of oracle/_ref/libref_nnd_cuda.so):  fma(dz,dz, fma(dx,dx, dy*dy)),
-// with d* = candidate - query (packed operations round each half like their scalar forms), so distances AND indices are
+// with d* = candidate - query, each operation IEEE-rounded on its own, so distances AND indices are
 // bit-identical to the reference kernel.
 #include "common.cuh"
 #include <math_constants.h>
@@ -35,8 +34,11 @@ constexpr float NND_FAR = 1e18f;                                   // padding ca
 
 // squared distances of the candidate pair (cx, cy, cz) to the query whose negated coordinates are duplicated in (nx, ny, nz)
 __device__ __forceinline__ float2 nnd_dist2(float2 cx, float2 cy, float2 cz, float2 nx, float2 ny, float2 nz) {
-  const float2 dx = __fadd2_rn(cx, nx), dy = __fadd2_rn(cy, ny), dz = __fadd2_rn(cz, nz);
-  return __ffma2_rn(dz, dz, __ffma2_rn(dx, dx, __fmul2_rn(dy, dy)));
+  const float2 dx = make_float2(__fadd_rn(cx.x, nx.x), __fadd_rn(cx.y, nx.y));
+  const float2 dy = make_float2(__fadd_rn(cy.x, ny.x), __fadd_rn(cy.y, ny.y));
+  const float2 dz = make_float2(__fadd_rn(cz.x, nz.x), __fadd_rn(cz.y, nz.y));
+  return make_float2(__fmaf_rn(dz.x, dz.x, __fmaf_rn(dx.x, dx.x, __fmul_rn(dy.x, dy.x))),
+                     __fmaf_rn(dz.y, dz.y, __fmaf_rn(dx.y, dx.y, __fmul_rn(dy.y, dy.y))));
 }
 __device__ __forceinline__ float nnd_dist1(float cx, float cy, float cz, float qx, float qy, float qz) {
   const float dx = __fadd_rn(cx, -qx), dy = __fadd_rn(cy, -qy), dz = __fadd_rn(cz, -qz);

@@ -636,13 +636,13 @@ extern "C" int genre_b200_render_spherical_forward_skip(const float *vox, int64_
   }
   if (int rc = check_launch("render_spherical occupancy kernel")) return rc;
   const int ngroups = (sph_res * sph_res + 3) / 4;
-  // one wave of resident CTAs over the whole batch (OCC per SM, 148 SMs), warps stride over the ray groups
+  // one wave of resident CTAs over the whole batch (OCC per SM on every SM), warps stride over the ray groups
   static int occ = 0;
   if (!occ) {
     const char *e = getenv("GENRE_B200_RENDER_OCC");   // tuning knob (profiles/): 4 or 5
     occ = (e && atoi(e) == 4) ? 4 : 5;
   }
-  int ctas = (int)((148 * occ) / N);
+  int ctas = (int)(((long long)sm_count() * occ) / N);
   const int max_ctas = (ngroups + RS_THREADS / 32 - 1) / (RS_THREADS / 32);
   if (ctas > max_ctas) ctas = max_ctas;
   if (ctas < 1) ctas = 1;

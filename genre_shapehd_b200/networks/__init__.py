@@ -3,7 +3,7 @@
 ``networks.networks`` (the 3D voxel nets, on the hot path) is provided here.  The 2D U-ResNet-18 modules
 (``networks.uresnet``, ``networks.revresnet``) are outside the hot path (SURVEY.md §2.1 #6) and keep resolving to a
 checkout of the reference when one is available: its ``networks`` directory is appended to this package's
-``__path__`` (nothing is copied).  Search order: $GENRE_REF, <repo>/baseline/_ref, /root/reference.
+``__path__`` (nothing is copied).  Search order: $GENRE_REF, <repo>/baseline/_ref.
 """
 import os
 import sys
@@ -15,7 +15,7 @@ if _REPO_ROOT not in sys.path:
 
 
 def _reference_networks_dir():
-    for root in (os.environ.get("GENRE_REF"), os.path.join(_REPO_ROOT, "baseline", "_ref"), "/root/reference"):
+    for root in (os.environ.get("GENRE_REF"), os.path.join(_REPO_ROOT, "baseline", "_ref")):
         if root:
             d = os.path.join(root, "networks")
             if os.path.isfile(os.path.join(d, "revresnet.py")):

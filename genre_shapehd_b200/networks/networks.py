@@ -12,7 +12,7 @@ Layers are created in the reference's order, so a model built under the same tor
 parameters (tests/test_networks.py checks digests recorded from the reference).
 
 Every convolution is a ``Conv3d`` / ``ConvTranspose3d`` below: a torch parameter container whose CUDA forward can be
-routed to the hand-written sm_100a implicit-GEMM kernels (genre_shapehd_b200/ops_conv.py) layer by layer; layers
+routed to the hand-written sm_90a implicit-GEMM kernels (genre_shapehd_b200/ops_conv.py) layer by layer; layers
 without a custom kernel run on cuDNN exactly like the reference does.
 """
 import torch
@@ -23,7 +23,7 @@ from genre_shapehd_b200 import ops_conv
 
 
 class Conv3d(nn.Conv3d):
-    """nn.Conv3d parameters + dispatch of the CUDA forward to the sm_100a kernel when one covers the layer."""
+    """nn.Conv3d parameters + dispatch of the CUDA forward to the sm_90a kernel when one covers the layer."""
 
     def forward(self, x):
         y = ops_conv.conv3d(x, self) if x.is_cuda else None

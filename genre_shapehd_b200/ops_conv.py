@@ -1,11 +1,11 @@
-"""Dispatch of the 3D convolutions of networks/networks.py to the hand-written sm_100a kernels.
+"""Dispatch of the 3D convolutions of networks/networks.py to the hand-written sm_90a kernels.
 
 ``conv3d(x, module)`` / ``conv_transpose3d(x, module)`` / ``deconv_skip(...)`` return the result computed by this
 library's kernels, or ``None`` when no kernel covers the layer (shape / dtype / device / autograd) — the caller then
 runs the layer the way the reference does (torch.nn -> cuDNN; in the fp32-accurate mode through ``exact_fallback``).
 
 Kernels and what they cover (routing conditions are the ``*_supported`` predicates below, all of them tested both ways):
-  csrc/convt3d.cu          tcgen05 implicit GEMM on halo tiles: ConvTranspose3d k 4 / 8, s 2 (planes 16 or 32 wide), Conv3d
+  csrc/convt3d.cu          wgmma implicit GEMM on halo tiles: ConvTranspose3d k 4 / 8, s 2 (planes 16 or 32 wide), Conv3d
                            k 4 s 2 via parity sub-volumes, Conv3d k 8 s 2 via space-to-depth, the 1-channel ConvTranspose3d
                            with 27 union taps; forward under autograd too, tensor-core input gradients for the k 8 layers
   csrc/convflat.cu         the same GEMM over a flattened, zero-separated volume for coarse sides <= 8^3 (inference)
@@ -24,14 +24,14 @@ import torch
 from . import _lib
 
 ENABLED = os.environ.get("GENRE_B200_CONV", "1") != "0"
-# Dispatch policy.  Every kernel is correct on every layer it supports; which layers are ROUTED to it is decided by
-# end-to-end measurements on a B200 (kernel + the NCDHW <-> channel-blocked conversions of csrc/layout.cu around it;
-# profiles/r01_conv_summary.md), B = 16, against cuDNN with TF32 allowed:
-#   convt_k8   ConvTranspose3d k=8 s=2 (Unet_3D.dec5: 7.2 -> 1.35 ms)
-#   conv_k8s2  Conv3d k=8 s=2 on few input channels (Unet_3D.enc1: 16.6 -> 0.8 ms)
-#   convt_c1   ConvTranspose3d k=4 -> 1 channel on already-blocked inputs (Unet_3D.dec6: 2.1 -> 1.3 ms)
-#   convt_k4   ConvTranspose3d k=4 s=2 (dec4 0.30 -> 0.23, VoxelDecoder/Generator stages 1.26 -> 1.01, 1.87 -> 1.46 ms)
-#   conv_k4s2  Conv3d k=4 s=2 (discriminator 1.18 -> 0.86 ms per layer, Unet_3D.enc2/enc3)
+# Dispatch policy.  Every kernel is correct on every layer it supports; which layers are ROUTED to it was decided by
+# end-to-end comparisons (kernel + the NCDHW <-> channel-blocked conversions of csrc/layout.cu around it), B = 16, against
+# cuDNN with TF32 allowed:
+#   convt_k8   ConvTranspose3d k=8 s=2 (Unet_3D.dec5)
+#   conv_k8s2  Conv3d k=8 s=2 on few input channels (Unet_3D.enc1)
+#   convt_c1   ConvTranspose3d k=4 -> 1 channel on already-blocked inputs (Unet_3D.dec6)
+#   convt_k4   ConvTranspose3d k=4 s=2 (dec4, VoxelDecoder/Generator stages)
+#   conv_k4s2  Conv3d k=4 s=2 (discriminator, Unet_3D.enc2/enc3)
 #   convt_c1_convert   the 1-channel layer when its input must first be converted; FP32-pipe kernel, so only up to
 #                      C1_MAX_CIN input channels (VoxelDecoder's 32 -> 1 wins, VoxelGenerator's 64 -> 1 does not)
 # GENRE_B200_CONV_POLICY = comma list restricts the set ("all" = everything, the default).
@@ -1209,7 +1209,7 @@ def _train_forward(x, m, supported):
 
 
 def conv3d(x, m, bn=None, slope=None):
-    """Conv3d on the tcgen05 kernel [+ folded eval BatchNorm3d + LeakyReLU]: k=8,s=2,p=3 on few input channels
+    """Conv3d on the tensor-core kernel [+ folded eval BatchNorm3d + LeakyReLU]: k=8,s=2,p=3 on few input channels
     (Unet_3D.enc1) via space-to-depth, or k=4,s=2,p=1 (discriminator, Unet_3D.enc2/enc3) via parity sub-volumes."""
     if not x.is_cuda:
         return None

@@ -1,5 +1,5 @@
 /*
- * genre_b200.h — C ABI of libgenre_b200.so (sm_100a).
+ * genre_b200.h — C ABI of libgenre_b200.so (sm_90a).
  *
  * This is the drop-in boundary for the GenRe/ShapeHD geometric-projection hot path.  Every entry
  * point takes plain device pointers, sizes, element strides and a cudaStream_t (passed as void*);
@@ -36,8 +36,8 @@ extern "C" {
 /* flags for the projection entry points */
 #define GENRE_B200_FLAG_SHIFT_TDF 1u /* fuse Camera_back_projection_layer.shift_tdf: 1 - R*tdf */
 #define GENRE_B200_FLAG_OVERLAP 2u  /* cam_bp_forward, experimental: project and splat overlapped in ONE kernel (interleaved block
-                                      order, per-map completion counters).  Measured on B200: slower than back to back (75.9 vs
-                                      68.0 us at batch 32), so off by default; see DESIGN.md 4.1 */
+                                      order, per-map completion counters).  Slower than back to back on the GPU it was
+                                      written for and not measured on the H100, so off by default */
 
 const char *genre_b200_last_error(void);
 /* library/ABI version: major*1000 + minor */
@@ -172,8 +172,8 @@ int genre_b200_voxelize_stage_splat(int64_t n_maps, int64_t pixels_per_map, int 
                                     void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
- * ConvTranspose3d(kernel K in {4, 8}, stride 2, padding K/2 - 1) forward as a tcgen05 implicit GEMM (TF32 operands,
- * FP32 accumulation in TMEM).  Replaces the cuDNN call behind nn.ConvTranspose3d in networks/networks.py:211-222
+ * ConvTranspose3d(kernel K in {4, 8}, stride 2, padding K/2 - 1) forward as a wgmma implicit GEMM (TF32 operands,
+ * FP32 accumulation in registers).  Replaces the cuDNN call behind nn.ConvTranspose3d in networks/networks.py:211-222
  * (Unet_3D Deconv3d_skip: the channel concatenation of :221 is walked as two K ranges, never materialised) and
  * :253-256 (deconv3d_2x of VoxelDecoder / VoxelGenerator).
  *   src0 [B*D][cg0][H][W][16 B], src1 [...] or NULL   channel-blocked activations; a channel group is 16 bytes per
@@ -190,7 +190,7 @@ int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, i
                                   const float *scale, const float *shift, float slope,
                                   float *out, int cgo, void *stream);
 
-/* Stride-1 convolution with `taps` (3 or 5) taps per dimension on channel-blocked activations, same tcgen05 kernel:
+/* Stride-1 convolution with `taps` (3 or 5) taps per dimension on channel-blocked activations, same wgmma kernel:
  *   out[b,z,y,x,n] = act(scale[n] * sum_{t,c} in[b, z+base-tz, y+base-ty, x+base-tx, c] * W[t][c][n] + shift[n])
  * Replaces the cuDNN call behind nn.Conv3d of Unet_3D.enc1 (networks/networks.py:151,197: Conv3d(2->20, k=8, s=2, p=3))
  * after a space-to-depth of the input (k=8/s=2 over C channels == 5 taps/s=1 over 8C channels).
@@ -203,7 +203,7 @@ int genre_b200_conv3d_taps_forward(const void *src0, int cg0, const void *src1, 
                                    const float *scale, const float *shift, float slope,
                                    float *out, int cgo, void *stream);
 
-/* Conv3d(kernel 4, stride 2, padding 1) forward on the same tcgen05 kernel.  Replaces the cuDNN call behind conv3d_half
+/* Conv3d(kernel 4, stride 2, padding 1) forward on the same wgmma kernel.  Replaces the cuDNN call behind conv3d_half
  * (VoxelDiscriminator, networks/networks.py:247-250) and Unet_3D.enc2..enc5 (:152-155).  The input arrives as its 8 parity
  * sub-volumes in one channel-blocked tensor src [B*D'][8*cgs][H'][W'][16 B] (D' = D/2 ...; group index = s*cgs + c,
  * s = (pz*2+py)*2+px); sub-volume s is a K range with 2 taps per dimension (kernel index 3 - 2t - p).
@@ -216,7 +216,7 @@ int genre_b200_conv3d_k4s2_forward(const void *src, int cgs, int kblocks, int64_
 
 /* The k 4 / s 2 / p 1 convolutions of the SMALL volumes (coarse side <= 8^3: Unet_3D.enc4, enc5, dec2, dec3,
  * networks/networks.py:157-165; the 4^3 / 8^3 stages of VoxelDecoder / VoxelGenerator / VoxelDiscriminator :40-57,:79-97,:247-256)
- * as a tcgen05 implicit GEMM over the flattened, zero-separated volume (csrc/convflat.cu).  Replaces the cuDNN calls behind
+ * as a wgmma implicit GEMM over the flattened, zero-separated volume (csrc/convflat.cu).  Replaces the cuDNN calls behind
  * those nn.Conv3d / nn.ConvTranspose3d modules in eval mode.
  *   genre_b200_convflat_positions: positions per channel-group array of the operand of a coarse (B, D, H, W) volume
  *       (*lead = index of position 0);
@@ -245,7 +245,7 @@ int genre_b200_skinny_gemm(const float *x, const float *W, int64_t M, int64_t N,
                            const float *scale, const float *shift, float slope, float *out, void *workspace,
                            size_t workspace_bytes, void *stream);
 
-/* ConvTranspose3d(Cin -> 1, kernel 4, stride 2, padding 1) on 64-wide volumes as a tcgen05 GEMM over the 64 kernel taps
+/* ConvTranspose3d(Cin -> 1, kernel 4, stride 2, padding 1) on 64-wide volumes as a wgmma GEMM over the 64 kernel taps
  * (P[position, tap] = sum_c x[c, position] W[c, tap]) followed by a shared-memory col2im (csrc/convt_c1_col2im.cu).  Replaces the
  * cuDNN call behind the last layer of each decoder (Unet_3D.dec6 networks/networks.py:167-168, VoxelDecoder :57, VoxelGenerator :98).
  *   src0 [B*D][parts*cg0][H][64][8 fp16], src1 likewise (cg1 groups) or NULL; parts 1 (op 1: fp16) | 2 (op 2: hi | lo' split,
@@ -384,7 +384,8 @@ int genre_b200_conv_set_tma(int enable);
 
 /* CTAs per thread-block cluster of the convolution kernels of csrc/convt3d.cu (1 = no clusters, 2, 4 or 8): the CTAs of a cluster
  * walk the same weight sequence, each fetches 1/n of every stage's weights and multicasts it to all of them (cp.async.bulk
- * .multicast::cluster), and a pipeline slot is released by a multicast tcgen05.commit.  Default: GENRE_B200_CONV_CLUSTER or 1.
+ * .multicast::cluster), and a pipeline slot is released once every consumer warp of every CTA of the cluster has arrived on
+ * it (remote mbarrier.arrive).  Default: GENRE_B200_CONV_CLUSTER or 1.
  * Returns the previous setting.  Process-wide. */
 int genre_b200_conv_set_cluster(int ctas);
 

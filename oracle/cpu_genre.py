@@ -1,7 +1,7 @@
 """The reference's CPU path of the GenRe forward (BASELINE configs[2]) — BASELINE INFRASTRUCTURE, see cpu_toolbox/README.md.
 
-build_cpu_genre_net() returns the frozen models/genre_full_model.Net (the reference's file, from baseline/_ref or
-/root/reference) on CPU with
+build_cpu_genre_net() returns the frozen models/genre_full_model.Net (the reference's file, from $GENRE_REF or
+baseline/_ref) on CPU with
     toolbox.*            -> oracle/cpu_toolbox (the CUDA-only ops restated on the CPU oracle, maps in parallel)
     networks.*           -> the reference's own networks/networks.py, uresnet.py, revresnet.py on torch CPU
 Must run in a process that never called genre_shapehd_b200.install() (bench.py --impl reference is such a process).
@@ -26,7 +26,7 @@ def build_cpu_genre_net(ref_root=None):
     from genre_shapehd_b200.synth_genre import init_genre_net_for_bench
     ref_root = ref_root or compat.find_reference()
     if ref_root is None:
-        raise FileNotFoundError("no staged reference callers (baseline/_ref): run __graft_entry__.build() where /root/reference exists")
+        raise FileNotFoundError("no staged reference callers (baseline/_ref): run __graft_entry__.build() where a reference checkout is found")
     sys.path.insert(0, ref_root)                                    # models, util, networks (the reference's own, CPU torch)
     sys.path.insert(0, os.path.join(HERE, "cpu_toolbox"))           # toolbox -> CPU oracle stand-ins
     compat.stub_optional_modules()

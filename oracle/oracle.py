@@ -2,8 +2,8 @@
 unmodified into oracle/_ref/.  TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__.smoke()
 and bench.py's cpu_baseline / --impl reference legs; never by the product package.
 
-Nothing here reads /root/reference at run time (it does not exist on the GPU box); the _ref/*.so files
-are built in the authoring container by oracle/Makefile and travel with the snapshot.
+Nothing here reads the reference checkout at run time; the _ref/*.so files are built by oracle/Makefile where a
+checkout is given (REF / $GENRE_REF) and are optional.
 """
 import ctypes
 import os

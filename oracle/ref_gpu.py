@@ -49,7 +49,7 @@ def _load(name):
     if name not in _libs:
         path = os.path.join(REF_DIR, name)
         if not os.path.exists(path):
-            raise RuntimeError("%s missing: it is built by `make -C oracle` where /root/reference exists" % path)
+            raise RuntimeError("%s missing: it is built by `make -C oracle REF=<GenRe-ShapeHD checkout>`" % path)
         _libs[name] = ctypes.CDLL(path)
     return _libs[name]
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE configs[4] without the two 2D U-ResNets: the GenRe 3D path trained end to end at B=4 on one B200 —
+"""BASELINE configs[4] without the two 2D U-ResNets: the GenRe 3D path trained end to end at B=4 on one H100 —
 depth (leaf that requires grad, standing in for the depth network's output) -> cam_bp -> render_spherical -> sph_pad ->
 backproject_spherical glue -> clamp/cat -> Unet_3D (train mode) -> BCE, backward through every op, SGD step — plus the
 stand-alone Chamfer nndistance forward+backward on [4,N,3] clouds the survey's C5 row asks for (SURVEY.md 8d).

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Unet_3D training step (forward + backward + SGD) at B=4 on one B200 — the 3D part of BASELINE configs[4] (GenRe
+"""Unet_3D training step (forward + backward + SGD) at B=4 on one H100 — the 3D part of BASELINE configs[4] (GenRe
 fine-tune): custom-kernel forward + cuDNN backward (ops_conv._ConvForward) against cuDNN for both."""
 import json, os, sys
 import torch

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Stage-level timing of the cam_bp forward on a B200 (CUDA events, warm, mean of `reps`), next to two ceilings
+"""Stage-level timing of the cam_bp forward on an H100 (CUDA events, warm, mean of `reps`), next to two ceilings
 (cudaMemset / torch fill of the same 256 MiB) and next to the REFERENCE's own kernels built unmodified for
-sm_100a (oracle/_ref, measurement tooling only).  Writes one JSON line; run under gpurun:
-    python profiles/microbench_cam_bp.py > gpurun_out/microbench.json
+sm_90a (oracle/_ref, measurement tooling only).  Writes one JSON line; run on the GPU:
+    python profiles/microbench_cam_bp.py > microbench.json
 """
 import json
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Timing of the tcgen05 ConvTranspose3d kernel against cuDNN on a B200 (CUDA events).  One JSON line.
-    python profiles/microbench_conv.py > gpurun_out/microbench_conv.json
+"""Timing of the tensor-core ConvTranspose3d kernel against cuDNN on an H100 (CUDA events).  One JSON line.
+    python profiles/microbench_conv.py > microbench_conv.json
 """
 import json
 import os

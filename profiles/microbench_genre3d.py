@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GenRe 3D hot path at batch 16 on one B200 (BASELINE configs[2] without the two 2D U-ResNets, which are out of scope):
+"""GenRe 3D hot path at batch 16 on one H100 (BASELINE configs[2] without the two 2D U-ResNets, which are out of scope):
 depth -> cam_bp(+shift) -> render_spherical -> sph_pad -> [inpainting net = identity] -> backproject_spherical glue
 -> clamp/cat -> Unet_3D (eval).  Glue lines are the frozen caller's (depth_pred_with_sph_inpaint.py:120-126,
 genre_full_model.py:120-143).  CUDA events per stage; one JSON line."""

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Device time (CUDA events) of every toolbox op at BASELINE sizes on one B200, next to the REFERENCE's own kernels
-(oracle/_ref, compiled unmodified for sm_100a; measurement tooling) and to the torch composition where the reference
+"""Device time (CUDA events) of every toolbox op at BASELINE sizes on one H100, next to the REFERENCE's own kernels
+(oracle/_ref, compiled unmodified for sm_90a; measurement tooling) and to the torch composition where the reference
 is a torch composition.  One JSON line."""
 import json, os, sys
 import torch

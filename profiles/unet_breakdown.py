@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-block device time of Unet_3D eval forward (B=16) on a B200: which layers matter after dec5."""
+"""Per-block device time of Unet_3D eval forward (B=16) on an H100: which layers matter after dec5."""
 import json, os, sys
 import torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

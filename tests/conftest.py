@@ -13,7 +13,7 @@ genre_shapehd_b200.install()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: pytest -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

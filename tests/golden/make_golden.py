@@ -3,7 +3,7 @@
 
 The reference ships no golden vectors or known-answer tests (SURVEY.md §4, §8c) and its Python packages cannot be
 imported on current PyTorch (they need torch.utils.ffi), so the vectors are produced by running the reference's
-CUDA sources -- compiled UNMODIFIED into oracle/_ref/ behind the THC stand-in (oracle/Makefile) -- on a B200, and
+CUDA sources -- compiled UNMODIFIED into oracle/_ref/ behind the THC stand-in (oracle/Makefile) -- on a GPU, and
 for nndistance additionally by the reference's CPU code (my_lib.c).  Run on the GPU box:
 
     gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'

@@ -1,14 +1,19 @@
 """bench.py's reference arm runs on host cores only, so its JSON line can be checked without a GPU: one line, the keys
-the driver reads, the metric/config of BASELINE.json configs[2] (GenRe full_model inference through the frozen Net.forward,
-here on the CPU oracle toolbox + the reference's networks), and the tier's `cpu_baseline` / `e2e` shape."""
+a consumer reads, the metric/config of BASELINE.json configs[2] (GenRe full_model inference through the frozen Net.forward,
+here on the CPU oracle toolbox + the reference's networks), and the `cpu_baseline` / `e2e` shape.  The arm runs the
+reference's own model files, which are not part of this repository: it needs a GenRe-ShapeHD checkout ($GENRE_REF)."""
 import json
 import os
 import subprocess
 import sys
 
+import pytest
+
 from conftest import REPO
+from genre_shapehd_b200 import compat
 
 
+@pytest.mark.skipif(compat.find_reference() is None, reason="no GenRe-ShapeHD checkout ($GENRE_REF)")
 def test_reference_arm_prints_one_contract_line():
     env = dict(os.environ, RANK="0", WORLD_SIZE="1")
     p = subprocess.run([sys.executable, os.path.join(REPO, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "0",

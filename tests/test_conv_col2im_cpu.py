@@ -9,7 +9,8 @@ import torch.nn.functional as F
 
 from genre_shapehd_b200 import ops_conv
 
-ROWS, W, UY, PITCH = 8, 64, 18, 136
+ROWS, W, PITCH = 2, 64, 136
+UY = 2 * ROWS + 2
 PLANE = UY * PITCH
 
 
@@ -31,8 +32,8 @@ def emulate(sources, segments, weight, bias):
     nbands = h // ROWS
     pairs = b * do * nbands - 1
     if nbands > 1:
-        for k in range(pairs):                                                               # cudaMemset2DAsync(out + 15 Wo, pitch 16 rows, 2 rows, pairs)
-            flat[15 + 16 * k: 17 + 16 * k] = 0.0
+        for k in range(pairs):                                       # cudaMemset2DAsync(out + (2 ROWS - 1) Wo, pitch 2 ROWS rows, 2 rows, pairs)
+            flat[2 * ROWS - 1 + 2 * ROWS * k: 2 * ROWS + 1 + 2 * ROWS * k] = 0.0
     for bi in range(b):
         for band in range(nbands):
             y0 = band * ROWS
@@ -53,8 +54,8 @@ def emulate(sources, segments, weight, bias):
                     else:
                         out[bi, oz, oy] = v
             for z in range(d):
-                pos = a[bi, :, z, y0:y0 + ROWS, :].reshape(-1, ROWS * W)                     # [K, 512], position = y*64 + x
-                p = pos.T @ wmat                                                             # [512, 64]
+                pos = a[bi, :, z, y0:y0 + ROWS, :].reshape(-1, ROWS * W)                     # [K, ROWS*64], position = y*64 + x
+                p = pos.T @ wmat                                                             # [ROWS*64, 64]
                 zs = (2 * z) & 3
                 for t in range(8):
                     tz, ty, tx = (t >> 2) & 1, (t >> 1) & 1, t & 1

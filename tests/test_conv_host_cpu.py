@@ -1,4 +1,4 @@
-"""Host side of the tcgen05 convolution path on CPU: the weight packers and layout transforms of
+"""Host side of the tensor-core convolution path on CPU: the weight packers and layout transforms of
 genre_shapehd_b200/ops_conv.py define, together with the kernel's tap geometry (csrc/convt3d.cu: input = j + base - t),
 a plain sum of shifted matrix products.  That sum is emulated here in torch and compared with torch's own
 conv_transpose3d / conv3d (networks/networks.py:40-57,151-167 layers), so a packing bug is caught without a GPU."""

@@ -1,4 +1,4 @@
-"""Golden vectors produced by the REFERENCE's own kernels (tests/golden/make_golden.py, run on a B200 against
+"""Golden vectors produced by the REFERENCE's own kernels (tests/golden/make_golden.py, run on a GPU against
 oracle/_ref = the reference .cu/.c files compiled unmodified).
 
 CPU part  : pins the ORACLE to the reference -- indices / counts bit-exact, values within float-atomic noise.

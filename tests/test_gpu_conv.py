@@ -1,4 +1,4 @@
-"""tcgen05 ConvTranspose3d kernel (csrc/convt3d.cu) against torch's fp32 conv_transpose3d (TF32 off)."""
+"""Tensor-core ConvTranspose3d kernel (csrc/convt3d.cu) against torch's fp32 conv_transpose3d (TF32 off)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -1,4 +1,4 @@
-"""The small-volume k4 s2 convolutions on the flattened-volume tcgen05 kernel (csrc/convflat.cu) against torch's fp32
+"""The small-volume k4 s2 convolutions on the flattened-volume wgmma kernel (csrc/convflat.cu) against torch's fp32
 convolutions (TF32 off): Unet_3D.enc4 / enc5 / dec2 / dec3 (networks/networks.py:157-165) and the 4^3 / 8^3 stages of the
 ShapeHD nets."""
 from contextlib import contextmanager

@@ -8,7 +8,8 @@ What it does:
   * genre_shapehd_b200.install(reference_root): toolbox / nndistance / networks resolve HERE, everything else
     (models, util, loggers, visualize, datasets, options, networks.uresnet/revresnet) in the reference checkout;
   * stubs the optional third-party modules the frozen files import at module level but never use on the
-    differentiable path (skimage, trimesh; visualize/visualizer.py:8, util/util_sph.py:1-3);
+    differentiable path (skimage, trimesh; visualize/visualizer.py:8, util/util_sph.py:1-3); the stub's
+    skimage.measure.marching_cubes_lewiner / marching_cubes run postprocess.marching_cubes on the GPU;
   * makes torchvision's resnet18(pretrained=True) build offline (random init) — there is no network here.
 """
 import os
@@ -38,6 +39,22 @@ def _unavailable(what):
     return f
 
 
+def marching_cubes_numpy(volume, level, spacing=(1.0, 1.0, 1.0)):
+    """Stand-in for skimage.measure.marching_cubes_lewiner / marching_cubes where skimage is absent: numpy [D,H,W] in,
+    (verts [V,3] float32, faces [F,3] int32, None, None) out, computed by postprocess.marching_cubes on the current CUDA
+    device in float32.  The frozen callers (visualize/visualizer.py:160, util/util_sph.py:47) discard skimage's normals and
+    values, so they are not computed.  The triangulation is not Lewiner's (see marching_cubes); the vertices are those of
+    any linear-interpolation marching cubes."""
+    import numpy as np
+    import torch
+    from .postprocess import marching_cubes
+    vol = torch.from_numpy(np.ascontiguousarray(volume, dtype=np.float32)).cuda()
+    if vol.dim() != 3:
+        raise ValueError("marching_cubes expects a 3D volume, got shape %s" % (tuple(vol.shape),))
+    verts, faces, _, _ = marching_cubes(vol[None], level, spacing=spacing)
+    return verts.cpu().numpy(), faces.cpu().numpy(), None, None
+
+
 def find_reference():
     """the frozen callers: $GENRE_REF, else the copy __graft_entry__.build() staged into <repo>/baseline/_ref"""
     for root in (os.environ.get("GENRE_REF"), os.path.join(genre_shapehd_b200.REPO_ROOT, "baseline", "_ref")):
@@ -62,8 +79,7 @@ def stub_optional_modules(offline_resnet=True):
     an offline torchvision resnet18"""
     sk = _stub("skimage")
     if getattr(sk, "__genre_b200_stub__", False):
-        measure = _stub("skimage.measure", marching_cubes_lewiner=_unavailable("skimage.measure.marching_cubes"),
-                        marching_cubes=_unavailable("skimage.measure.marching_cubes"))
+        measure = _stub("skimage.measure", marching_cubes_lewiner=marching_cubes_numpy, marching_cubes=marching_cubes_numpy)
         sk.measure = measure
         _stub("skimage.io", imread=_unavailable("skimage.io.imread"), imsave=_unavailable("skimage.io.imsave"))
         _stub("skimage.transform", resize=_unavailable("skimage.transform.resize"))

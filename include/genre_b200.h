@@ -420,6 +420,34 @@ size_t genre_b200_voxel_surface_workspace_bytes(int64_t N, int res);
 int genre_b200_voxel_surface(const float *vox, int64_t N, int res, int iterations, int transpose_flip, float *out,
                              void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Batched marching cubes (SURVEY 8f-3).  Replaces skimage.measure.marching_cubes_lewiner(df, th, spacing=...) in
+ * Visualizer._save_iso_obj (visualize/visualizer.py:160) and util_sph.py:47, for a batch resident on the device.
+ *   vol     [N, D, H, W] dense fp32; 2 <= D, H, W <= 512, 1 <= N <= 65535.  A point is inside iff v > level (NaN: outside).
+ *   vertices: one per grid edge with ends on different sides; point p owns its edges to p+e0, p+e1, p+e2.  For the edge from p
+ *             (value v0) to q (value v1) along axis a: t = fl(fl(level - v0) / fl(v1 - v0)),
+ *             x_a = fl(fl(fl(p_a + t) * spacing_a) - shift_a), x_b = fl(fl(p_b * spacing_b) - shift_b) for the other axes
+ *             (one rounding per step, no FMA).  Axis 0 is the first array axis (skimage's convention).
+ *             Order: sample, point index (i*H + j)*W + k, axis.
+ *   faces:    per-cell segment linking with the asymptotic decider on ambiguous faces (inside corners a, d on a diagonal
+ *             are joined iff fl(a'*d') > fl(b'*c'), x' = fl(x - level)); loops fanned as (v0, v_i, v_{i+1}).  Interior
+ *             ambiguities (Lewiner's tunnel cases) are not resolved; the triangles are not skimage's.  Counter-clockwise
+ *             seen from the <= level side.  Order: sample, cell index, loop (by smallest local edge id 4a + 2*ob + oc),
+ *             fan position.  int32 indices into the sample's own vertex block.
+ *             The full rules are in csrc/isosurface.cu; oracle_iso/isosurface_oracle.c restates them bit for bit.
+ * Output sizes depend on the data, so there are two calls and the caller allocates between them:
+ *   count: counts [N, 2] int64 (vertices, faces) on the device; per-tile offsets stay in the workspace.
+ *   emit:  vert_off, face_off [N+1] int64 on the device, the exclusive prefix sums of counts[:, 0] and counts[:, 1];
+ *          verts [sum V, 3] fp32, faces [sum F, 3] int32.  Same vol, level and workspace as the count call, untouched in between.
+ *   workspace: genre_b200_isosurface_workspace_bytes(N, D, H, W) bytes (0: unsupported shape), 16-byte aligned, caller-owned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_isosurface_workspace_bytes(int64_t N, int D, int H, int W);
+int genre_b200_isosurface_count(const float *vol, int64_t N, int D, int H, int W, float level, int64_t *counts,
+                                void *workspace, size_t workspace_bytes, void *stream);
+int genre_b200_isosurface_emit(const float *vol, int64_t N, int D, int H, int W, float level, float sx, float sy, float sz,
+                               float shx, float shy, float shz, const int64_t *vert_off, const int64_t *face_off, float *verts,
+                               int32_t *faces, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,10 @@ What it does:
     (models, util, loggers, visualize, datasets, options, networks.uresnet/revresnet) in the reference checkout;
   * stubs the optional third-party modules the frozen files import at module level but never use on the
     differentiable path (skimage, trimesh; visualize/visualizer.py:8, util/util_sph.py:1-3); the stub's
-    skimage.measure.marching_cubes_lewiner / marching_cubes run postprocess.marching_cubes on the GPU;
+    skimage.measure.marching_cubes_lewiner / marching_cubes run postprocess.marching_cubes on the GPU, and the stub's
+    trimesh.Trimesh(...).ray.intersects_id runs postprocess.raycast, so util_sph.render_spherical (the published test path,
+    forward_with_trimesh) runs unchanged;
+  * where scipy.misc.imresize is gone (scipy >= 1.3), installs a stand-in for the one call util_camera makes;
   * makes torchvision's resnet18(pretrained=True) build offline (random init) — there is no network here.
 """
 import os
@@ -55,6 +58,59 @@ def marching_cubes_numpy(volume, level, spacing=(1.0, 1.0, 1.0)):
     return verts.cpu().numpy(), faces.cpu().numpy(), None, None
 
 
+class _RayIntersector:
+    def __init__(self, mesh):
+        self.mesh = mesh
+
+    def intersects_id(self, ray_origins, ray_directions, multiple_hits=True, max_hits=20, return_locations=False):
+        """trimesh's RayMeshIntersector.intersects_id with multiple_hits=False: the closest hit of every ray (postprocess.raycast
+        on the current CUDA device, fp32).  Returns (index_tri, index_ray[, locations]) for the rays that hit, as int64 /
+        float64 numpy arrays."""
+        import numpy as np
+        import torch
+        from .postprocess import raycast
+        if multiple_hits:
+            raise NotImplementedError("the trimesh stand-in returns the first hit only (multiple_hits=False)")
+        o = np.asarray(ray_origins, dtype=np.float64).reshape(-1, 3)
+        d = np.asarray(ray_directions, dtype=np.float64).reshape(-1, 3)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        v = torch.from_numpy(np.ascontiguousarray(self.mesh.vertices, dtype=np.float32).reshape(-1, 3)).to(dev)
+        f = torch.from_numpy(np.ascontiguousarray(self.mesh.faces, dtype=np.int32).reshape(-1, 3)).to(dev)
+        vo = torch.tensor([0, len(v)], dtype=torch.int64, device=dev)
+        fo = torch.tensor([0, len(f)], dtype=torch.int64, device=dev)
+        t, face = raycast(v, f, vo, fo, torch.from_numpy(o).float().to(dev)[None], torch.from_numpy(d).float().to(dev)[None])
+        t, face = t[0].cpu().numpy().astype(np.float64), face[0].cpu().numpy().astype(np.int64)
+        index_ray = np.nonzero(face >= 0)[0]
+        index_tri = face[index_ray]
+        if not return_locations:
+            return index_tri, index_ray
+        d32 = d.astype(np.float32).astype(np.float64)
+        return index_tri, index_ray, o[index_ray] + t[index_ray, None] * d32[index_ray]
+
+
+class Trimesh:
+    """Stand-in for trimesh.Trimesh(vertices=, faces=) where trimesh is absent: holds the arrays; ``.ray.intersects_id``
+    casts rays on the GPU (first hit only)."""
+
+    def __init__(self, vertices=None, faces=None, **kwargs):
+        import numpy as np
+        self.vertices = np.asarray(vertices, dtype=np.float64).reshape(-1, 3)
+        self.faces = np.asarray(faces, dtype=np.int64).reshape(-1, 3)
+        self.ray = _RayIntersector(self)
+
+
+def imresize(arr, size, interp="bilinear", mode=None):
+    """Stand-in for scipy.misc.imresize (removed in scipy 1.3) covering the one call the frozen code makes
+    (util/util_camera.py:120-121): mode='F' at the same size, which returns the array as float32.  Anything else raises."""
+    import numpy as np
+    arr = np.asarray(arr)
+    same = (isinstance(size, float) and size == 1.0) or (isinstance(size, tuple) and tuple(size) == arr.shape)
+    if mode != "F" or arr.ndim != 2 or not same:
+        raise NotImplementedError("imresize stand-in: only mode='F' at the same size is supported (got mode=%r, size=%r, "
+                                  "shape %s)" % (mode, size, arr.shape))
+    return arr.astype(np.float32)
+
+
 def find_reference():
     """the frozen callers: $GENRE_REF, else the copy __graft_entry__.build() staged into <repo>/baseline/_ref"""
     for root in (os.environ.get("GENRE_REF"), os.path.join(genre_shapehd_b200.REPO_ROOT, "baseline", "_ref")):
@@ -71,12 +127,31 @@ def bootstrap(reference_root=None, offline_resnet=True):
     os.environ["GENRE_REF"] = root
     genre_shapehd_b200.install(root)
     stub_optional_modules(offline_resnet)
+    _patch_tsdf_renderer()
     return root
 
 
+def _patch_tsdf_renderer():
+    """util_camera.tsdf_renderer.check_valid (util/util_camera.py:164-174) starts with `self.depth == []`, which numpy 1 answered
+    with False for a depth array and numpy >= 2 refuses; the same test by size keeps depth_to_mesh_df running.  The method
+    returns True for every non-empty map either way (its resolution check only prints)."""
+    try:
+        import util.util_camera as uc
+    except ImportError:     # numba or the reference checkout missing: the test path cannot run anyway
+        return
+
+    def check_valid(self, warning=True):
+        import numpy as np
+        if np.size(self.depth) == 0:
+            print('No depth map available!')
+            return False
+        return True
+    uc.tsdf_renderer.check_valid = check_valid
+
+
 def stub_optional_modules(offline_resnet=True):
-    """stand-ins for skimage / trimesh (imported at module level by the frozen files, unused on the differentiable path) and
-    an offline torchvision resnet18"""
+    """stand-ins for skimage / trimesh (imported at module level by the frozen files) and scipy.misc.imresize, and an offline
+    torchvision resnet18"""
     sk = _stub("skimage")
     if getattr(sk, "__genre_b200_stub__", False):
         measure = _stub("skimage.measure", marching_cubes_lewiner=marching_cubes_numpy, marching_cubes=marching_cubes_numpy)
@@ -85,8 +160,16 @@ def stub_optional_modules(offline_resnet=True):
         _stub("skimage.transform", resize=_unavailable("skimage.transform.resize"))
     tm = _stub("trimesh")
     if getattr(tm, "__genre_b200_stub__", False):
-        tm.Trimesh = _unavailable("trimesh.Trimesh")
+        tm.Trimesh = Trimesh
         tm.load = _unavailable("trimesh.load")
+    import scipy
+    try:
+        import scipy.misc as misc
+    except ImportError:
+        misc = _stub("scipy.misc")
+        scipy.misc = misc
+    if not hasattr(misc, "imresize"):
+        misc.imresize = imresize
     if offline_resnet:
         import torchvision.models as tvm
         if not getattr(tvm.resnet18, "__genre_b200_offline__", False):

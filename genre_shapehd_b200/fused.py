@@ -22,6 +22,8 @@ from genre_shapehd_b200 import _lib
 from toolbox.cam_bp.cam_bp.modules.camera_backprojection_module import Camera_back_projection_layer
 from toolbox.spherical_proj import gen_sph_grid, render_forward, render_spherical, sph_pad
 
+from genre_shapehd_b200.postprocess import spherical_from_depth
+
 
 class GenRe3DGlue(torch.nn.Module):
     def __init__(self, res=128, sph_res=128, z_res=256, margin=16, scale=50.0, lo=1e-5, hi=1 - 1e-5):
@@ -68,9 +70,9 @@ def genre_forward_fused(net, input_struct, glue=None):
     """Batched, mesh-free GenRe inference: the same tensors as the frozen ``Net.forward`` (models/genre_full_model.py:116-132;
     same keys, same values up to rounding) with the 3D glue of the callers folded into the kernels (``GenRe3DGlue``).
 
-    It also stands in for the published test path ``Model.forward_with_trimesh`` (genre_full_model.py:202-233), which renders the
-    spherical map on the CPU through marching cubes + trimesh ray casting (util_sph.py:36-57), needs batch size 1 and is not
-    differentiable: here the spherical map comes from the differentiable renderer, for any batch, on the device (SURVEY 8f-4).
+    Its partial spherical map comes from the differentiable voxel renderer, as in ``Net.forward``.  The published test path
+    ``Model.forward_with_trimesh`` renders that map differently (marching cubes + mesh ray casting, util_sph.py:36-57), so
+    its values differ; ``genre_forward_trimesh`` is the batched form of that path.
 
     net: models.genre_full_model.Net (reference class, unmodified), eval mode.  Returns the dict of Net.forward."""
     dn = net.depth_and_inpaint
@@ -90,4 +92,32 @@ def genre_forward_fused(net, input_struct, glue=None):
     out["pred_proj_sph_full"] = refine_input[:, 0:1]
     out["pred_proj_depth"] = refine_input[:, 1:2]
     out["pred_voxel"] = net.refine_net(refine_input)
+    return out
+
+
+@torch.no_grad()
+def genre_forward_trimesh(net, input_struct, grid=None):
+    """The published test path ``Model.forward_with_trimesh`` (models/genre_full_model.py:202-233) for any batch size, on the
+    device: the same keys, transposes and flips, with the partial spherical map of ``util_sph.render_spherical`` (480^2
+    depth -> TDF -> marching cubes -> first-hit ray casting) computed by ``postprocess.spherical_from_depth`` instead of
+    one sample at a time on the CPU.  The projection is the net's own cam_bp layer, as in ``GenRe3DGlue.project_and_render``.
+
+    net: models.genre_full_model.Net (reference class, unmodified), eval mode; input_struct with .rgb and .silhou.
+    Returns forward_with_trimesh's dict: net1's outputs plus pred_sph_full, pred_sph_partial, pred_proj_depth, pred_voxel
+    and pred_proj_sph_full."""
+    dn = net.depth_and_inpaint
+    out = dn.net1(input_struct)
+    proj = dn.proj_depth(dn.get_abs_depth(out, input_struct))
+    pred_depth = dn.base_class.postprocess(out["depth"].detach())
+    silhou = net.base_class.postprocess(input_struct.silhou).detach()
+    sph_partial = sph_pad(spherical_from_depth(pred_depth, out["depth_minmax"].detach(), silhou, grid))
+    out2 = dn.net2(sph_partial)
+    pred_proj_sph = torch.flip(torch.transpose(net.backproject_spherical(out2["spherical"]), 3, 4), [3])
+    proj = torch.flip(torch.transpose(proj, 3, 4), [3])
+    pred_voxel = net.refine_net(torch.cat((pred_proj_sph, proj), dim=1))
+    out["pred_sph_full"] = out2["spherical"]
+    out["pred_sph_partial"] = sph_partial
+    out["pred_proj_depth"] = proj
+    out["pred_voxel"] = pred_voxel.flip([3]).transpose(3, 4)
+    out["pred_proj_sph_full"] = pred_proj_sph
     return out

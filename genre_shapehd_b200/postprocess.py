@@ -5,6 +5,10 @@ the device: the reference runs ``scipy.ndimage.binary_erosion`` on every sample 
 
 ``marching_cubes`` / ``write_obj`` / ``save_iso_objs`` turn predicted voxel grids into meshes and ``.obj`` files, the job of
 ``skimage.measure.marching_cubes_lewiner`` and ``Visualizer._save_iso_obj`` (visualize/visualizer.py:138-205) in the reference.
+
+``raycast`` / ``render_mesh_spherical`` / ``spherical_from_depth`` are the partial spherical map of the published test path
+(``util_sph.render_spherical``, util/util_sph.py:36-57: depth -> TDF -> marching cubes -> trimesh ray casting), batched on
+the device.
 """
 import numpy as np
 import torch
@@ -143,3 +147,145 @@ def save_iso_objs(voxels, output_pattern, counter=0, th=0.25, use_sigmoid=True, 
         write_obj(path, verts[vo[b]:vo[b + 1]], faces[fo[b]:fo[b + 1]])
         paths.append(path)
     return paths
+
+
+# cells per axis of raycast's uniform grid (the result does not depend on it): the fastest whole count + build + first_hit of
+# profiles/microbench_raycast.py over 32 / 64 / 128 (DESIGN §4.2)
+RAYCAST_GRID = 32
+
+
+def raycast(verts, faces, vert_off, face_off, origins, dirs, grid=None):
+    """First hit of every ray on every sample's triangle mesh, on the device.
+
+    verts [V,3] fp32, faces [F,3] int32 (indices into the sample's own vertex block), vert_off / face_off [B+1] int64: the
+    packed meshes ``marching_cubes`` returns.  origins, dirs [B|1, R, 3] fp32: one table per sample, or one shared by all.
+    Returns (t [B,R] fp32, face [B,R] int32): the ray parameter of the closest hit (the distance when |dir| = 1) and the hit
+    face, local to the sample, ties to the smallest index; +inf and -1 on a miss.  The test is two-sided and watertight (a ray
+    through an edge or a vertex of a closed mesh does not slip through), zero-area faces never hit, and the result equals a
+    loop over all faces bit for bit (oracle_ray/), whatever ``grid`` (cells per axis of the acceleration grid, 1..256).
+
+    The number of grid references depends on the data: it is copied to the host once (a device synchronisation) before the
+    reference list is allocated, so the call cannot be captured in a CUDA graph."""
+    _lib.require_cuda(verts, faces, vert_off, face_off, origins, dirs)
+    _lib.require_f32(verts, origins, dirs)
+    if faces.dtype != torch.int32 or vert_off.dtype != torch.int64 or face_off.dtype != torch.int64:
+        raise TypeError("raycast expects int32 faces and int64 offsets, got %s, %s, %s" % (faces.dtype, vert_off.dtype,
+                                                                                          face_off.dtype))
+    n = vert_off.numel() - 1
+    if n < 1 or face_off.numel() != n + 1 or verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("raycast: verts [V,3], faces [F,3] and offsets [B+1] expected, got %s, %s, %s, %s"
+                         % (tuple(verts.shape), tuple(faces.shape), tuple(vert_off.shape), tuple(face_off.shape)))
+    if origins.shape != dirs.shape or origins.dim() != 3 or origins.shape[2] != 3 or origins.shape[0] not in (1, n):
+        raise ValueError("raycast: origins and dirs [B|1, R, 3] expected with B = %d, got %s and %s"
+                         % (n, tuple(origins.shape), tuple(dirs.shape)))
+    g = RAYCAST_GRID if grid is None else int(grid)
+    lib = _lib.load()
+    nbytes = lib.genre_b200_raycast_workspace_bytes(n, g)
+    if nbytes == 0:
+        raise ValueError("raycast: %d meshes with a %d^3 grid unsupported (1 <= B <= 65535, 1 <= grid <= 256)" % (n, g))
+    dev = verts.device
+    stream = _lib.stream_ptr(verts)
+    r = origins.shape[1]
+    verts, faces, vert_off, face_off = verts.contiguous(), faces.contiguous(), vert_off.contiguous(), face_off.contiguous()
+    o, d = origins.contiguous(), dirs.contiguous()
+    mesh = (verts.data_ptr(), verts.shape[0], faces.data_ptr(), faces.shape[0], vert_off.data_ptr(), face_off.data_ptr(), n, g)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    refs = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.call("genre_b200_raycast_count", *mesh, refs.data_ptr(), ws.data_ptr(), nbytes, stream)
+    ref_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+    ref_off[1:] = torch.cumsum(refs, 0)
+    ref_ids = torch.empty(int(ref_off[-1]), dtype=torch.int32, device=dev)
+    _lib.call("genre_b200_raycast_build", *mesh, ref_off.data_ptr(), ref_ids.data_ptr(), ws.data_ptr(), nbytes, stream)
+    t = torch.empty((n, r), dtype=torch.float32, device=dev)
+    face = torch.empty((n, r), dtype=torch.int32, device=dev)
+    if r > 0:
+        _lib.call("genre_b200_raycast_first_hit", *mesh, ref_off.data_ptr(), ref_ids.data_ptr(), o.data_ptr(), d.data_ptr(), r,
+                  0 if o.shape[0] == 1 else 3 * r, t.data_ptr(), face.data_ptr(), ws.data_ptr(), nbytes, stream)
+    return t, face
+
+
+_SPH_RAYS = {}
+
+
+def _sph_rays(sph_res, device):
+    """make_sgrid(sph_res / 2) (util_sph.py:21-33) as fp32 ray origins on the unit sphere and directions towards the centre"""
+    key = (sph_res, str(device))
+    if key not in _SPH_RAYS:
+        from toolbox.spherical_proj import _sph_dirs   # the same table as gen_sph_grid (spherical_proj.py:6-16)
+        sgrid = _sph_dirs(sph_res).reshape(1, -1, 3)
+        _SPH_RAYS[key] = (torch.from_numpy(sgrid).float().to(device), torch.from_numpy(-sgrid).float().to(device))
+    return _SPH_RAYS[key]
+
+
+def render_mesh_spherical(verts, faces, vert_off, face_off, sph_res=128, grid=None):
+    """util_sph.render_model + its reshape and clamp (util_sph.py:7-18, 51-53) for a batch of packed meshes: the distance
+    from each point of the make_sgrid(sph_res / 2) table on the unit sphere to the first hit of the ray towards the centre,
+    1 where the ray misses, values above 1 set to 1.  Returns [B, sph_res, sph_res] fp32."""
+    o, d = _sph_rays(sph_res, verts.device)
+    t, _ = raycast(verts, faces, vert_off, face_off, o, d, grid)
+    dist = t * torch.linalg.vector_norm(d[0], dim=1)
+    return torch.clamp(dist, max=1.0).view(-1, sph_res, sph_res)   # +inf (a miss) -> 1
+
+
+# util_img.depth_to_mesh_df's camera (util/util_img.py:53-89): 480 x 480 pixels, focal length 0.05 on a 0.0306 sensor, at
+# (-2.2, 0, 0) looking along +x
+SPH_DEPTH_RES = 480
+SPH_FL = 0.05 / (0.03059411708155671 / SPH_DEPTH_RES)   # 784.4645406 pixels
+SPH_CAM_DIST = 2.2
+
+
+def resize_bicubic(x, size):
+    """[B,C,H,W] -> [B,C,size,size] with torch's bicubic (align_corners=False), the step util_img.resize takes with
+    cv2.INTER_CUBIC.  The two differ by up to 3.4e-5 on U(0,1) data at 256 -> 480 (tests/test_raycast_cpu.py bounds it at 5e-5)."""
+    return torch.nn.functional.interpolate(x, size=(size, size), mode="bicubic", align_corners=False)
+
+
+def spherical_from_depth(depth, depth_minmax, silhou, grid=None):
+    """The batched util_sph.render_spherical (util/util_sph.py:36-57), all on the device.
+
+    depth [B,1,H,W] (the network's relative depth after postprocess), depth_minmax [B,2], silhou [B,1,H,W], fp32 on CUDA.
+      1. both maps go to 480 x 480 (``resize_bicubic``); depth pixels where the resized silhouette is not > 0.95 become 0;
+      2. abs = (1 - d) * (max - min) + min (no +1e-4, unlike to_abs_depth), rounded as the reference rounds it (fp64, then the
+         fp32 of imresize(mode='F')); pixels with d == 0 are skipped;
+      3. depth_to_mesh_df's TDF: cam_bp_forward at fl = 784.4645406 px, cam_dist 2.2, unshifted.  The reference's point of pixel
+         (h, w) is cam_bp's point of pixel (479 - w, h), so cam_bp reads the depth through the view D'[h'][w'] = D[w'][479 - h']
+         (a negative stride, no copy), and its [ix][iy][iz] volume is already the reference's [x][y][z] (no permutation);
+      4. marching_cubes(tdf, 0.999/128, spacing 1/128, shift 0.5): grid point i sits at i/128 - 0.5, half a voxel off the
+         voxel centres, as in the reference;
+      5. render_mesh_spherical.
+    Returns [B,1,128,128] fp32.  An empty silhouette gives an all-ones map, as the reference's except branch does."""
+    _lib.require_cuda(depth, depth_minmax, silhou)
+    _lib.require_f32(depth, depth_minmax, silhou)
+    if depth.dim() != 4 or depth.shape[1] != 1 or silhou.shape != depth.shape or tuple(depth_minmax.shape) != (depth.shape[0], 2):
+        raise ValueError("spherical_from_depth expects depth, silhou [B,1,H,W] and depth_minmax [B,2], got %s, %s, %s"
+                         % (tuple(depth.shape), tuple(silhou.shape), tuple(depth_minmax.shape)))
+    tdf = _tdf_480(_abs_depth_480(depth, depth_minmax, silhou))
+    verts, faces, vo, fo = marching_cubes(tdf, 0.999 / 128, spacing=(1 / 128,) * 3, shift=(0.5,) * 3)
+    return render_mesh_spherical(verts, faces, vo, fo, 128, grid)[:, None]
+
+
+def _abs_depth_480(depth, depth_minmax, silhou):
+    """steps 1-2 of spherical_from_depth: the gated 480^2 absolute depth, -1 on skipped pixels"""
+    res = SPH_DEPTH_RES
+    b = depth.shape[0]
+    d = resize_bicubic(depth, res)
+    d = torch.where(resize_bicubic(silhou, res) > 0.95, d, torch.zeros_like(d))
+    mn, mx = depth_minmax[:, 0], depth_minmax[:, 1]
+    scale = (mx - mn).double().view(b, 1, 1, 1)
+    absd = ((1 - d.double()) * scale + mn.double().view(b, 1, 1, 1)).float()
+    return torch.where(d == 0, torch.full_like(absd, -1.0), absd).contiguous()
+
+
+def _tdf_480(absd):
+    """step 3 of spherical_from_depth: cam_bp_forward through the view D'[h'][w'] = D[w'][479 - h'] -> [B,1,128,128,128]"""
+    b, res = absd.shape[0], absd.shape[-1]
+    dev = absd.device
+    sN, sC, sH, sW = absd.stride()
+    fl = torch.full((b, 1), SPH_FL, dtype=torch.float32, device=dev)
+    cd = torch.full((b, 1), SPH_CAM_DIST, dtype=torch.float32, device=dev)
+    tdf = torch.empty((b, 1, 128, 128, 128), dtype=torch.float32, device=dev)
+    ws, nbytes = _lib.workspace_for(b, res * res, 128, dev)
+    _lib.call("genre_b200_cam_bp_forward", absd.data_ptr() + 4 * (res - 1) * sW, b, 1, res, res, sN, sC, -sW, sH,
+              fl.data_ptr(), *fl.stride(), cd.data_ptr(), *cd.stride(), tdf.data_ptr(), None, 128, 0, ws.data_ptr(), nbytes,
+              _lib.stream_ptr(absd))
+    return tdf

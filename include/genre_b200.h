@@ -448,6 +448,40 @@ int genre_b200_isosurface_emit(const float *vol, int64_t N, int D, int H, int W,
                                float shx, float shy, float shz, const int64_t *vert_off, const int64_t *face_off, float *verts,
                                int32_t *faces, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * First-hit ray casting of batched triangle meshes (SURVEY 8f-4).  Replaces trimesh's
+ * mesh.ray.intersects_id(origins, dirs, multiple_hits=False) in util_sph.render_model (util/util_sph.py:7-18), one mesh per
+ * sample, for a batch resident on the device.
+ *   meshes  the packed output of genre_b200_isosurface_*: verts [V, 3] fp32 (finite), faces [F, 3] int32 indexing the sample's
+ *           own vertex block, vert_off / face_off [N+1] int64 on the device (exclusive prefix sums; V, F the totals).
+ *   rays    origins, dirs [N|1, R, 3] fp32; ray_batch_stride = 3*R (per-sample rays) or 0 (one table shared by the batch).
+ *           A ray with a non-finite component or a zero direction misses.
+ *   hit     a face is DEGENERATE iff fl(fl(v1 - v0) x fl(v2 - v0)) is the zero vector; degenerate faces never hit.  Otherwise
+ *           the two-sided watertight test of Woop, Benthin and Wald (2013) in fp32, one rounding per step, as spelled out in
+ *           csrc/raycast.cu: kz = argmax |d| (lowest axis on ties), shear by d_kx/d_kz, d_ky/d_kz, 1/d_kz, edge functions
+ *           U, V, W, det = (U+V)+W, T = (U*Az + V*Bz) + W*Cz, t = T/det; a hit iff the edge functions do not have mixed
+ *           signs, det != 0 and 0 < t < inf.
+ *   result  t [N, R] fp32 and face [N, R] int32 (local to the sample): the hit with the smallest t, ties to the smallest face
+ *           index; +inf and -1 on a miss.  Equal, bit for bit, to a loop over all of the sample's faces for every G
+ *           (the argument is in csrc/raycast.cu); oracle_ray/raycast_oracle.c is that loop.
+ * Three calls; the caller owns every buffer, the library never synchronises:
+ *   count:     refs [N] int64 on the device, the number of (cell, face) references of each sample's uniform G^3 grid.
+ *   build:     ref_off [N+1] int64 on the device, the exclusive prefix sums of refs; ref_ids [sum refs] int32.
+ *   first_hit: writes t and face.  Same meshes, G and workspace in all three calls, untouched in between.
+ *   G in [1, 256], N in [1, 65535]; workspace: genre_b200_raycast_workspace_bytes(N, G) bytes (0: unsupported), 16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_raycast_workspace_bytes(int64_t N, int G);
+int genre_b200_raycast_count(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                             const int64_t *face_off, int64_t N, int G, int64_t *refs, void *workspace,
+                             size_t workspace_bytes, void *stream);
+int genre_b200_raycast_build(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                             const int64_t *face_off, int64_t N, int G, const int64_t *ref_off, int32_t *ref_ids,
+                             void *workspace, size_t workspace_bytes, void *stream);
+int genre_b200_raycast_first_hit(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                                 const int64_t *face_off, int64_t N, int G, const int64_t *ref_off, const int32_t *ref_ids,
+                                 const float *origins, const float *dirs, int64_t R, int64_t ray_batch_stride, float *t,
+                                 int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

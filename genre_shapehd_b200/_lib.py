@@ -20,6 +20,7 @@ _uint = ctypes.c_uint
 _ptr = ctypes.c_void_p
 _size = ctypes.c_size_t
 _f32 = ctypes.c_float
+_f64 = ctypes.c_double
 
 # name -> argument types, in include/genre_b200.h order
 _SIGNATURES = {
@@ -80,6 +81,11 @@ _SIGNATURES = {
     "genre_b200_raycast_build": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_raycast_first_hit": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _ptr, _ptr, _ptr, _ptr, _i64, _i64, _ptr,
                                      _ptr, _ptr, _size, _ptr],
+    "genre_b200_voxel_fill": [_ptr, _i64, _int, _int, _int, _f32, _int, _ptr, _ptr, _size, _ptr],
+    "genre_b200_voxel_transform": [_ptr, _i64, _int, _int, _int, _ptr, _uint, _f64, _f64, _f64, _ptr, _ptr],
+    "genre_b200_voxel_stats": [_ptr, _ptr, _i64, _int, _int, _int, _int, _int, _f64, _f64, _ptr, _ptr, _ptr],
+    "genre_b200_voxel_downsample": [_ptr, _i64, _int, _int, _int, _ptr, _ptr],
+    "genre_b200_voxel_translate": [_ptr, _i64, _int, _int, _int, _ptr, _ptr, _ptr, _ptr],
 }
 
 # every symbol include/genre_b200.h declares (tests check the library exports all of them)
@@ -88,7 +94,7 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_convt_c1_wgrad_workspace_bytes", "genre_b200_conv_k8s2_wgrad_workspace_bytes",
     "genre_b200_bn_workspace_bytes", "genre_b200_render_spherical_workspace_bytes",
     "genre_b200_voxel_surface_workspace_bytes", "genre_b200_conv_set_tma", "genre_b200_conv_set_cluster", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
-    "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes"])
+    "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
@@ -108,6 +114,8 @@ _LAUNCHES = {
     "genre_b200_convt3d_s2_merged_forward": 1, "genre_b200_conv3d_k8s2_s4d_forward": 1, "genre_b200_ncdhw_to_blocked": 1, "genre_b200_blocked_to_ncdhw": 1,
     "genre_b200_isosurface_count": 2, "genre_b200_isosurface_emit": 2,
     "genre_b200_raycast_count": 3, "genre_b200_raycast_build": 2, "genre_b200_raycast_first_hit": 1,
+    "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
+    "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,
 }
 
 
@@ -152,6 +160,8 @@ def load():
     lib.genre_b200_isosurface_workspace_bytes.argtypes = [_i64, _int, _int, _int]
     lib.genre_b200_raycast_workspace_bytes.restype = _size
     lib.genre_b200_raycast_workspace_bytes.argtypes = [_i64, _int]
+    lib.genre_b200_voxel_fill_workspace_bytes.restype = _size
+    lib.genre_b200_voxel_fill_workspace_bytes.argtypes = [_i64, _int, _int, _int]
     _lib = lib
     return lib
 

@@ -9,6 +9,10 @@ the device: the reference runs ``scipy.ndimage.binary_erosion`` on every sample 
 ``raycast`` / ``render_mesh_spherical`` / ``spherical_from_depth`` are the partial spherical map of the published test path
 (``util_sph.render_spherical``, util/util_sph.py:36-57: depth -> TDF -> marching cubes -> trimesh ray casting), batched on
 the device.
+
+``voxel_fill`` / ``voxel_transform`` / ``find_bound`` / ``bounding_box_align`` / ``translate`` / ``downsample`` / ``voxel_iou``
+are the reference's voxel toolkit (util/util_voxel.py: exterior fill, affine resampling, bounding boxes, integer shifts and
+pooling) plus the IoU an evaluation computes from them, batched on the device.
 """
 import numpy as np
 import torch
@@ -289,3 +293,220 @@ def _tdf_480(absd):
               fl.data_ptr(), *fl.stride(), cd.data_ptr(), *cd.stride(), tdf.data_ptr(), None, 128, 0, ws.data_ptr(), nbytes,
               _lib.stream_ptr(absd))
     return tdf
+
+
+# ---- voxel-grid utilities: the batched util/util_voxel.py ----------------------------------------------------------------
+def _per_sample(x, n, name, dtype=np.float64):
+    """-> [B,3] numpy array from a scalar or 3 values (the same for every sample; a flat sequence of 3 is always one
+    3-vector, the reference's form), [B,1] (one scalar per sample, used on all 3 axes) or [B,3] (one 3-vector per sample)"""
+    if isinstance(x, torch.Tensor):
+        x = x.detach().cpu().numpy()
+    a = np.asarray(x, dtype=np.float64)
+    if a.ndim == 0 or a.shape == (3,) or a.shape == (n, 1):
+        a = np.broadcast_to(a, (n, 3))
+    if a.shape != (n, 3):
+        raise ValueError("%s: expected a scalar, 3 values, [%d, 1] or [%d, 3], got shape %s (one scalar per sample goes as "
+                         "[B, 1])" % (name, n, n, a.shape))
+    return np.ascontiguousarray(a.astype(dtype))
+
+
+def _rotation(angles):
+    """util_voxel.get_rotation_matrix (util/util_voxel.py:114-126): rotations about axis 0, then 1, then 2, multiplied in that
+    order"""
+    a, b, g = angles
+    rx = np.array([[1, 0, 0], [0, np.cos(a), -np.sin(a)], [0, np.sin(a), np.cos(a)]])
+    ry = np.array([[np.cos(b), 0, -np.sin(b)], [0, 1, 0], [np.sin(b), 0, np.cos(b)]])
+    rz = np.array([[np.cos(g), -np.sin(g), 0], [np.sin(g), np.cos(g), 0], [0, 0, 1]])
+    return np.dot(np.dot(rx, ry), rz)
+
+
+def transform_params(n, angles=(0, 0, 0), scales=(1, 1, 1), offset=(0, 0, 0)):
+    """[n, 12] fp64 numpy parameters of the voxel_transform kernel, formed on the host as util_voxel.transform does
+    (util/util_voxel.py:133-161): M = inv(R(angles) . diag(scales)) row-major, then the translation -offset."""
+    ang = _per_sample(angles, n, "angles")
+    sc = _per_sample(scales, n, "scales")
+    off = _per_sample(offset, n, "offset")
+    params = np.empty((n, 12), dtype=np.float64)
+    for b in range(n):
+        params[b, :9] = np.linalg.inv(np.dot(_rotation(ang[b]), np.diag(sc[b]))).reshape(-1)
+    params[:, 9:] = -off
+    return params
+
+
+def _transform(v, params, threshold=None, clamp=False):
+    n, d, h, w = v.shape
+    flags = (1 if clamp else 0) | (2 if threshold is not None else 0)
+    out = torch.empty(v.shape, dtype=torch.uint8 if threshold is not None else torch.float32, device=v.device)
+    _lib.call("genre_b200_voxel_transform", v.data_ptr(), n, d, h, w, params.data_ptr(), flags, 0.0, 1.0,
+              float(threshold) if threshold is not None else 0.0, out.data_ptr(), _lib.stream_ptr(v))
+    return out
+
+
+def voxel_transform(voxel, angles=(0, 0, 0), scales=(1, 1, 1), offset=(0, 0, 0), threshold=None, clamp=False):
+    """The batched util_voxel.transform (util/util_voxel.py:133-161): rotate by ``angles``, then scale by ``scales``, about the
+    grid centre n/2, then move by ``offset``; each a scalar or 3 values (for every sample), [B,1] or [B,3] (per sample).
+
+    voxel [B,1,D,H,W] or [B,D,H,W] fp32 on CUDA, every dimension in [2, 512].  Output point i samples the input at
+    inv(R S) (i - n/2) + n/2 - offset with scipy's RegularGridInterpolator(method='linear', bounds_error=False,
+    fill_value=0): 0 outside the grid, the upper end point inside.  The matrix is inverted on the host in fp64; the
+    coordinates and the 8-tap sum are fp64 on the device (the order is in include/genre_b200.h), so the result is within one
+    fp32 rounding of scipy's fp64 value at the same coordinates.  ``clamp`` clips to [0, 1]; with ``threshold`` the result is
+    uint8 (value > threshold, compared in fp64), as in the reference.  Returns the input's shape, fp32 or uint8."""
+    v = _volumes(voxel, "voxel_transform")
+    params = torch.from_numpy(transform_params(v.shape[0], angles, scales, offset)).to(v.device)
+    return _transform(v, params, threshold, clamp).view(voxel.shape)
+
+
+def voxel_fill(voxel, six_way=True, threshold=0.5):
+    """The batched util_voxel.fill (util/util_voxel.py:167-238): 1 where a voxel is occupied (v > threshold) or is an empty
+    voxel the outside cannot reach through empty voxels, 0 elsewhere.  Neighbours are the 6 face neighbours (``six_way``) or
+    all 26.  The reference casts its input to uint8, so on {0, 1} grids threshold = 0.5 is its semantics.
+
+    voxel [B,1,D,H,W] or [B,D,H,W] fp32 on CUDA, every dimension in [2, 512].  Returns uint8 of the input's shape.  The
+    kernels label the empty voxels by union-find (a fixed number of passes whatever the shape, unlike the reference's
+    depth-first search) and the result is deterministic."""
+    v = _volumes(voxel, "voxel_fill")
+    n, d, h, w = v.shape
+    nbytes = _lib.load().genre_b200_voxel_fill_workspace_bytes(n, d, h, w)
+    if nbytes == 0:
+        raise ValueError("voxel_fill: %d volumes of %dx%dx%d unsupported (1 <= B <= 65535, every dimension in [2, 512])"
+                         % (n, d, h, w))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+    out = torch.empty(v.shape, dtype=torch.uint8, device=v.device)
+    _lib.call("genre_b200_voxel_fill", v.data_ptr(), n, d, h, w, float(threshold), 6 if six_way else 26, out.data_ptr(),
+              ws.data_ptr(), nbytes, _lib.stream_ptr(v))
+    return out.view(voxel.shape)
+
+
+def _bounds(v, threshold):
+    """[B,6] int32 on the device: (min_0, min_1, min_2, max_0, max_1, max_2) of v > threshold, zeros for an empty sample"""
+    n, d, h, w = v.shape
+    bounds = torch.empty((n, 6), dtype=torch.int32, device=v.device)
+    _lib.call("genre_b200_voxel_stats", v.data_ptr(), None, n, d, h, w, 1, 0, float(threshold), 0.0, bounds.data_ptr(), None,
+              _lib.stream_ptr(v))
+    return bounds
+
+
+def find_bound(voxel, threshold=0.5):
+    """The batched util_voxel.find_bound (util/util_voxel.py:31-52): per sample, the box of voxel > threshold as
+    (bmin [B,3], bmax [B,3]) int64 on the device, lower bound inclusive, upper bound exclusive, zeros for an empty sample."""
+    b = _bounds(_volumes(voxel, "find_bound"), threshold).long()
+    return b[:, :3], b[:, 3:]
+
+
+def bounding_box_align(voxel, gt, threshold=0.5):
+    """Scale and move every sample of ``voxel`` onto the box of v > threshold of the same sample of ``gt``: the uniform scale
+    s = (gt's longest side) / (voxel's longest side), about the box centres, so that voxel's box centre lands on gt's and
+    its longest side takes the length of gt's.  A box centre is the midpoint of its first and last voxel, (bmin + bmax - 1) / 2
+    per axis, and the scaling is about the voxels' extent, so a box of whole voxels maps onto a box of whole voxels: when
+    the sides' ratios all equal s, find_bound of the result is gt's box.
+
+    This is what util_voxel.bounding_box_align (util/util_voxel.py:55-61) evidently means, not what it computes:
+      * it reads find_bound(voxel) for both boxes (:57), so it always returns its input resampled at the grid points, i.e.
+        unchanged; here the second box is gt's;
+      * its offset, the difference of the (bmin + bmax) / 2 centres passed to transform(scales=s), would move the centre
+        to s * (c_gt - n/2) + n/2 rather than to c_gt once the scale is not 1; here the translation of voxel_transform
+        is t = (c_voxel - n/2) - (c_gt - n/2) * (1/s), so that output c_gt samples input c_voxel.
+    A sample whose box, or gt's, is empty is returned unchanged (the reference divides by zero there).  The parameters are
+    derived from the boxes on the device (fp64, in the order written above), and the resampling is voxel_transform's.
+
+    voxel, gt [B,1,D,H,W] or [B,D,H,W] fp32 on CUDA, of the same shape.  Returns fp32 of voxel's shape."""
+    v, g = _volumes(voxel, "bounding_box_align"), _volumes(gt, "bounding_box_align")
+    if v.shape != g.shape:
+        raise ValueError("bounding_box_align: voxel %s and gt %s differ in shape" % (tuple(v.shape), tuple(g.shape)))
+    bv, bg = _bounds(v, threshold).double(), _bounds(g, threshold).double()
+    ev = (bv[:, 3:] - bv[:, :3]).amax(1)
+    eg = (bg[:, 3:] - bg[:, :3]).amax(1)
+    ok = (ev > 0) & (eg > 0)
+    inv_scale = torch.where(ok, 1 / (eg / torch.where(ok, ev, torch.ones_like(ev))), torch.ones_like(ev))
+    half = torch.tensor(v.shape[1:], dtype=torch.float64, device=v.device) / 2
+    cv = (bv[:, :3] + bv[:, 3:] - 1) / 2
+    cg = (bg[:, :3] + bg[:, 3:] - 1) / 2
+    t = (cv - half) - (cg - half) * inv_scale[:, None]
+    params = torch.zeros((v.shape[0], 12), dtype=torch.float64, device=v.device)
+    params[:, 0] = params[:, 4] = params[:, 8] = inv_scale
+    params[:, 9:] = torch.where(ok[:, None], t, torch.zeros_like(t))
+    return _transform(v, params).view(voxel.shape)
+
+
+def translate(voxel, offset=None, translate_type=None, generator=None):
+    """The batched util_voxel.translate (util/util_voxel.py:64-90): move the contents of every sample's box of v > 0.5 by an
+    integer offset; everything outside the box is dropped, as in the reference.
+
+    Either ``offset`` (3 values, [B,1] or [B,3], truncated to integers, or a [3] or [B,3] tensor on the device) or
+    ``translate_type``:
+    'origin' moves the box to the grid's low corner, 'middle' to ceil((-bmin + shape - bmax) / 2), and 'random' draws
+    ceil(u * (shape - bmax + bmin + 1) - bmin - 1) with u uniform in [0, 1) from ``generator`` (torch's stream, not the
+    reference's numpy one).  Raises ValueError, as the reference's assert does, when a moved box would leave the grid;
+    that check copies one flag to the host.  Returns fp32 of the input's shape."""
+    v = _volumes(voxel, "translate")
+    n, d, h, w = v.shape
+    dev = v.device
+    bounds = _bounds(v, 0.5)
+    bmin, bmax = bounds[:, :3].long(), bounds[:, 3:].long()
+    shape = torch.tensor([d, h, w], dtype=torch.int64, device=dev)
+    if offset is None:
+        lo, hi = -bmin, shape - bmax
+        if translate_type == "random":
+            gdev = generator.device if generator is not None else torch.device("cpu")
+            u = torch.rand((n, 3), generator=generator, dtype=torch.float64, device=gdev).to(dev)
+            off = torch.ceil(u * (hi - lo + 1) + lo - 1).long()
+        elif translate_type == "origin":
+            off = lo
+        elif translate_type == "middle":
+            off = -torch.div(-(lo + hi), 2, rounding_mode="floor")
+        else:
+            raise ValueError("unknown translate_type: " + str(translate_type))
+    else:
+        if translate_type is not None:
+            raise ValueError("translate: give offset or translate_type, not both")
+        if isinstance(offset, torch.Tensor) and offset.is_cuda:
+            if tuple(offset.shape) not in ((3,), (n, 3)):
+                raise ValueError("translate: offset tensor of shape %s, expected [3] or [%d, 3]" % (tuple(offset.shape), n))
+            off = offset.to(dev).long().expand(n, 3)
+        else:
+            off = torch.from_numpy(_per_sample(offset, n, "offset").astype(np.int64)).to(dev)
+    if not bool(((bmin + off >= 0) & (bmax + off <= shape)).all()):
+        raise ValueError("translate: a moved box would leave the grid")
+    off32 = off.to(torch.int32).contiguous()
+    out = torch.empty_like(v)
+    _lib.call("genre_b200_voxel_translate", v.data_ptr(), n, d, h, w, bounds.data_ptr(), off32.data_ptr(), out.data_ptr(),
+              _lib.stream_ptr(v))
+    return out.view(voxel.shape)
+
+
+def downsample(voxel, times, use_max=True):
+    """The batched util_voxel.downsample (util/util_voxel.py:10-28): [B,(1,)R,R,R] -> [B,(1,)d,d,d] fp32, d = R // times (the
+    remainder ignored, as the reference does), the maximum of each times^3 block (exact) or its mean (summed in fp64,
+    rounded once to fp32)."""
+    v = _volumes(voxel, "downsample")
+    n, r = v.shape[0], v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]):
+        raise ValueError("downsample expects cubic volumes, got %s" % (tuple(voxel.shape),))
+    times = int(times)
+    dd = r // times if times >= 1 else 0
+    out = torch.empty((n, dd, dd, dd), dtype=torch.float32, device=v.device)
+    _lib.call("genre_b200_voxel_downsample", v.data_ptr(), n, r, times, 1 if use_max else 0, out.data_ptr(), _lib.stream_ptr(v))
+    return out.view(voxel.shape[:-3] + (dd, dd, dd))
+
+
+def voxel_iou(pred, gt, threshold=0.5, gt_threshold=0.5, pool=1, pool_mode="max"):
+    """Per-sample IoU of A = downsample(pred, pool) > threshold and B = downsample(gt, pool) > gt_threshold, in one pass over
+    both grids (pool = 1: the voxels themselves; the remainder of a pool that does not divide the grid is ignored).
+    At pool = 1 the fp32 voxels compare with the thresholds rounded to fp32 (as numpy and torch compare an fp32 grid with a
+    Python float); pooled values compare in fp64, as the reference thresholds its fp64 downsample output, so a block mean
+    just above the threshold counts even where its fp32 rounding (what ``downsample`` returns) would not.
+    IoU = |A and B| / |A or B|, 1.0 when both are empty.  pred, gt [B,1,D,H,W] or [B,D,H,W] fp32 on CUDA, of the same shape;
+    pool_mode 'max' or 'mean' (as ``downsample``).  Returns (iou [B] fp32, counts [B,3] int64 = |A|, |B|, |A and B|)."""
+    a, b = _volumes(pred, "voxel_iou"), _volumes(gt, "voxel_iou")
+    if a.shape != b.shape:
+        raise ValueError("voxel_iou: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(b.shape)))
+    if pool_mode not in ("max", "mean"):
+        raise ValueError("voxel_iou: pool_mode must be 'max' or 'mean', got %r" % (pool_mode,))
+    n, d, h, w = a.shape
+    counts = torch.empty((n, 3), dtype=torch.int64, device=a.device)
+    _lib.call("genre_b200_voxel_stats", a.data_ptr(), b.data_ptr(), n, d, h, w, int(pool), 0 if pool_mode == "max" else 1,
+              float(threshold), float(gt_threshold), None, counts.data_ptr(), _lib.stream_ptr(a))
+    union = counts[:, 0] + counts[:, 1] - counts[:, 2]
+    iou = torch.where(union > 0, counts[:, 2].double() / union.clamp(min=1).double(), torch.ones_like(union, dtype=torch.float64))
+    return iou.float(), counts

@@ -482,6 +482,69 @@ int genre_b200_raycast_first_hit(const float *verts, int64_t V, const int32_t *f
                                  const float *origins, const float *dirs, int64_t R, int64_t ray_batch_stride, float *t,
                                  int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Voxel-grid utilities.  Replace the per-sample CPU toolkit util/util_voxel.py for a batch resident on the device.
+ * Common rules: vol [N, D, H, W] dense fp32, every dimension in [2, 512], 1 <= N <= 65535; the caller owns every buffer and
+ * workspace; the library allocates nothing and never synchronises; argument errors are reported before any launch.
+ *
+ * fill (replaces _fill / fill, util_voxel.py:167-238): a voxel is occupied iff v > threshold (NaN: empty; the reference
+ *   casts its input to uint8, so threshold = 0.5 is its semantics on {0, 1} grids).  out [N, D, H, W] uint8 is 1 for occupied
+ *   voxels and for empty voxels not connected, through empty voxels, to the outside (a virtual empty shell around the grid);
+ *   connectivity 6 (faces) or 26 (faces, edges, corners: the reference's six_way=False).  Union-find labelling of the empty
+ *   voxels (csrc/voxel_tools.cu): a fixed number of passes whatever the shape.  The result is a set membership, so it does not
+ *   depend on the order the unions happen in: it is deterministic.
+ *   workspace: genre_b200_voxel_fill_workspace_bytes(N, D, H, W) bytes (0: unsupported shape), 16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_voxel_fill_workspace_bytes(int64_t N, int D, int H, int W);
+int genre_b200_voxel_fill(const float *vol, int64_t N, int D, int H, int W, float threshold, int connectivity, uint8_t *out,
+                          void *workspace, size_t workspace_bytes, void *stream);
+
+/* transform (replaces transform_by_matrix / transform, util_voxel.py:133-161): resampling by an affine map from output grid
+ * indices to input coordinates.  params [N, 12] fp64 on the device: a row-major 3x3 matrix M and a translation t per sample.
+ * For output point (i0, i1, i2), with n = (D, H, W): u_b = i_b - n_b/2, and for every axis a, in this order and one rounding
+ * per step (no contraction):
+ *     x_a = (((M[a][0]*u_0 + M[a][1]*u_1) + M[a][2]*u_2) + n_a/2) + t_a
+ * (the reference forms inv(matrix) . (i - n/2) + n/2 - offset; M = inv(R(angles) S(scales)) and t = -offset give it).
+ * The value is scipy's RegularGridInterpolator(method='linear', bounds_error=False, fill_value=0): 0 when x_a lies outside
+ * [0, n_a - 1] on any axis (or is NaN); else, with c_a = min(floor(x_a), n_a - 2), y_a = x_a - c_a, the 8 corners in C order
+ * (last axis fastest) each add vol[corner] * ((w_0 * w_1) * w_2) to a sum that starts at 0, w_a = 1 - y_a or y_a, all in fp64.
+ * Epilogues (flags): GENRE_B200_VOXEL_CLAMP clips the fp64 value to [clamp_lo, clamp_hi] (np.clip); then either
+ * GENRE_B200_VOXEL_THRESHOLD writes out [N, D, H, W] uint8 = value > threshold (compared in fp64), or out [N, D, H, W] fp32
+ * gets the value rounded once to fp32.
+ * ------------------------------------------------------------------------------------------- */
+#define GENRE_B200_VOXEL_CLAMP 1u
+#define GENRE_B200_VOXEL_THRESHOLD 2u
+int genre_b200_voxel_transform(const float *vol, int64_t N, int D, int H, int W, const double *params, unsigned flags,
+                               double clamp_lo, double clamp_hi, double threshold, void *out, void *stream);
+
+/* stats: one pass over a (and b).  bounds [N, 6] int32 (or NULL): find_bound (util_voxel.py:31-52) of a > th_a, as
+ * (min_0, min_1, min_2, max_0, max_1, max_2), lower bound inclusive, upper bound exclusive, all zeros for an empty sample.
+ * counts [N, 3] int64 (or NULL; needs b): |A|, |B|, |A and B| with A = pool(a) > th_a, B = pool(b) > th_b, pool = downsample
+ * (util_voxel.py:10-28) by `pool` on every axis (the remainder ignored), GENRE_B200_POOL_MAX (exact) or GENRE_B200_POOL_MEAN
+ * (fp64 sum in C order, divided by pool^3 in fp64).  Comparisons: the fp32 voxels (the bounds, and the counts at pool = 1)
+ * with the threshold rounded to fp32, as numpy and torch compare an fp32 grid with a Python float; pooled values (pool > 1)
+ * in fp64 with the fp64 threshold, as the reference thresholds the fp64 output of its downsample.  The bounds are always
+ * those of the full-resolution a.  1 <= pool <= min(D, H, W).  No workspace; at least one of bounds, counts.
+ * ------------------------------------------------------------------------------------------- */
+#define GENRE_B200_POOL_MAX 0
+#define GENRE_B200_POOL_MEAN 1
+int genre_b200_voxel_stats(const float *a, const float *b, int64_t N, int D, int H, int W, int pool, int pool_mode,
+                           double th_a, double th_b, int32_t *bounds, int64_t *counts, void *stream);
+
+/* downsample (replaces downsample, util_voxel.py:10-28): vol [N, R, R, R] -> out [N, d, d, d] fp32, d = R / times (the
+ * remainder ignored, as the reference does), 1 <= times <= R.  use_max != 0: the block's maximum (exact; NaN propagates, as
+ * np.max); else the mean: fp64 sum in C order divided by times^3 in fp64, rounded once to fp32.
+ * ------------------------------------------------------------------------------------------- */
+int genre_b200_voxel_downsample(const float *vol, int64_t N, int R, int times, int use_max, float *out, void *stream);
+
+/* translate (replaces the copy of translate, util_voxel.py:87-90): bounds [N, 6] int32 as stats writes them, offsets [N, 3]
+ * int32, both on the device.  out[p] = vol[p - off] when p - off lies inside the box [min, max) (and the grid), else 0: the
+ * box's contents move by off and everything outside the box is dropped, as in the reference.  Choosing the offset and
+ * checking that the moved box stays inside the grid (the reference's assert) is the caller's.
+ * ------------------------------------------------------------------------------------------- */
+int genre_b200_voxel_translate(const float *vol, int64_t N, int D, int H, int W, const int32_t *bounds, const int32_t *offsets,
+                               float *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,8 +13,10 @@
 //   backward: g = dy * act'(pre);  dbeta = sum g;  dgamma = sum g * xhat;
 //             dx = gamma * invstd * (g - dbeta / N - xhat * dgamma / N)
 //
-// STATUS: written at the end of round 1 after the GPU budget was spent; not yet run on a GPU.  Opt-in from Python
-// (GENRE_B200_BN_TRAIN=1); nothing routes here by default.
+// The pre-activation is formed by ONE helper, bn_pre(), in the forward and in both backward kernels: the backward's
+// activation mask is then exactly the sign of what the forward computed (autograd differentiates what ran), and x == mean
+// with beta == 0 gives exactly 0.  Routed by default for training-mode BatchNorm3d (ops_conv.BN_TRAIN,
+// GENRE_B200_BN_TRAIN=0 turns it off); tests/test_gpu_train_fp64.py checks it against an fp64 reference.
 #include "common.cuh"
 
 namespace gb {
@@ -95,6 +97,10 @@ bn_sqdev_kernel(const float4 *__restrict__ x, BnShape sh, const float *__restric
 
 __device__ __forceinline__ float act_fwd(float v, float slope) { return v > 0.0f ? v : v * slope; }
 
+// normalised value and pre-activation in the order of torch's CUDA BatchNorm, ((x - mean) * invstd) * gamma + beta
+__device__ __forceinline__ float bn_xhat(float x, float mean, float invstd) { return (x - mean) * invstd; }
+__device__ __forceinline__ float bn_pre(float xh, float gamma, float beta) { return fmaf(xh, gamma, beta); }
+
 // pass 3: normalise + affine + activation; split 0 also publishes mean / invstd and updates the running statistics
 __global__ void __launch_bounds__(BN_THREADS)
 bn_apply_kernel(const float4 *__restrict__ x, BnShape sh, const float *__restrict__ psum, const float *__restrict__ psq,
@@ -108,7 +114,6 @@ bn_apply_kernel(const float4 *__restrict__ x, BnShape sh, const float *__restric
   const float var = total_of(psq, c, sh.nsplit) / n;
   const float invstd = rsqrtf(var + eps);
   const float g = gamma ? gamma[c] : 1.0f, bt = beta ? beta[c] : 0.0f;
-  const float sc = g * invstd, sf = bt - mean * sc;
   if (split == 0 && threadIdx.x == 0) {
     save_mean[c] = mean;
     save_invstd[c] = invstd;
@@ -119,10 +124,10 @@ bn_apply_kernel(const float4 *__restrict__ x, BnShape sh, const float *__restric
     const size_t at = ((size_t)b * sh.C + c) * n4 + i;
     const float4 v = __ldg(x + at);
     float4 o;
-    o.x = act_fwd(fmaf(v.x, sc, sf), slope);
-    o.y = act_fwd(fmaf(v.y, sc, sf), slope);
-    o.z = act_fwd(fmaf(v.z, sc, sf), slope);
-    o.w = act_fwd(fmaf(v.w, sc, sf), slope);
+    o.x = act_fwd(bn_pre(bn_xhat(v.x, mean, invstd), g, bt), slope);
+    o.y = act_fwd(bn_pre(bn_xhat(v.y, mean, invstd), g, bt), slope);
+    o.z = act_fwd(bn_pre(bn_xhat(v.z, mean, invstd), g, bt), slope);
+    o.w = act_fwd(bn_pre(bn_xhat(v.w, mean, invstd), g, bt), slope);
     y[at] = o;
   });
 }
@@ -144,8 +149,8 @@ bn_bwd_sum_kernel(const float4 *__restrict__ x, const float4 *__restrict__ dy, B
     const float xv[4] = {v.x, v.y, v.z, v.w}, dv[4] = {d.x, d.y, d.z, d.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float xh = (xv[k] - mean) * invstd;
-      const float pre = fmaf(xh, g0, bt);
+      const float xh = bn_xhat(xv[k], mean, invstd);
+      const float pre = bn_pre(xh, g0, bt);
       const float gk = pre > 0.0f ? dv[k] : dv[k] * slope;
       a0 += gk;
       a1 = fmaf(gk, xh, a1);
@@ -183,8 +188,8 @@ bn_bwd_apply_kernel(const float4 *__restrict__ x, const float4 *__restrict__ dy,
     float o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float xh = (xv[k] - mean) * invstd;
-      const float pre = fmaf(xh, g0, bt);
+      const float xh = bn_xhat(xv[k], mean, invstd);
+      const float pre = bn_pre(xh, g0, bt);
       const float gk = pre > 0.0f ? dv[k] : dv[k] * slope;
       o[k] = k0 * (gk - m0 - xh * m1);
     }

@@ -122,13 +122,19 @@ struct ConvTCfg {
 // MODE 4: ConvTranspose3d(k 4, s 2, p 1) to ONE output channel (the last layer of every decoder): MODE 3's geometry with
 //         N = 16 columns of which 8 are the output classes; the epilogue adds the bias (shift[0]), optionally applies
 //         the sigmoid, and writes the NCDHW fp32 volume directly.
-// OP: operand type: 0 = TF32 (fp32 storage), 1 = fp16, 2 = fp16 hi/lo split (X2, see ConvTCfg)
+// OP: operand type: 0 = TF32 (fp32 storage), 1 = fp16, 2 = fp16 hi/lo split (X2, see ConvTCfg), 3 = TF32 operands of the
+//     3xTF32 split (lo | hi | hi along K) with a two-level accumulator: the tensor core's fp32 accumulator truncates, so a
+//     step's error scales with the partial sum it joins, and over the thousands of K steps of a k=8 layer (Unet_3D.dec5's
+//     input gradient: 3 x 1280) that bias grows past 1e-4 of the result.  OP 3 hands each stage's MMA partial sums to a
+//     second register set with round-to-nearest fp32 adds and restarts the MMA accumulator from 0; the two sets take the
+//     register budget of twice the columns (launch_convt_impl narrows the tile as for X2).
 template <int TZ, int T, int NPAD, int MT, int MODE, int OP, bool TMA>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1) {
-  constexpr bool F16 = OP != 0, X2 = OP == 2;
+  constexpr bool F16 = OP == 1 || OP == 2, X2 = OP == 2, FLUSH = OP == 3;
   using Cfg = ConvTCfg<T, NPAD, MT, X2, TMA>;
   constexpr int NACC = Cfg::NACC;
+  static_assert(!FLUSH || 2 * MT * NACC <= CT_ACC_COLS, "two-level accumulators exceed the register budget");
   constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *stages = smem;
@@ -302,10 +308,17 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     // ===================== consumers: warpgroup wg issues the wgmma of rows [64 wg, 64 wg + 64) of every M-tile ===========
     const int wg = (warp - 4) >> 2;
     float acc[MT][NACC / 2];
+    float tot[FLUSH ? MT : 1][FLUSH ? NACC / 2 : 1];   // OP 3: the round-to-nearest sum of the stages' MMA partial sums
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
       for (int j = 0; j < NACC / 2; ++j) acc[mt][j] = 0.0f;
+    if constexpr (FLUSH) {
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int j = 0; j < NACC / 2; ++j) tot[mt][j] = 0.0f;
+    }
     int it = 0;
     for (int q = 0; q < n_q; ++q) {
       int tz, kc, ys, bz, by, bx;
@@ -343,6 +356,15 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       }
       wgmma_commit();
       wgmma_wait<0>();
+      if constexpr (FLUSH) {
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int j = 0; j < NACC / 2; ++j) {
+            tot[mt][j] += acc[mt][j];
+            acc[mt][j] = 0.0f;
+          }
+      }
       }
       // frees the slot (in every CTA of the cluster): this warp's wgmma that read it are done
       __syncwarp();
@@ -355,8 +377,10 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     // every stage has been consumed, so no copy can still land in the ring: it becomes the accumulator image
     asm volatile("bar.sync 1, 256;" ::: "memory");   // ... by BOTH consumer warpgroups: the other one may still be reading it
 #pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-      store_acc_tile<NPAD, X2>(acc[mt], acc_img + (size_t)(64 * wg) * Cfg::ACC_LD + mt * NPAD, Cfg::ACC_LD);
+    for (int mt = 0; mt < MT; ++mt) {
+      if constexpr (FLUSH) store_acc_tile<NPAD, X2>(tot[mt], acc_img + (size_t)(64 * wg) * Cfg::ACC_LD + mt * NPAD, Cfg::ACC_LD);
+      else store_acc_tile<NPAD, X2>(acc[mt], acc_img + (size_t)(64 * wg) * Cfg::ACC_LD + mt * NPAD, Cfg::ACC_LD);
+    }
   }
   __syncthreads();
   if (warp < 4) {
@@ -560,7 +584,7 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
 template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
 static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
   // narrower x tiles (more CTAs, each with fewer M-tiles) until the accumulators fit the consumers' registers
-  if constexpr (MT > 1 && MT * (OP == 2 ? 2 : 1) * NPAD > CT_ACC_COLS) {
+  if constexpr (MT > 1 && MT * (OP >= 2 ? 2 : 1) * NPAD > CT_ACC_COLS) {
     return launch_convt_impl<TZ, T, NPAD, MT / 2, MODE, OP>(p, st);
   } else {
     if (conv_use_tma()) return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, true>(p, st);
@@ -568,7 +592,8 @@ static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
   }
 }
 
-static thread_local int g_conv_op = 0;  // operand type of the next launch (set by the C ABI entry points): 0 TF32, 1 fp16, 2 fp16 hi/lo
+// operand type of the next launch (set by the C ABI entry points): 0 TF32, 1 fp16, 2 fp16 hi/lo, 3 3xTF32 (two-level accumulator)
+static thread_local int g_conv_op = 0;
 // X2 doubles the accumulator columns (launch_convt_impl narrows the tile to fit them)
 template <int TZ, int T, int NPAD, int MT, int MODE>
 static int launch_convt_x2(const ConvTParams &p, cudaStream_t st) {
@@ -581,6 +606,12 @@ static int launch_convt_x2(const ConvTParams &p, cudaStream_t st) {
 template <int TZ, int T, int NPAD, int MT, int MODE>
 static int launch_convt_op(const ConvTParams &p, cudaStream_t st) {
   if (g_conv_op == 2) return launch_convt_x2<TZ, T, NPAD, MT, MODE>(p, st);
+  if (g_conv_op == 3) {
+    if constexpr (2 * NPAD > CT_ACC_COLS)   // N > 128: no room for the second register set, one-level accumulation
+      return launch_convt_impl<TZ, T, NPAD, MT, MODE, 0>(p, st);
+    else
+      return launch_convt_impl<TZ, T, NPAD, MT, MODE, 3>(p, st);
+  }
   return g_conv_op == 1 ? launch_convt_impl<TZ, T, NPAD, MT, MODE, 1>(p, st) : launch_convt_impl<TZ, T, NPAD, MT, MODE, 0>(p, st);
 }
 template <int T, int NPAD, int MT, bool PAR>

@@ -57,6 +57,9 @@ K4S2_MIN_CIN = 8
 #   "exact" (DEFAULT)  fp32-accurate: the reference's fp32 semantics (north_star: occupancies within 1e-4).  Implemented by
 #                      EXACT_IMPL: "f16x2" = fp16 hi/lo operand split, 2 MMAs per K step, separate accumulators for the
 #                      hi*hi and the cross terms; "fp32x3" = 3xTF32 with the three products along K (3 MMAs per K=8 step)
+#                      f16x2 keeps ONE truncating fp32 accumulator per part: each output stays within 1e-4 of max|ref|, but
+#                      the truncation is biased, so a mean over many outputs carries it (training-mode BatchNorm running
+#                      means of Unet_3D at batch 4: up to 64x cuDNN fp32's error against fp64, still ~3e-6 of the value)
 #   "f16"              single pass, fp16 operands (10-bit mantissa, 5-bit exponent), fp32 accumulation: opt-in, tested at
 #                      4e-3 * max|ref| per layer; inputs beyond fp16's range are the caller's responsibility
 #   "tf32"             single pass, TF32 operands (what cuDNN does while torch.backends.cudnn.allow_tf32 is on)
@@ -70,8 +73,10 @@ S4D_SPLIT_Z = os.environ.get("GENRE_B200_S4D_SPLIT_Z", "0") != "0"   # measured:
 
 
 # With torch.backends.cudnn.allow_tf32 off the caller asks for fp32 convolutions: the kernels then run the 3xTF32 scheme
-# (operands split into TF32 hi + lo parts, A_lo*W_hi + A_hi*W_lo + A_hi*W_hi accumulated in fp32: ~1e-5 relative error, set by the accumulator's truncation,
-# 3x the MMAs of the TF32 mode) so that occupancies match the fp32 reference within 1e-4.  "0": fall back to cuDNN fp32.
+# (operands split into TF32 hi + lo parts, A_lo*W_hi + A_hi*W_lo + A_hi*W_hi accumulated in fp32, 3x the MMAs of the TF32
+# mode).  The tensor core's fp32 accumulator truncates; the kernel therefore adds each pipeline stage's MMA partial sums
+# into a second, round-to-nearest accumulator (csrc/convt3d.cu OP 3), which keeps Unet_3D.dec5's input gradient (10240
+# terms per element) within 1e-5 of max|ref| against fp64 (tests/test_gpu_train_fp64.py).  "0": fall back to cuDNN fp32.
 EXACT_WHEN_TF32_OFF = os.environ.get("GENRE_B200_CONV_EXACT", "1") != "0"
 
 
@@ -185,8 +190,9 @@ def _x2():
 
 
 def _op_flag():
-    """`op` argument of the C ABI: 0 = TF32 operands, 1 = fp16, 2 = fp16 hi/lo split"""
-    return 2 if _x2() else 1 if _f16() else 0
+    """`op` argument of the C ABI: 0 = TF32 operands, 1 = fp16, 2 = fp16 hi/lo split, 3 = the 3xTF32 split (csrc/convt3d.cu
+    then keeps a second, round-to-nearest accumulator per stage)"""
+    return 2 if _x2() else 1 if _f16() else 3 if _x3() else 0
 
 
 def _tf32_hi(w):
@@ -539,12 +545,12 @@ def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0):
         # the four (y,x) parity classes share one MMA stream: N = 4 x 20 columns (csrc/convt3d.cu MODE 2)
         wpack = _pack(module, ("convt_merged", 20, g), lambda wt: pack_convt_merged_weights(wt, 20, g), 2)
         _lib.call("genre_b200_convt3d_s2_merged_forward", src0.data_ptr(), cg0, src1.data_ptr() if src1 is not None else None,
-                  cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, _op_flag() if g == 8 else 0, aff[0].data_ptr(),
+                  cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, _op_flag() if g == 8 or _x3() else 0, aff[0].data_ptr(),
                   aff[1].data_ptr(), float(slope), out.data_ptr(), cgo, _lib.stream_ptr(src0))
         return out
     wpack = _pack(module, ("convt", npad, g), lambda wt: pack_convt_weights(wt, npad, g), 4)
     _lib.call("genre_b200_convt3d_s2_forward", src0.data_ptr(), cg0, src1.data_ptr() if src1 is not None else None, cg1,
-              batch, bd // batch, h, w, wpack.data_ptr(), module.kernel_size[0], npad, _op_flag() if g == 8 else 0,
+              batch, bd // batch, h, w, wpack.data_ptr(), module.kernel_size[0], npad, _op_flag() if g == 8 or _x3() else 0,
               aff[0].data_ptr(), aff[1].data_ptr(), float(slope), out.data_ptr(), cgo, _lib.stream_ptr(src0))
     return out
 
@@ -1061,7 +1067,7 @@ def dgrad_convt_k8s2(gy, m):
             one = m.__dict__["_gb_dgrad_affine"] = (torch.ones(96, device=gy.device), torch.zeros(96, device=gy.device))
         out = torch.empty((bd, cgo, hh, ww, 4), device=gy.device, dtype=torch.float32)
         _lib.call("genre_b200_conv3d_taps_forward", xb.data_ptr(), cg, None, 0, b, bd // b, hh, ww, wpack.data_ptr(), 5, 2, 96,
-                  0, one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, _lib.stream_ptr(gy))
+                  _op_flag(), one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, _lib.stream_ptr(gy))
         dx = from_blocked(out, b, cin_t)
         dx.__dict__.pop("_gb_blocked", None)
         return dx
@@ -1089,7 +1095,7 @@ def dgrad_conv_k8s2(gy, m):
             one = m.__dict__["_gb_dgrad_affine"] = (torch.ones(96, device=gy.device), torch.zeros(96, device=gy.device))
         out = torch.empty((bd * 2, cgo, 2 * hh, 2 * ww, 4), device=gy.device, dtype=torch.float32)
         _lib.call("genre_b200_convt3d_s2_merged_forward", src.data_ptr(), cg, None, 0, b, bd // b, hh, ww, wpack.data_ptr(), 8, 80,
-                  0, one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, _lib.stream_ptr(gy))
+                  _op_flag(), one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, _lib.stream_ptr(gy))
         dx = from_blocked(out, b, cin)
         dx.__dict__.pop("_gb_blocked", None)
         return dx
@@ -1235,7 +1241,7 @@ def conv3d(x, m, bn=None, slope=None):
         if aff is None:
             return None
         g, b, cout = _group(), x.shape[0], m.out_channels
-        split_z = S4D_SPLIT_Z or _x2()     # f16x2 doubles the accumulator columns: 8 classes x 20 x 2 = 320 > 256, 4 classes fit
+        split_z = S4D_SPLIT_Z or _x2() or _x3()   # f16x2 / fp32x3 double the accumulator columns: 8 classes x 20 x 2 = 320 > 256
         wpack = _pack(m, ("k8s2_s4d", 20, g, split_z), lambda wt: pack_conv_k8s2_s4d_weights(wt, 20, g, split_z),
                       2 if split_z else 1)
         if _x2_direct(x):

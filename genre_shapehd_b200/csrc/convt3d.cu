@@ -23,7 +23,8 @@
 // MT * NACC <= 256 (launch_convt_impl narrows the x tile until it fits).  After the last K step they store the
 // accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.
 // Pipeline: STAGES-deep ring of (halo chunk, weight chunk) with full/empty mbarriers; every consumer warp arrives on a slot's
-// empty barrier once its wgmma that read the slot have completed.
+// empty barrier once its wgmma that read the slot have completed.  With 3 or more stages a stage's MMAs stay in flight while
+// the next stage is awaited and issued (wgmma.wait_group 1): its slot is released after the next stage's MMAs are committed.
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (the entry point is resolved through the runtime: no -lcuda)
 #include <cstdlib>
 #include <cstring>
@@ -59,12 +60,15 @@ struct ConvTParams {
 // ---- the kernel ----------------------------------------------------------------------------------------------
 // T: taps per dimension of a parity class (K/2: 2 for k=4, 4 for k=8); NPAD: padded Cout (32 or 64); MT = W/8.
 // X2: the fp32-accurate fp16 hi/lo operand split.  Activations arrive as [B*D][2 parts: hi, lo'][cg][H][W][8 fp16] with
-// lo' = (a - hi) * 2^11, weights as [W_hi | W_lo'] side by side along N (lo' = (w - hi) * 2^11).  Per K step and tap:
-//     A_hi  x [W_hi | W_lo']  ->  accumulator columns [0, 2*NPAD)      (one MMA, N = 2*NPAD)
-//     A_lo' x  W_hi           ->  accumulator columns [NPAD, 2*NPAD)   (one MMA, N = NPAD)
+// lo' = (a - hi) * 2^11, weights as [W_hi | W_lo'] side by side along N (lo' = (w - hi) * 2^11).  Per K step and tap,
+// three N = NPAD MMAs, in this order:
+//     A_hi  x W_hi   ->  accumulator columns [0, NPAD)        (acc_hi)
+//     A_hi  x W_lo'  ->  accumulator columns [NPAD, 2*NPAD)   (acc_cross)
+//     A_lo' x W_hi   ->  accumulator columns [NPAD, 2*NPAD)   (acc_cross)
 // so the hi*hi products and the 2^11-scaled cross terms keep separate accumulators (the tensor core's fp32 accumulator
 // truncates: a step's error scales with the partial sum it joins, and the cross terms would otherwise ride on the big one),
-// and the epilogue returns acc_hi + 2^-11 * acc_cross.  2 MMAs per K step instead of the 3 of a K-expanded split.
+// and the epilogue returns acc_hi + 2^-11 * acc_cross.  The first two could be one N = 2*NPAD MMA, but the third would then
+// write into half of its registers, which makes ptxas serialize every wgmma of the kernel.
 // TMA: the halo of a channel group arrives as ONE cp.async.bulk.tensor (5-D tiled tensor map over [plane][cg][H][W][16 B], box
 // [1][1][PY][PX][16 B], out-of-bounds elements zero-filled = the convolution's padding) instead of PY*PX 16-byte cp.async
 // issued by 128 threads; each channel group then starts on a 128-byte boundary of shared memory (the LBO of the A descriptor
@@ -82,6 +86,8 @@ struct ConvTCfg {
   static constexpr int B_TAP_BYTES = 2 * (NACC / 8) * 128;     // one (y,x) tap: [2 kcore][NACC/8][8 rows][16 B]
   // A stage holds the halo of one (z tap, K chunk) and the weights of ROWS of its T tap rows; YS = T / ROWS (rounded up)
   // stages walk the same halo when all T*T taps do not fit twice into shared memory (X2 with 5x5 union taps: 128 KB).
+  // dec5 keeps 2 stages of 3 + 2 tap rows: 3 stages of 2 + 2 + 1 rows would let its MMAs stay in flight across stages (the
+  // kernel's INFLIGHT), but load each halo three times, and measured 5.40 ms per call against 4.97 (H100 80GB HBM3, 700 W).
   static constexpr int stage_bytes(int ys) { return ((A_BYTES + ((T + ys - 1) / ys) * T * B_TAP_BYTES + 127) / 128) * 128; }
   static constexpr int pick_ys() {
     for (int ys = 1; ys < T; ++ys)
@@ -90,6 +96,7 @@ struct ConvTCfg {
   }
   static constexpr int YS = pick_ys();
   static constexpr int ROWS = (T + YS - 1) / YS;
+  static constexpr int rows_of(int ys) { return (ys + 1) * ROWS <= T ? ROWS : T - ys * ROWS; }   // tap rows of stage ys
   static constexpr int B_BYTES = ROWS * T * B_TAP_BYTES;
   static constexpr int STAGE_BYTES = stage_bytes(YS);
   // one CTA per SM (the accumulators take half the register file): the whole 227 KB of shared memory serves the ring
@@ -136,6 +143,9 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   constexpr int NACC = Cfg::NACC;
   static_assert(!FLUSH || 2 * MT * NACC <= CT_ACC_COLS, "two-level accumulators exceed the register budget");
   constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4;
+  // a stage's MMAs stay in flight while the next stage is issued (its slot is released one stage late) only with a ring of 3
+  // or more, where the producer still has a slot to fill meanwhile; OP 3 reads its accumulators after every stage
+  constexpr int INFLIGHT = Cfg::STAGES >= 3 && !FLUSH ? 1 : 0;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *stages = smem;
   uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)Cfg::RING_BYTES);
@@ -154,12 +164,12 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   const int y0 = yt * CT_BY, x0 = xt * Cfg::W;
   const int nchunk = (p.cg0 + p.cg1) / CT_KCG;
 
-  // Stage enumeration shared by the producer and the MMA issuer: q = tz * nchunk + kc, skipped when the z tap plane
-  // of that K chunk lies outside the input (it contributes nothing).  The per-dimension base offset of a chunk is
-  // uniform (parity class / plain convolution) or a function of the chunk's source sub-volume (strided conv).
-  auto stage_of = [&](int q, int &tz, int &kc, int &ys, int &bz, int &by, int &bx) -> bool {
-    ys = q % Cfg::YS;
-    const int qq = q / Cfg::YS;
+  // (z tap, K chunk) enumeration shared by the producer and the MMA issuer: qq = tz * nchunk + kc, skipped when the z tap
+  // plane of that K chunk lies outside the input (it contributes nothing).  Each qq is YS stages, stage ys holding the
+  // tap rows [ys * ROWS, min(T, ys * ROWS + ROWS)): an unrolled loop, so every stage's MMA sequence has a compile-time
+  // shape (a runtime bound on the tap rows makes ptxas serialize every wgmma).  The per-dimension base offset of a chunk
+  // is uniform (parity class / plain convolution) or a function of the chunk's source sub-volume (strided conv).
+  auto stage_of = [&](int qq, int &tz, int &kc, int &bz, int &by, int &bx) -> bool {
     tz = qq / nchunk;
     kc = qq - tz * nchunk;
     if (p.srcpar_cgs) {
@@ -175,7 +185,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     const int zi = zj + bz - tz;
     return zi >= 0 && zi < p.D;
   };
-  const int n_q = TZ * nchunk * Cfg::YS;
+  const int n_qq = TZ * nchunk;
   // Cluster of NCL CTAs along blockIdx.x (same parity class, hence the same weight sequence): every CTA fetches 1/NCL of each
   // stage's weights and multicasts it to all of them, so the L2 serves the weights once per cluster instead of once per CTA.
   // The CTAs then walk the SAME stage sequence in lockstep: a stage whose z-tap plane lies outside this CTA's volume is not
@@ -208,31 +218,33 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       // ===================== producer: ONE thread issues the tensor copies of every stage ==========================
       if (tid == 0) {
         int it = 0;
-        for (int q = 0; q < n_q; ++q) {
-          int tz, kc, ys, bz, by, bx;
-          const bool valid = stage_of(q, tz, kc, ys, bz, by, bx);
+        for (int qq = 0; qq < n_qq; ++qq) {
+          int tz, kc, bz, by, bx;
+          const bool valid = stage_of(qq, tz, kc, bz, by, bx);
           if (!valid && ncl == 1) continue;
-          const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-          ++it;
-          if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
-          uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
-          const int rows = (ys + 1) * Cfg::ROWS <= T ? Cfg::ROWS : T - ys * Cfg::ROWS;
-          const uint32_t wbytes = (uint32_t)(rows * T * Cfg::B_TAP_BYTES);
-          const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
-                              (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
-          mbar_arrive_expect_tx(&full[s], wbytes + (valid ? (uint32_t)Cfg::A_TX_BYTES : 0u));
-          load_weights(sa + Cfg::A_BYTES, wsrc, wbytes, &full[s]);
-          if (!valid) continue;
-          const int zi = zj + bz - tz;
-          const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);
 #pragma unroll
-          for (int part = 0; part < Cfg::PARTS; ++part) {
+          for (int ys = 0; ys < Cfg::YS; ++ys) {
+            const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
+            ++it;
+            if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
+            uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
+            const uint32_t wbytes = (uint32_t)(Cfg::rows_of(ys) * T * Cfg::B_TAP_BYTES);
+            const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
+                                (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
+            mbar_arrive_expect_tx(&full[s], wbytes + (valid ? (uint32_t)Cfg::A_TX_BYTES : 0u));
+            load_weights(sa + Cfg::A_BYTES, wsrc, wbytes, &full[s]);
+            if (!valid) continue;
+            const int zi = zj + bz - tz;
+            const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);
 #pragma unroll
-            for (int c = 0; c < CT_KCG; ++c) {
-              int cg = kc * CT_KCG + c;
-              const CUtensorMap *tm = &tmap0;
-              if (cg >= p.cg0) { cg -= p.cg0; tm = &tmap1; }
-              tma_load_5d(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE, tm, gx0, gy0, cg, (b * p.D + zi) * Cfg::PARTS + part, &full[s]);
+            for (int part = 0; part < Cfg::PARTS; ++part) {
+#pragma unroll
+              for (int c = 0; c < CT_KCG; ++c) {
+                int cg = kc * CT_KCG + c;
+                const CUtensorMap *tm = &tmap0;
+                if (cg >= p.cg0) { cg -= p.cg0; tm = &tmap1; }
+                tma_load_5d(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE, tm, gx0, gy0, cg, (b * p.D + zi) * Cfg::PARTS + part, &full[s]);
+              }
             }
           }
         }
@@ -248,7 +260,9 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       hx[i] = idx - hy[i] * Cfg::PX;
       hoff[i] = idx < Cfg::POS ? idx * 16 : -1;
     }
-    constexpr int LAG = Cfg::STAGES - 1 < 2 ? 1 : 2;  // cp.async groups in flight before a stage is published
+    // cp.async groups in flight before a stage is published: the slot a publication waits for must not be one the consumers
+    // still hold, so LAG + INFLIGHT < STAGES
+    constexpr int LAG = Cfg::STAGES - 1 - INFLIGHT < 2 ? Cfg::STAGES - 1 - INFLIGHT : 2;
     int it = 0;                                        // stages issued so far
     auto publish = [&]() {  // after committing group `it`: group it - LAG has landed -> hand it to the async proxy
       cp_async_commit();
@@ -259,47 +273,49 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       }
       ++it;
     };
-    for (int q = 0; q < n_q; ++q) {
-      int tz, kc, ys, bz, by, bx;
-      const bool valid = stage_of(q, tz, kc, ys, bz, by, bx);
+    for (int qq = 0; qq < n_qq; ++qq) {
+      int tz, kc, bz, by, bx;
+      const bool valid = stage_of(qq, tz, kc, bz, by, bx);
       if (!valid && ncl == 1) continue;
-      const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-      if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
-      uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
-      if (tid == 0) {
-        // weights of tap rows [ys*ROWS, ...) of this (class, z tap, K chunk): a contiguous slice of its T*T-tap block
-        const int rows = (ys + 1) * Cfg::ROWS <= T ? Cfg::ROWS : T - ys * Cfg::ROWS;
-        const uint32_t bytes = (uint32_t)(rows * T * Cfg::B_TAP_BYTES);
-        const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
-                            (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
-        mbar_arrive_expect_tx(&full[s], bytes);
-        load_weights(sa + Cfg::A_BYTES, wsrc, bytes, &full[s]);
-      }
-      const int zi = zj + bz - tz;
-      const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);  // halo row hy holds input row gy0 + hy
-      if (valid) {
 #pragma unroll
-      for (int part = 0; part < Cfg::PARTS; ++part) {
+      for (int ys = 0; ys < Cfg::YS; ++ys) {
+        const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
+        if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
+        uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
+        if (tid == 0) {
+          // weights of tap rows [ys*ROWS, ...) of this (class, z tap, K chunk): a contiguous slice of its T*T-tap block
+          const uint32_t bytes = (uint32_t)(Cfg::rows_of(ys) * T * Cfg::B_TAP_BYTES);
+          const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
+                              (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
+          mbar_arrive_expect_tx(&full[s], bytes);
+          load_weights(sa + Cfg::A_BYTES, wsrc, bytes, &full[s]);
+        }
+        const int zi = zj + bz - tz;
+        const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);  // halo row hy holds input row gy0 + hy
+        if (valid) {
 #pragma unroll
-        for (int c = 0; c < CT_KCG; ++c) {
-          int cg = kc * CT_KCG + c;
-          const float *src = p.src0;
-          int ncg = p.cg0;
-          if (cg >= p.cg0) { cg -= p.cg0; src = p.src1; ncg = p.cg1; }
-          // X2: [B*D][part][cg][H][W][16 B]
-          const float *plane = src + (((((size_t)b * p.D + zi) * Cfg::PARTS + part) * ncg + cg) * p.H) * (size_t)p.W * 4;
+        for (int part = 0; part < Cfg::PARTS; ++part) {
 #pragma unroll
-          for (int i = 0; i < Cfg::POS_PER_THREAD; ++i) {
-            if (hoff[i] < 0) continue;
-            const int gy = gy0 + hy[i], gx = gx0 + hx[i];
-            const bool ok = (gy >= 0) & (gy < p.H) & (gx >= 0) & (gx < p.W);
-            const float *g = ok ? plane + ((size_t)gy * p.W + gx) * 4 : plane;
-            cp_async16_zfill(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE + hoff[i], g, ok);
+          for (int c = 0; c < CT_KCG; ++c) {
+            int cg = kc * CT_KCG + c;
+            const float *src = p.src0;
+            int ncg = p.cg0;
+            if (cg >= p.cg0) { cg -= p.cg0; src = p.src1; ncg = p.cg1; }
+            // X2: [B*D][part][cg][H][W][16 B]
+            const float *plane = src + (((((size_t)b * p.D + zi) * Cfg::PARTS + part) * ncg + cg) * p.H) * (size_t)p.W * 4;
+#pragma unroll
+            for (int i = 0; i < Cfg::POS_PER_THREAD; ++i) {
+              if (hoff[i] < 0) continue;
+              const int gy = gy0 + hy[i], gx = gx0 + hx[i];
+              const bool ok = (gy >= 0) & (gy < p.H) & (gx >= 0) & (gx < p.W);
+              const float *g = ok ? plane + ((size_t)gy * p.W + gx) * 4 : plane;
+              cp_async16_zfill(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE + hoff[i], g, ok);
+            }
           }
         }
+        }
+        publish();
       }
-      }
-      publish();
     }
     for (int e = 0; e < LAG; ++e) publish();  // drain: empty groups push the last real ones through
 
@@ -319,61 +335,94 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
         for (int j = 0; j < NACC / 2; ++j) tot[mt][j] = 0.0f;
     }
+    // frees a slot (in every CTA of the cluster): this warp's wgmma that read it are done
+    auto release = [&](int slot) {
+      __syncwarp();
+      if (lane == 0) {
+        if (ncl == 1) mbar_arrive(&empty[slot]);
+        else
+          for (uint32_t c = 0; c < ncl; ++c) mbar_arrive_cluster(&empty[slot], c);
+      }
+    };
     int it = 0;
-    for (int q = 0; q < n_q; ++q) {
-      int tz, kc, ys, bz, by, bx;
-      const bool valid = stage_of(q, tz, kc, ys, bz, by, bx);
+    int held = -1;   // the slot of the last committed stage, whose MMAs may still be running
+    for (int qq = 0; qq < n_qq; ++qq) {
+      int tz, kc, bz, by, bx;
+      const bool valid = stage_of(qq, tz, kc, bz, by, bx);
       if (!valid && ncl == 1) continue;
-      const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-      ++it;
-      mbar_wait(&full[s], use & 1);
-      if (valid) {
-      wgmma_fence();
-      const uint32_t sa = smem_u32(stages + (size_t)s * Cfg::STAGE_BYTES);
-      const uint32_t sb = sa + Cfg::A_BYTES;
-      const int ty0 = ys * Cfg::ROWS;
 #pragma unroll
-      for (int r = 0; r < Cfg::ROWS; ++r) {
-        const int ty = ty0 + r;
-        if (ty >= T) break;
+      for (int ys = 0; ys < Cfg::YS; ++ys) {
+        const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
+        ++it;
+        mbar_wait(&full[s], use & 1);
+        if (!valid) {   // walked in lockstep with the cluster: the weights pass through, no MMAs
+          // the held slot belongs to the last stage WITH MMAs, which may lie several stages back: the producers need it
+          // (from every CTA of the cluster) before they can publish the stage STAGES later, possibly the next one this CTA
+          // waits for, so it is not kept across stages walked without MMAs
+          if (held >= 0) {
+            wgmma_wait<0>();
+            release(held);
+            held = -1;
+          }
+          release(s);
+          continue;
+        }
+        wgmma_fence();
+        const uint32_t sa = smem_u32(stages + (size_t)s * Cfg::STAGE_BYTES);
+        const uint32_t sb = sa + Cfg::A_BYTES;
 #pragma unroll
-        for (int tx = 0; tx < T; ++tx) {
-          const uint64_t bdesc = gmma_desc(sb + (r * T + tx) * Cfg::B_TAP_BYTES, (NACC / 8) * 128, 128);
+        for (int r = 0; r < Cfg::rows_of(ys); ++r) {
+          const int ty = ys * Cfg::ROWS + r;
 #pragma unroll
-          for (int mt = 0; mt < MT; ++mt) {
-            // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x; this warpgroup's
-            // 64 rows are y = 8 wg .. 8 wg + 7
-            const uint32_t a0 = sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
-            const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, Cfg::PX * 16);
-            if constexpr (F16) wgmma_f16<NACC>(acc[mt], adesc, bdesc);
-            else wgmma_tf32<NACC>(acc[mt], adesc, bdesc);
-            if constexpr (X2) {   // A_lo' x W_hi: the first NPAD columns of the same B tile
-              const uint64_t adesc_lo = gmma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, Cfg::PX * 16);
-              wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc_lo, bdesc);
+          for (int tx = 0; tx < T; ++tx) {
+            const uint32_t btap = sb + (r * T + tx) * Cfg::B_TAP_BYTES;
+            const uint64_t bdesc = gmma_desc(btap, (NACC / 8) * 128, 128);
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt) {
+              // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x; this warpgroup's
+              // 64 rows are y = 8 wg .. 8 wg + 7
+              const uint32_t a0 = sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
+              const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+              if constexpr (X2) {
+                // A_hi x W_hi into the hi accumulator, then the cross terms A_hi x W_lo' and A_lo' x W_hi, in that order,
+                // into the cross accumulator: three N = NPAD MMAs on disjoint registers (an MMA that writes into part of
+                // another's accumulator registers makes ptxas serialize every wgmma)
+                const uint64_t adesc_lo = gmma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+                wgmma_f16<NPAD>(acc[mt], adesc, bdesc);
+                wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc, gmma_desc(btap + (NPAD / 8) * 128, (NACC / 8) * 128, 128));
+                wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc_lo, bdesc);
+              } else if constexpr (F16) {
+                wgmma_f16<NACC>(acc[mt], adesc, bdesc);
+              } else {
+                wgmma_tf32<NACC>(acc[mt], adesc, bdesc);
+              }
             }
           }
         }
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      if constexpr (FLUSH) {
+        wgmma_commit();
+        if constexpr (!INFLIGHT) {
+          wgmma_wait<0>();
+          if constexpr (FLUSH) {
 #pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
+            for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-          for (int j = 0; j < NACC / 2; ++j) {
-            tot[mt][j] += acc[mt][j];
-            acc[mt][j] = 0.0f;
+              for (int j = 0; j < NACC / 2; ++j) {
+                tot[mt][j] += acc[mt][j];
+                acc[mt][j] = 0.0f;
+              }
           }
-      }
-      }
-      // frees the slot (in every CTA of the cluster): this warp's wgmma that read it are done
-      __syncwarp();
-      if (lane == 0) {
-        if (ncl == 1) mbar_arrive(&empty[s]);
-        else
-          for (uint32_t c = 0; c < ncl; ++c) mbar_arrive_cluster(&empty[s], c);
+          release(s);
+        } else {
+          // keep this stage's MMAs in flight while the next stage's operands are awaited: only the previous stage's
+          // must be done before its slot is handed back
+          wgmma_wait<1>();
+          if (held >= 0) release(held);
+          held = s;
+        }
       }
     }
+    wgmma_wait<0>();
+    if (held >= 0) release(held);
     // every stage has been consumed, so no copy can still land in the ring: it becomes the accumulator image
     asm volatile("bar.sync 1, 256;" ::: "memory");   // ... by BOTH consumer warpgroups: the other one may still be reading it
 #pragma unroll

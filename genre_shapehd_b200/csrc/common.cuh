@@ -1,6 +1,7 @@
 // common.cuh — shared helpers for libgenre_b200 (sm_90a only; no torch, no CPU fallback).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stddef.h>
 #include <stdio.h>
@@ -38,6 +39,37 @@ __device__ __forceinline__ void st_stream_f4(float *p, float4 v) {
 }
 __device__ __forceinline__ void st_stream_f1(float *p, float v) {
   asm volatile("st.global.cs.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+
+// 8 fp16 -> one 16-byte unit
+__device__ __forceinline__ uint4 pack_half8(const __half (&h)[8]) {
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) w[i] = (uint32_t)__half_as_ushort(h[2 * i]) | ((uint32_t)__half_as_ushort(h[2 * i + 1]) << 16);
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// 8 fp32 -> one 16-byte unit of 8 fp16, each rounded to nearest (the operand of the single-pass f16 mode)
+__device__ __forceinline__ uint4 pack_f16x8(const float (&x)[8]) {
+  __half h[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) h[i] = __float2half_rn(x[i]);
+  return pack_half8(h);
+}
+
+// The activation operand of the fp32-accurate f16x2 convolution mode for 8 channels: hi = fp16(a), lo' = fp16((a - hi) * 2^11),
+// a = hi + lo' * 2^-11 to ~2^-22 |a|.  Every producer of this operand (the layout kernels and the convolution epilogues) calls this
+// function: the intrinsics are never contracted into an FMA with the code that computed `a`, so the same fp32 value gives the
+// same bits wherever it is split.  |a| > 65504 becomes inf (and stays visible in the output).
+__device__ __forceinline__ void split_hi_lo8(const float (&x)[8], uint4 &hi, uint4 &lo) {
+  __half h[8], l[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    h[i] = __float2half_rn(x[i]);
+    l[i] = __float2half_rn(__fmul_rn(__fsub_rn(x[i], __half2float(h[i])), 2048.0f));
+  }
+  hi = pack_half8(h);
+  lo = pack_half8(l);
 }
 
 __device__ __forceinline__ unsigned lanemask_lt() {

@@ -55,7 +55,42 @@ struct ConvTParams {
   int act_sigmoid = 0;       // MODE 4: apply a sigmoid after the bias
   int srcpar_cgs;            // 0, or: the K range is 8 parity sub-volumes of srcpar_cgs channel groups each (strided
                              // Conv3d k=4 s=2 p=1 after space-to-depth); sub-volume s = (pz,py,px) uses base 1 - p per dim
+  // fp16 modes: the epilogue writes the fp16 operand(s) of the next layers instead of `out` when odst[0] is set (OP_PLAIN or
+  // OP_PARITY layout, ocg groups of 8 channels, oparts parts: 2 = hi | lo' of split_hi_lo8, 1 = fp16).  Channels >= 4 * cgo
+  // are written as zeros.
+  uint4 *odst[2] = {nullptr, nullptr};
+  int olayout[2] = {0, 0};
+  int ocg[2] = {0, 0};
+  int oparts = 0;
 };
+// operand output layouts (Do, Ho, Wo: the output extent)
+//   OP_PLAIN   [B*Do][oparts][ocg][Ho][Wo][8 fp16]: the blocked operand of a following ConvTranspose3d
+//   OP_PARITY  [B*Do/2][oparts][8 s][ocg][Ho/2][Wo/2][8 fp16], s = ((z&1)*2 + (y&1))*2 + (x&1): the parity sub-volumes of a
+//              following Conv3d(k 4, s 2, p 1) (genre_b200_ncdhw_to_blocked mode 2, cpad = 8 * ocg)
+constexpr int OP_PLAIN = 1, OP_PARITY = 2;
+
+// one 8-channel group k of output position (b, oz, oy, ox) into every operand destination that has a group k
+__device__ __forceinline__ void store_operand(const ConvTParams &p, int k, int b, int oz, int oy, int ox, int Do, int Ho, int Wo,
+                                              const float (&v)[8]) {
+  uint4 u[2];
+  if (p.oparts == 2) split_hi_lo8(v, u[0], u[1]);
+  else u[0] = pack_f16x8(v);
+#pragma unroll
+  for (int d = 0; d < 2; ++d) {
+    if (p.odst[d] == nullptr || k >= p.ocg[d]) continue;
+    size_t idx, pstride;
+    if (p.olayout[d] == OP_PLAIN) {
+      pstride = (size_t)p.ocg[d] * Ho * Wo;
+      idx = ((size_t)(b * Do + oz) * p.oparts * p.ocg[d] + k) * ((size_t)Ho * Wo) + (size_t)oy * Wo + ox;
+    } else {
+      const int H2 = Ho >> 1, W2 = Wo >> 1, s = ((oz & 1) * 2 + (oy & 1)) * 2 + (ox & 1);
+      pstride = (size_t)8 * p.ocg[d] * H2 * W2;
+      idx = (((size_t)(b * (Do >> 1) + (oz >> 1)) * p.oparts * 8 + s) * p.ocg[d] + k) * ((size_t)H2 * W2) + (size_t)(oy >> 1) * W2 + (ox >> 1);
+    }
+    p.odst[d][idx] = u[0];
+    if (p.oparts == 2) p.odst[d][idx + pstride] = u[1];
+  }
+}
 
 // ---- the kernel ----------------------------------------------------------------------------------------------
 // T: taps per dimension of a parity class (K/2: 2 for k=4, 4 for k=8); NPAD: padded Cout (32 or 64); MT = W/8.
@@ -440,6 +475,17 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     constexpr bool UP = PAR || MERGE || MERGE8 || C1;
     const int Ho = UP ? 2 * p.H : p.H, Wo = UP ? 2 * p.W : p.W, Do = UP ? 2 * p.D : p.D;
     const int oz_plain = UP ? 2 * zj + pz : zj, oy = PAR ? 2 * (y0 + yy) + py : y0 + yy;
+    auto act = [&](float a, int n) {
+      const float t = fmaf(a, __ldg(p.scale + n), __ldg(p.shift + n));
+      return t > 0.0f ? t : t * p.slope;
+    };
+    // operand outputs: groups of 8 channels past those the accumulators hold are the destinations' zero padding
+    const bool to_operands = F16 && p.odst[0] != nullptr;
+    auto store_zero_groups = [&](int k0, int oz, int oyy, int ox) {
+      const int kmax = max(p.ocg[0], p.odst[1] ? p.ocg[1] : 0);
+      const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      for (int k = k0; k < kmax; ++k) store_operand(p, k, b, oz, oyy, ox, Do, Ho, Wo, z);
+    };
     if constexpr (C1) {
       const float bias = __ldg(p.shift);
 #pragma unroll
@@ -470,6 +516,27 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
           const int qz = MERGE8 ? qzy >> 1 : 0, qy = qzy & 1;
           const int oyy = 2 * (y0 + yy) + qy;
           const int oz = MERGE8 ? 2 * zj + qz : 2 * zj + pz;
+          if (to_operands) {
+#pragma unroll
+            for (int qx = 0; qx < 2; ++qx) {
+              const float *cls = arow + mt * NPAD + (qzy * 2 + qx) * CP;   // the CP channels of class (qz, qy, qx)
+#pragma unroll
+              for (int k = 0; k < (CP + 7) / 8; ++k) {
+                float v[8];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int c0 = 8 * k + 4 * h;
+                  float v4[4] = {0.f, 0.f, 0.f, 0.f};
+                  if (c0 < CP) ld_row<4>(cls + c0, v4);
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) v[4 * h + e] = c0 < CP && c0 + e < 4 * p.cgo ? act(v4[e], c0 + e) : 0.0f;
+                }
+                store_operand(p, k, b, oz, oyy, oxb + qx, Do, Ho, Wo, v);
+              }
+              store_zero_groups((CP + 7) / 8, oz, oyy, oxb + qx);
+            }
+            continue;
+          }
 #pragma unroll
           for (int cgo = 0; cgo < CP / 4; ++cgo) {
             if (cgo >= p.cgo) continue;  // uniform across the CTA
@@ -501,6 +568,25 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
       const int ox = PAR ? 2 * (x0 + 8 * mt + xx) + px : x0 + 8 * mt + xx;
+      if (to_operands) {
+#pragma unroll
+        for (int nb = 0; nb < NPAD / 32; ++nb) {
+          float v[32];
+          ld_row<32>(arow + mt * NPAD + nb * 32, v);
+#pragma unroll
+          for (int k8 = 0; k8 < 4; ++k8) {
+            float g[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int n = nb * 32 + k8 * 8 + e;
+              g[e] = n < 4 * p.cgo ? act(v[k8 * 8 + e], n) : 0.0f;
+            }
+            store_operand(p, nb * 4 + k8, b, oz_plain, oy, ox, Do, Ho, Wo, g);
+          }
+        }
+        store_zero_groups(NPAD / 8, oz_plain, oy, ox);
+        continue;
+      }
 #pragma unroll
       for (int nb = 0; nb < NPAD / 32; ++nb) {
         float v[32];
@@ -671,6 +757,31 @@ template <int TZ, int T, int NPAD, int MT>
 static int launch_convt_merged(const ConvTParams &p, cudaStream_t st) {
   return launch_convt_op<TZ, T, NPAD, MT, 2>(p, st);
 }
+// the operand destinations of the *_operands entry points
+struct OperandOut {
+  void *dst[2];
+  int layout[2], cpad[2];
+};
+static int set_operand_outputs(ConvTParams &p, const OperandOut &o, int f16, int64_t Do, int64_t Ho, int64_t Wo, const char *who) {
+  GB_REQUIRE(f16 == 1 || f16 == 2, GENRE_B200_EINVAL, "%s: operand outputs need fp16 operands (f16 = 1 or 2), not %d", who, f16);
+  GB_REQUIRE(o.dst[0], GENRE_B200_EINVAL, "%s: null pointer (first operand destination)", who);
+  for (int d = 0; d < 2; ++d) {
+    if (!o.dst[d]) continue;
+    GB_REQUIRE(o.layout[d] == OP_PLAIN || o.layout[d] == OP_PARITY, GENRE_B200_EINVAL,
+               "%s: operand layout %d unknown (1 = plain blocked, 2 = parity sub-volumes)", who, o.layout[d]);
+    GB_REQUIRE(o.cpad[d] % 8 == 0 && o.cpad[d] >= 4 * p.cgo, GENRE_B200_EINVAL,
+               "%s: operand cpad %d must be a multiple of 8 and cover the %d output channels", who, o.cpad[d], 4 * p.cgo);
+    GB_REQUIRE(o.layout[d] == OP_PLAIN || (Do % 2 == 0 && Ho % 2 == 0 && Wo % 2 == 0), GENRE_B200_EINVAL,
+               "%s: parity sub-volumes of an odd output extent", who);
+    GB_REQUIRE(aligned16(o.dst[d]), GENRE_B200_EALIGN, "%s: operand destinations must be 16-byte aligned", who);
+    p.odst[d] = reinterpret_cast<uint4 *>(o.dst[d]);
+    p.olayout[d] = o.layout[d];
+    p.ocg[d] = o.cpad[d] / 8;
+  }
+  p.oparts = f16 == 2 ? 2 : 1;
+  return 0;
+}
+
 template <int MT>
 static int launch_convt_c1(const ConvTParams &p, cudaStream_t st) {
   if (g_conv_op == 2)   // not routed (ops_conv.convt_c1_tc): the exact FP32-pipe stencil serves the fp32-accurate modes
@@ -708,13 +819,12 @@ extern "C" int genre_b200_conv_set_cluster(int ctas) {
 //   scale, shift [npad]: per-channel affine applied to the accumulator (bias and folded eval-mode BatchNorm),
 //   slope: LeakyReLU slope (1 = none).   out [B*2D][cgo][2H][2W][4]
 // Supported: W in {16, 32}, H % 16 == 0, cg0 + cg1 even, 4*cgo <= npad, npad in {32, 64}.
-extern "C" int genre_b200_convt3d_s2_forward(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B,
-                                             int64_t D, int64_t H, int64_t W, const void *wpack_, int ksize, int npad,
-                                             int f16, const float *scale, const float *shift, float slope, float *out,
-                                             int cgo, void *stream) {
+static int convt3d_s2(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D, int64_t H, int64_t W,
+                      const void *wpack_, int ksize, int npad, int f16, const float *scale, const float *shift, float slope,
+                      float *out, int cgo, const OperandOut *ops, void *stream) {
   const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
   g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && scale && shift && out, GENRE_B200_EINVAL, "convt3d: null pointer");
+  GB_REQUIRE(src0 && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "convt3d: null pointer");
   GB_REQUIRE(ksize == 4 || ksize == 8, GENRE_B200_EINVAL, "convt3d: kernel size %d unsupported (4 or 8)", ksize);
   GB_REQUIRE(npad == 32 || npad == 64, GENRE_B200_EINVAL, "convt3d: npad %d unsupported (32 or 64)", npad);
   GB_REQUIRE(W == 16 || W == 32, GENRE_B200_EINVAL, "convt3d: input width %lld unsupported (16 or 32)", (long long)W);
@@ -723,13 +833,17 @@ extern "C" int genre_b200_convt3d_s2_forward(const void *src0_, int cg0, const v
              "convt3d: channel groups (%d + %d) must be even in total", cg0, cg1);
   GB_REQUIRE(cgo > 0 && 4 * cgo <= npad, GENRE_B200_EINVAL, "convt3d: %d output channels exceed npad %d", 4 * cgo, npad);
   GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "convt3d: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && aligned16(out) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
+  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && (!out || aligned16(out)) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
              "convt3d: buffers must be 16-byte aligned");
   ConvTParams p;
   p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
   p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
   p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
   p.srcpar_cgs = 0;
+  if (ops) {
+    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "convt3d");
+    if (rc) return rc;
+  }
   const int pad = ksize / 2 - 1;
   for (int par = 0; par < 2; ++par) {
     const int k0 = (par + pad) % 2;
@@ -749,6 +863,21 @@ extern "C" int genre_b200_convt3d_s2_forward(const void *src0_, int cg0, const v
 #undef GB_CT
   return fail_arg(GENRE_B200_EINVAL, "convt3d: no kernel instance for k=%d npad=%d W=%lld", ksize, npad, (long long)W);
 }
+extern "C" int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B, int64_t D,
+                                             int64_t H, int64_t W, const void *wpack, int ksize, int npad, int f16,
+                                             const float *scale, const float *shift, float slope, float *out, int cgo,
+                                             void *stream) {
+  return convt3d_s2(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
+}
+// The same layer writing the fp16 operand(s) of the next layers (layouts OP_PLAIN / OP_PARITY above) instead of `out`.
+extern "C" int genre_b200_convt3d_s2_forward_operands(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                                                      int64_t D, int64_t H, int64_t W, const void *wpack, int ksize, int npad,
+                                                      int f16, const float *scale, const float *shift, float slope, int cgo,
+                                                      void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                                      void *stream) {
+  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
+  return convt3d_s2(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
+}
 
 // ConvTranspose3d(kernel 8, stride 2, padding 3) with the four (y,x) output parity classes merged along N (kernel MODE 2):
 // the layer that dominates Unet_3D, dec5 = ConvT(80 -> 20) on 32^3 (networks/networks.py:166).  Same operands as
@@ -756,13 +885,12 @@ extern "C" int genre_b200_convt3d_s2_forward(const void *src0_, int cg0, const v
 //   wpack [2 z-parity][4 z-tap][Cin chunk][5*5 union taps][2][npad/8][8][g], npad = 4 * cpad columns ordered
 //         n = (py*2+px)*cpad + co  (ops_conv.pack_convt_merged_weights);  scale, shift [cpad].
 // Supported: ksize 8, npad = 80 (Cout <= 20), W = 16 or a multiple of 32, H % 16 == 0.
-extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B,
-                                                    int64_t D, int64_t H, int64_t W, const void *wpack_, int ksize,
-                                                    int npad, int f16, const float *scale, const float *shift,
-                                                    float slope, float *out, int cgo, void *stream) {
+static int convt3d_s2_merged(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D, int64_t H,
+                             int64_t W, const void *wpack_, int ksize, int npad, int f16, const float *scale,
+                             const float *shift, float slope, float *out, int cgo, const OperandOut *ops, void *stream) {
   const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
   g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && scale && shift && out, GENRE_B200_EINVAL, "convt3d_merged: null pointer");
+  GB_REQUIRE(src0 && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "convt3d_merged: null pointer");
   GB_REQUIRE(ksize == 8, GENRE_B200_EINVAL, "convt3d_merged: kernel size %d unsupported (8)", ksize);
   GB_REQUIRE(npad == 80, GENRE_B200_EINVAL, "convt3d_merged: npad %d unsupported (80 = 4 classes x 20 channels)", npad);
   GB_REQUIRE(W == 16 || (W > 0 && W % 32 == 0), GENRE_B200_EINVAL,
@@ -772,13 +900,17 @@ extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0_, int cg0, 
              "convt3d_merged: channel groups (%d + %d) must be even in total", cg0, cg1);
   GB_REQUIRE(cgo > 0 && 16 * cgo <= npad, GENRE_B200_EINVAL, "convt3d_merged: %d output channels exceed npad/4", 4 * cgo);
   GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "convt3d_merged: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && aligned16(out) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
+  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && (!out || aligned16(out)) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
              "convt3d_merged: buffers must be 16-byte aligned");
   ConvTParams p;
   p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
   p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
   p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
   p.srcpar_cgs = 0;
+  if (ops) {
+    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "convt3d_merged");
+    if (rc) return rc;
+  }
   const int pad = ksize / 2 - 1;
   for (int par = 0; par < 2; ++par) {
     const int k0 = (par + pad) % 2;
@@ -788,6 +920,21 @@ extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0_, int cg0, 
   if (W % 32 == 0) return launch_convt_merged<4, 5, 80, 4>(p, st);  // 32-wide x tiles
   return launch_convt_merged<4, 5, 80, 2>(p, st);
 }
+extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                                                    int64_t D, int64_t H, int64_t W, const void *wpack, int ksize,
+                                                    int npad, int f16, const float *scale, const float *shift,
+                                                    float slope, float *out, int cgo, void *stream) {
+  return convt3d_s2_merged(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
+}
+extern "C" int genre_b200_convt3d_s2_merged_forward_operands(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                                                             int64_t D, int64_t H, int64_t W, const void *wpack, int ksize,
+                                                             int npad, int f16, const float *scale, const float *shift,
+                                                             float slope, int cgo, void *dst0, int layout0, int cpad0,
+                                                             void *dst1, int layout1, int cpad1, void *stream) {
+  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
+  return convt3d_s2_merged(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, nullptr, cgo, &ops,
+                           stream);
+}
 
 // Conv3d(kernel 8, stride 2, padding 3), few input channels, Cout <= 20, on a 4x space-to-depth input (kernel MODE 3):
 // Unet_3D.enc1 = Conv3d(2 -> 20) on 128^3 (networks/networks.py:151).
@@ -795,29 +942,46 @@ extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0_, int cg0, 
 //   wpack [3 z-tap][chunk][9 taps][2][npad/8][8][g], npad = 160 columns n = ((qz*2+qy)*2+qx)*20 + co
 //         (ops_conv.pack_conv_k8s2_s4d_weights);  scale, shift [20];  out [B*2D][cgo][2H][2W][4] fp32
 // Supported: W % 16 == 0, H % 16 == 0, cg even.
-extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src_, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
-                                                  const void *wpack_, int npad, int f16, const float *scale,
-                                                  const float *shift, float slope, float *out, int cgo, void *stream) {
+static int conv3d_k8s2_s4d(const void *src_, int cg, int64_t B, int64_t D, int64_t H, int64_t W, const void *wpack_, int npad,
+                           int f16, const float *scale, const float *shift, float slope, float *out, int cgo,
+                           const OperandOut *ops, void *stream) {
   const float *src = (const float *)src_, *wpack = (const float *)wpack_;
   g_conv_op = f16;
-  GB_REQUIRE(src && wpack && scale && shift && out, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: null pointer");
+  GB_REQUIRE(src && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "conv3d_k8s2_s4d: null pointer");
   GB_REQUIRE(npad == 160 || npad == 80, GENRE_B200_EINVAL,
              "conv3d_k8s2_s4d: npad %d unsupported (160 = 8 classes x 20 channels, or 80 = 4 (y,x) classes per z class)", npad);
   GB_REQUIRE(W > 0 && W % 16 == 0 && H > 0 && H % CT_BY == 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: bad extent");
   GB_REQUIRE(cg > 0 && cg % CT_KCG == 0, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: channel groups must be even");
   GB_REQUIRE(cgo > 0 && cgo <= 5, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: too many output channels");
   GB_REQUIRE(B * D * (H / CT_BY) * (W / 16) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_k8s2_s4d: grid too large");
-  GB_REQUIRE(aligned16(src) && aligned16(wpack) && aligned16(out), GENRE_B200_EALIGN, "conv3d_k8s2_s4d: alignment");
+  GB_REQUIRE(aligned16(src) && aligned16(wpack) && (!out || aligned16(out)), GENRE_B200_EALIGN, "conv3d_k8s2_s4d: alignment");
   ConvTParams p;
   p.src0 = src; p.src1 = nullptr; p.cg0 = cg; p.cg1 = 0;
   p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
   p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
   p.srcpar_cgs = 0;
+  if (ops) {
+    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "conv3d_k8s2_s4d");
+    if (rc) return rc;
+  }
   p.base[0] = p.base[1] = 1;  // input cell = j + 1 - t
   // npad 80: the z class moves to blockIdx.y (MODE 2 with 3 z taps per class; wpack [2 qz][3][chunk][9][2][10][8][g]):
   // twice the MMAs of the 8-class form, but half the accumulator columns and weight bytes per stage
   if (npad == 80) return launch_convt_merged<3, 3, 80, 2>(p, as_stream(stream));
   return launch_conv_merged8<3, 160, 2>(p, as_stream(stream));
+}
+extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
+                                                  const void *wpack, int npad, int f16, const float *scale,
+                                                  const float *shift, float slope, float *out, int cgo, void *stream) {
+  return conv3d_k8s2_s4d(src, cg, B, D, H, W, wpack, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
+}
+// enc1 writing the fp16 operands of enc2 (OP_PARITY: output class q at coarse position j IS sub-volume q at j) and dec6
+extern "C" int genre_b200_conv3d_k8s2_s4d_forward_operands(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
+                                                           const void *wpack, int npad, int f16, const float *scale,
+                                                           const float *shift, float slope, int cgo, void *dst0, int layout0,
+                                                           int cpad0, void *dst1, int layout1, int cpad1, void *stream) {
+  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
+  return conv3d_k8s2_s4d(src, cg, B, D, H, W, wpack, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
 }
 
 // ConvTranspose3d(Cin -> 1, k 4, s 2, p 1) on the tensor cores (kernel MODE 4): the last layer of every decoder
@@ -912,24 +1076,28 @@ extern "C" int genre_b200_conv3d_taps_forward(const void *src0_, int cg0, const 
 //   wpack [2 z-tap][kblocks*8*cgs/2 chunk][4 taps][2][npad/8][8][g];  out [B*D'][cgo][H'][W'][4] fp32
 //   kblocks (1, or 3 for the hi|lo|hi operand of the 3xTF32 mode): how many such 8-sub-volume blocks the K range holds
 // Supported: W' in {16, 32}, H' % 16 == 0, cgs even, npad in {32, 64, 96, 128}.
-extern "C" int genre_b200_conv3d_k4s2_forward(const void *src_, int cgs, int kblocks, int64_t B, int64_t D, int64_t H,
-                                              int64_t W, const void *wpack_, int npad, int f16, const float *scale,
-                                              const float *shift, float slope, float *out, int cgo, void *stream) {
+static int conv3d_k4s2(const void *src_, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W, const void *wpack_,
+                       int npad, int f16, const float *scale, const float *shift, float slope, float *out, int cgo,
+                       const OperandOut *ops, void *stream) {
   const float *src = (const float *)src_, *wpack = (const float *)wpack_;
   g_conv_op = f16;
-  GB_REQUIRE(src && wpack && scale && shift && out, GENRE_B200_EINVAL, "conv3d_k4s2: null pointer");
+  GB_REQUIRE(src && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "conv3d_k4s2: null pointer");
   GB_REQUIRE(npad == 32 || npad == 64 || npad == 96 || npad == 128, GENRE_B200_EINVAL, "conv3d_k4s2: npad %d", npad);
   GB_REQUIRE(W == 16 || W == 32, GENRE_B200_EINVAL, "conv3d_k4s2: output width %lld unsupported (16 or 32)", (long long)W);
   GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "conv3d_k4s2: bad extent");
   GB_REQUIRE(cgs > 0 && cgs % CT_KCG == 0, GENRE_B200_EINVAL, "conv3d_k4s2: channel groups per sub-volume must be even");
   GB_REQUIRE(cgo > 0 && 4 * cgo <= npad, GENRE_B200_EINVAL, "conv3d_k4s2: too many output channels");
   GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_k4s2: grid too large");
-  GB_REQUIRE(aligned16(src) && aligned16(wpack) && aligned16(out), GENRE_B200_EALIGN, "conv3d_k4s2: alignment");
+  GB_REQUIRE(aligned16(src) && aligned16(wpack) && (!out || aligned16(out)), GENRE_B200_EALIGN, "conv3d_k4s2: alignment");
   ConvTParams p;
   p.src0 = src; p.src1 = nullptr; p.cg0 = 8 * cgs * (kblocks > 0 ? kblocks : 1); p.cg1 = 0;
   p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
   p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
   p.srcpar_cgs = cgs;
+  if (ops) {
+    const int rc = set_operand_outputs(p, *ops, f16, D, H, W, "conv3d_k4s2");
+    if (rc) return rc;
+  }
   p.base[0] = p.base[1] = 0;
   cudaStream_t st = as_stream(stream);
 #define GB_CS(NN, MM) return launch_convt<2, NN, MM, false>(p, st)
@@ -946,4 +1114,16 @@ extern "C" int genre_b200_conv3d_k4s2_forward(const void *src_, int cgs, int kbl
   }
 #undef GB_CS
   return fail_arg(GENRE_B200_EINVAL, "conv3d_k4s2: no kernel instance");
+}
+extern "C" int genre_b200_conv3d_k4s2_forward(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
+                                              const void *wpack, int npad, int f16, const float *scale, const float *shift,
+                                              float slope, float *out, int cgo, void *stream) {
+  return conv3d_k4s2(src, cgs, kblocks, B, D, H, W, wpack, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
+}
+extern "C" int genre_b200_conv3d_k4s2_forward_operands(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H,
+                                                       int64_t W, const void *wpack, int npad, int f16, const float *scale,
+                                                       const float *shift, float slope, int cgo, void *dst0, int layout0,
+                                                       int cpad0, void *dst1, int layout1, int cpad1, void *stream) {
+  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
+  return conv3d_k4s2(src, cgs, kblocks, B, D, H, W, wpack, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
 }

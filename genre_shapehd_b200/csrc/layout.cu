@@ -37,21 +37,8 @@ __device__ __forceinline__ void store_unit(void *dst, size_t unit_index, const f
 // X2 output (the fp32-accurate conv mode's operand): [r][2 parts][CG][plane] units of 8 fp16, part 0 = hi = fp16(a), part 1 =
 // lo' = fp16((a - hi) * 2^11).  `u` is the unit index in the single-part layout [r][CG][plane]; units_per_r = CG * plane.
 __device__ __forceinline__ void store_unit_x2(void *dst, size_t u, size_t r, size_t units_per_r, const float (&x)[8]) {
-  __half hi[8], lo[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    hi[i] = __float2half_rn(x[i]);
-    lo[i] = __float2half_rn((x[i] - __half2float(hi[i])) * 2048.0f);
-  }
   uint4 ph, pl;
-  ph.x = (uint32_t)__half_as_ushort(hi[0]) | ((uint32_t)__half_as_ushort(hi[1]) << 16);
-  ph.y = (uint32_t)__half_as_ushort(hi[2]) | ((uint32_t)__half_as_ushort(hi[3]) << 16);
-  ph.z = (uint32_t)__half_as_ushort(hi[4]) | ((uint32_t)__half_as_ushort(hi[5]) << 16);
-  ph.w = (uint32_t)__half_as_ushort(hi[6]) | ((uint32_t)__half_as_ushort(hi[7]) << 16);
-  pl.x = (uint32_t)__half_as_ushort(lo[0]) | ((uint32_t)__half_as_ushort(lo[1]) << 16);
-  pl.y = (uint32_t)__half_as_ushort(lo[2]) | ((uint32_t)__half_as_ushort(lo[3]) << 16);
-  pl.z = (uint32_t)__half_as_ushort(lo[4]) | ((uint32_t)__half_as_ushort(lo[5]) << 16);
-  pl.w = (uint32_t)__half_as_ushort(lo[6]) | ((uint32_t)__half_as_ushort(lo[7]) << 16);
+  split_hi_lo8(x, ph, pl);
   uint4 *o = reinterpret_cast<uint4 *>(dst) + u + r * units_per_r;
   o[0] = ph;
   o[units_per_r] = pl;
@@ -289,21 +276,8 @@ split2_f16_kernel(const float4 *__restrict__ src, uint4 *__restrict__ dst, int c
     const float4 a = __ldg(s);
     const float4 b = 2 * g + 1 < cg4 ? __ldg(s + plane) : make_float4(0.f, 0.f, 0.f, 0.f);
     const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    __half hi[8], lo[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      hi[i] = __float2half_rn(x[i]);
-      lo[i] = __float2half_rn((x[i] - __half2float(hi[i])) * 2048.0f);
-    }
     uint4 ph, pl;
-    ph.x = (uint32_t)__half_as_ushort(hi[0]) | ((uint32_t)__half_as_ushort(hi[1]) << 16);
-    ph.y = (uint32_t)__half_as_ushort(hi[2]) | ((uint32_t)__half_as_ushort(hi[3]) << 16);
-    ph.z = (uint32_t)__half_as_ushort(hi[4]) | ((uint32_t)__half_as_ushort(hi[5]) << 16);
-    ph.w = (uint32_t)__half_as_ushort(hi[6]) | ((uint32_t)__half_as_ushort(hi[7]) << 16);
-    pl.x = (uint32_t)__half_as_ushort(lo[0]) | ((uint32_t)__half_as_ushort(lo[1]) << 16);
-    pl.y = (uint32_t)__half_as_ushort(lo[2]) | ((uint32_t)__half_as_ushort(lo[3]) << 16);
-    pl.z = (uint32_t)__half_as_ushort(lo[4]) | ((uint32_t)__half_as_ushort(lo[5]) << 16);
-    pl.w = (uint32_t)__half_as_ushort(lo[6]) | ((uint32_t)__half_as_ushort(lo[7]) << 16);
+    split_hi_lo8(x, ph, pl);
     uint4 *o = dst + ((r * 2) * cg8 + g) * plane + hw;
     o[0] = ph;
     o[(size_t)cg8 * plane] = pl;

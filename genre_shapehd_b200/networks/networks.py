@@ -221,8 +221,16 @@ class Conv3d_block(nn.Module):
         super().__init__()
         self.net = nn.Sequential(Conv3d(ncin, ncout, kernel_size, stride, pad), nn.BatchNorm3d(ncout), nn.LeakyReLU())
 
-    def forward(self, x):
-        y = ops_conv.conv3d(x, self.net[0], self.net[1], self.net[2].negative_slope) if x.is_cuda else None
+    def operand_layout(self, shape):
+        """the fp16 operand layout in which this block reads an input of `shape` straight from its producer, or None"""
+        return ops_conv.conv_operand_layout(shape, self.net[0], self.net[1])
+
+    def forward(self, x, operands=None):
+        """operands: the operand layouts of this block's consumers (Unet_3D.forward): the output may then be an
+        ops_conv.OperandActivation"""
+        y = ops_conv.conv3d(x, self.net[0], self.net[1], self.net[2].negative_slope, operands) if x.is_cuda else None
+        if y is None:
+            ops_conv._fp32_only(x)
         if y is None and ops_conv.BN_TRAIN and x.is_cuda and self.net[1].training:
             c = self.net[0](x)
             z = ops_conv.bn_act_train(c, self.net[1], self.net[2])
@@ -238,17 +246,25 @@ class Deconv3d_skip(nn.Module):
         deconv = ConvTranspose3d(ncin, ncout, kernel_size, stride, pad, extra)
         self.net = nn.Sequential(deconv, nn.BatchNorm3d(ncout), nn.LeakyReLU()) if is_activate else deconv
 
-    def forward(self, x, skip_in, keep_blocked=False):
-        """keep_blocked: the caller promises the result only feeds another Deconv3d_skip (Unet_3D.forward does for
-        dec5 -> dec6), so a custom kernel may leave it in its blocked layout (ops_conv.BlockedActivation)."""
+    def _conv_bn(self):
+        return (self.net[0], self.net[1]) if isinstance(self.net, nn.Sequential) else (self.net, None)
+
+    def operand_layout(self, x_shape, skip_shape):
+        """the fp16 operand layout in which this block reads inputs of these shapes straight from their producers, or None"""
+        return ops_conv.deconv_operand_layout(x_shape, skip_shape, *self._conv_bn())
+
+    def forward(self, x, skip_in, operands=None):
+        """operands: the operand layouts of this block's consumers (Unet_3D.forward): the output may then be an
+        ops_conv.OperandActivation"""
         if not x.is_cuda:
             y = None
         elif isinstance(self.net, nn.Sequential):
-            y = ops_conv.deconv_skip(x, skip_in, self.net[0], self.net[1], self.net[2].negative_slope, keep_blocked)
+            y = ops_conv.deconv_skip(x, skip_in, self.net[0], self.net[1], self.net[2].negative_slope, operands)
         else:
             y = ops_conv.deconv_skip(x, skip_in, self.net)
         if y is not None:
             return y
+        ops_conv._fp32_only(x, skip_in)
         if isinstance(x, ops_conv.BlockedActivation):
             x = x.ncdhw()
         if ops_conv.BN_TRAIN and x.is_cuda and isinstance(self.net, nn.Sequential) and self.net[1].training:
@@ -276,15 +292,45 @@ class Unet_3D(nn.Module):
         self.dec6 = Deconv3d_skip(2 * nf, 1, 4, 2, 1, 0, is_activate=False)
         self.no_linear = no_linear
 
+    @staticmethod
+    def _out_shape(conv, shape):
+        if isinstance(conv, nn.ConvTranspose3d):
+            sp = [(s - 1) * st - 2 * p + k + op for s, st, p, k, op in
+                  zip(shape[2:], conv.stride, conv.padding, conv.kernel_size, conv.output_padding)]
+        else:
+            sp = [(s + 2 * p - k) // st + 1 for s, st, p, k in zip(shape[2:], conv.stride, conv.padding, conv.kernel_size)]
+        return (shape[0], conv.out_channels) + tuple(sp)
+
+    @staticmethod
+    def _request(layouts):
+        """operand outputs to ask a producer for: one per distinct layout, and only when EVERY consumer reads one"""
+        if not layouts or any(l is None for l in layouts):
+            return None
+        return list(dict.fromkeys(layouts))
+
     def forward(self, x):
+        # A layer whose consumers all read their input as the fp16 operand of a tensor-core kernel writes that operand from
+        # its epilogue (ops_conv.OperandActivation): no fp32 output, no layout passes.  enc i feeds enc i+1 and dec 7-i.
         skips = []
         for i in range(1, 7):
-            x = getattr(self, "enc%d" % i)(x)
+            enc = getattr(self, "enc%d" % i)
+            operands = None
+            if i < 6 and x.is_cuda:
+                out = self._out_shape(enc.net[0], x.shape)
+                dec = getattr(self, "dec%d" % (7 - i))
+                dec_x = (out[0], dec._conv_bn()[0].in_channels - out[1]) + out[2:]
+                operands = self._request([getattr(self, "enc%d" % (i + 1)).operand_layout(out), dec.operand_layout(dec_x, out)])
+            x = enc(x, operands)
             skips.append(x)
         enc6 = skips[-1]
         if not self.no_linear:
             b = enc6.size(0)
             x = self.full_conv_block(enc6.view(b, self.nf * 32)).view(b, self.nf * 32, 1, 1, 1)
         for i in range(1, 7):
-            x = getattr(self, "dec%d" % i)(x, skips[6 - i], keep_blocked=(i == 5))   # dec5's only consumer is dec6
+            dec = getattr(self, "dec%d" % i)
+            operands = None
+            if i < 6 and x.is_cuda:
+                out = self._out_shape(dec._conv_bn()[0], (x.shape[0], x.shape[1] + skips[6 - i].shape[1]) + tuple(x.shape[2:]))
+                operands = self._request([getattr(self, "dec%d" % (i + 1)).operand_layout(out, skips[5 - i].shape)])
+            x = dec(x, skips[6 - i], operands)
         return x

@@ -309,6 +309,8 @@ def to_blocked(x, group=4, dtype=None):
 
 
 def _to_operand(x):
+    if isinstance(x, OperandActivation):
+        return x.operand(PLAIN, x.shape[1])[0]
     if _x2():   # the fp32 blocked twin a previous custom layer left behind saves the NCDHW round trip
         twin = _cached_blocked(x)
         if twin is not None and twin.shape[1] * 4 == x.shape[1] and twin.shape[0] == x.shape[0] * x.shape[2]:
@@ -333,10 +335,100 @@ def from_blocked(y, batch, channels):
     return out
 
 
+# ---- operand activations: a layer's output written by its epilogue as the fp16 operand its consumers read -------------------
+PLAIN, PARITY = 1, 2     # operand layouts of csrc/convt3d.cu: blocked [B*D][parts][cpad/8][H][W][8]; parity sub-volumes
+                         # [B*D/2][parts][8][cpad/8][H/2][W/2][8] (the input of a Conv3d k4 s2, = space_to_depth_sources)
+
+
+class OperandActivation:
+    """The output of a layer that exists only as the fp16 operand(s) of the layers consuming it: `operands[layout]` =
+    (tensor, cpad) for PLAIN (a following ConvTranspose3d) and / or PARITY (a following Conv3d k4 s2).  Quacks like the
+    NCDHW fp32 tensor for the routing predicates but holds no fp32 values: the hi/lo split loses ~2 bits, so fp32 cannot be
+    rebuilt from it, and a layer that would need fp32 refuses it (operand()).  Producers write one only when
+    conv_operand_layout / deconv_operand_layout said that every consumer reads it directly."""
+    is_cuda, dtype, requires_grad = True, torch.float32, False
+
+    def __init__(self, shape, device=None):
+        self.shape, self.device, self.mode, self.operands = torch.Size(shape), device, _mode(), {}
+
+    def dim(self):
+        return 5
+
+    def size(self, i=None):
+        return self.shape if i is None else self.shape[i]
+
+    def operand(self, layout, cpad=None):
+        hit = self.operands.get(layout)
+        if hit is None or self.mode != _mode() or (cpad is not None and hit[1] != cpad):
+            raise RuntimeError("an activation written only as a %s fp16 operand reached a layer that needs %s"
+                               % (self.mode, "the fp32 activation" if hit is None else "another operand"))
+        return hit
+
+
+def _fp32_only(*xs):
+    for x in xs:
+        if isinstance(x, OperandActivation):
+            x.operand(None)     # raises
+
+
+def _operand_outputs_ok(m, bn):
+    """can a layer with module m [and BatchNorm bn] read its input straight from the producer's operand output?  The fp16
+    modes only (the fp32x3 / tf32 operands are fp32 values), no autograd, no batch statistics"""
+    return (_mode() in ("f16x2", "f16") and _no_autograd(m.weight, m.bias) and not _needs_grad(m.weight, m.bias)
+            and (bn is None or (not bn.training and bn.track_running_stats)))
+
+
+def conv_operand_layout(x_shape, m, bn=None):
+    """(layout, cpad) in which conv3d(x, m, bn) reads an input of x_shape as the kernel operand in the current mode, or None
+    when it needs the fp32 activation.  Same predicates, in the same order, as conv3d's routing."""
+    x = OperandActivation(x_shape)
+    if (not _operand_outputs_ok(m, bn) or _skinny_conv_supported(x, m) or _flat_conv_supported(x, m)
+            or not _conv_k4s2_supported(x, m)):
+        return None
+    return PARITY, _k4s2_cpad(x_shape[1])
+
+
+def deconv_operand_layout(x_shape, skip_shape, conv, bn=None):
+    """(layout, cpad) in which deconv_skip reads each of its two inputs (shapes x_shape, skip_shape) as the kernel operand
+    in the current mode, or None when it needs the fp32 activations.  Same predicates, in the same order, as deconv_skip's
+    routing; the two inputs have the same channel count in Unet_3D, so one layout serves both."""
+    x, s = OperandActivation(x_shape), OperandActivation(skip_shape)
+    if x_shape[1] != skip_shape[1] or not _operand_outputs_ok(conv, bn):
+        return None
+    if bn is None and conv.out_channels == 1:
+        cpad = -(-x_shape[1] // 8) * 8     # the padding _operand_of gives the fp32 blocked twin
+        return (PLAIN, cpad) if _convt_c1_col2im_supported((x, s), conv) and (2 * cpad) % 16 == 0 else None
+    if _flat_convt_supported((x, s), conv) or not _deconv_kernel_supported(x, s, conv):
+        return None
+    return PLAIN, x_shape[1]
+
+
+def _operand_request(operands):
+    """the operand outputs a producer is asked for, if the current mode writes fp16 operands"""
+    return operands if operands and _mode() in ("f16x2", "f16") else None
+
+
+def _operand_destinations(operands, shape, device):
+    """allocate the producer's operand outputs (every element, the channel padding included, is written by the epilogue) ->
+    (OperandActivation, the dst0, layout0, cpad0, dst1, layout1, cpad1 arguments of the C ABI)"""
+    b, c, d, h, w = shape
+    parts = _parts()
+    act = OperandActivation(shape, device)
+    args = []
+    for layout, cpad in operands:
+        if layout == PLAIN:
+            t = torch.empty((b * d, parts * (cpad // 8), h, w, 8), device=device, dtype=torch.float16)
+        else:
+            t = torch.empty((b * (d // 2), parts * 8 * (cpad // 8), h // 2, w // 2, 8), device=device, dtype=torch.float16)
+        act.operands[layout] = (t, cpad)
+        args += [t.data_ptr(), layout, cpad]
+    return act, args + [None, 0, 0] * (2 - len(operands))
+
+
 class BlockedActivation:
-    """An activation that exists only in the blocked layout (the output of a custom layer whose sole consumer is the
-    next custom layer, e.g. Unet_3D.dec5 -> dec6).  Quacks like the NCDHW tensor for the dispatch checks; ncdhw()
-    materialises it if a consumer turns out to need the plain layout."""
+    """An activation that exists only in the fp32 blocked layout [B*D, C/4, H, W, 4].  Quacks like the NCDHW tensor for
+    the dispatch checks: the custom layers read its blocked tensor directly, and ncdhw() materialises it for a layer that
+    needs the plain layout."""
     is_cuda, dtype, requires_grad = True, torch.float32, False
 
     def __init__(self, y, batch, channels):
@@ -366,6 +458,7 @@ def _cached_blocked(x):
 
 def _blocked_f32(x):
     """fp32 group-of-4 blocked view of an NCDHW tensor: the cached one if x came out of a custom layer"""
+    _fp32_only(x)
     y = _cached_blocked(x)
     if y is not None and y.shape[1] * 4 >= x.shape[1] and y.shape[0] == x.shape[0] * x.shape[2] \
             and (y.shape[1] - 1) * 4 < x.shape[1] + 4 and x.shape[1] % 4 == 0:
@@ -524,9 +617,10 @@ def _convt_supported(shape_bcdhw, module):
             and c % (2 * _group()) == 0 and module.out_channels <= 64)
 
 
-def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0):
+def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0, operands=None):
     """Run the kernel on blocked operands (fp32 groups of 4 or fp16 groups of 8, matching PRECISION); returns the
-    blocked fp32 output [B*2D, cgo, 2H, 2W, 4], or None when `bn` needs batch statistics."""
+    blocked fp32 output [B*2D, cgo, 2H, 2W, 4], or None when `bn` needs batch statistics.  operands: [(layout, cpad)] ->
+    the output is written only as those fp16 operands of the next layers (an OperandActivation) in the fp16 modes."""
     src0, src1 = _x3_operands(src0, src1)
     bd, cg0, h, w, _ = src0.shape
     cg1 = src1.shape[1] if src1 is not None else 0
@@ -540,18 +634,30 @@ def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0):
     aff = _affine(module, bn, npad, dev)
     if aff is None:
         return None
-    out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=dev, dtype=torch.float32)
+    operands = _operand_request(operands)
+    if operands:
+        act, dst = _operand_destinations(operands, (batch, cout, 2 * (bd // batch), 2 * h, 2 * w), dev)
+    else:
+        out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=dev, dtype=torch.float32)
+    src1_ptr = src1.data_ptr() if src1 is not None else None
+    op = _op_flag() if g == 8 or _x3() else 0
     if merged:
         # the four (y,x) parity classes share one MMA stream: N = 4 x 20 columns (csrc/convt3d.cu MODE 2)
         wpack = _pack(module, ("convt_merged", 20, g), lambda wt: pack_convt_merged_weights(wt, 20, g), 2)
-        _lib.call("genre_b200_convt3d_s2_merged_forward", src0.data_ptr(), cg0, src1.data_ptr() if src1 is not None else None,
-                  cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, _op_flag() if g == 8 or _x3() else 0, aff[0].data_ptr(),
-                  aff[1].data_ptr(), float(slope), out.data_ptr(), cgo, _lib.stream_ptr(src0))
+        head = (src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, op, aff[0].data_ptr(),
+                aff[1].data_ptr(), float(slope))
+        if operands:
+            _lib.call("genre_b200_convt3d_s2_merged_forward_operands", *head, cgo, *dst, _lib.stream_ptr(src0))
+            return act
+        _lib.call("genre_b200_convt3d_s2_merged_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(src0))
         return out
     wpack = _pack(module, ("convt", npad, g), lambda wt: pack_convt_weights(wt, npad, g), 4)
-    _lib.call("genre_b200_convt3d_s2_forward", src0.data_ptr(), cg0, src1.data_ptr() if src1 is not None else None, cg1,
-              batch, bd // batch, h, w, wpack.data_ptr(), module.kernel_size[0], npad, _op_flag() if g == 8 or _x3() else 0,
-              aff[0].data_ptr(), aff[1].data_ptr(), float(slope), out.data_ptr(), cgo, _lib.stream_ptr(src0))
+    head = (src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w, wpack.data_ptr(), module.kernel_size[0], npad, op,
+            aff[0].data_ptr(), aff[1].data_ptr(), float(slope))
+    if operands:
+        _lib.call("genre_b200_convt3d_s2_forward_operands", *head, cgo, *dst, _lib.stream_ptr(src0))
+        return act
+    _lib.call("genre_b200_convt3d_s2_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(src0))
     return out
 
 
@@ -810,27 +916,39 @@ def _affine(m, bn, npad, dev):
     return out
 
 
-def _conv_k4s2(x, m, bn, slope):
+def _k4s2_cpad(cin):
+    """channels per parity sub-volume of the conv3d_k4s2 operand: a K chunk (2 channel groups) must not straddle sub-volumes"""
+    g = _group()
+    return (cin + 2 * g - 1) // (2 * g) * (2 * g)
+
+
+def _conv_k4s2(x, m, bn, slope, operands=None):
     cout = m.out_channels
     npad = 32 * ((cout + 31) // 32)
     aff = _affine(m, bn, npad, x.device)
     if aff is None:
         return None
     g = _group()
-    cin = x.shape[1]
-    cpad = (cin + 2 * g - 1) // (2 * g) * (2 * g)      # a K chunk (2 channel groups) must not straddle sub-volumes
+    cpad = _k4s2_cpad(x.shape[1])
     wpack = _pack(m, ("k4s2", cpad, npad, g), lambda w: pack_conv_k4s2_weights(w, cpad, npad, g), 1)
-    if _x2_direct(x):
+    if isinstance(x, OperandActivation):
+        xb = x.operand(PARITY, cpad)[0]
+    elif _x2_direct(x):
         xb = space_to_depth_sources(x, cpad, 16, torch.float16)
     else:
         xb = _finish_operand(space_to_depth_sources(x, cpad, _act_group(), torch.float16 if _f16() else None))
     b = x.shape[0]
     bd, _, h, wd, _ = xb.shape
     cgo = (cout + 3) // 4
+    head = (xb.data_ptr(), cpad // g, 3 if _x3() else 1, b, bd // b, h, wd, wpack.data_ptr(), npad, _op_flag(), aff[0].data_ptr(),
+            aff[1].data_ptr(), 1.0 if slope is None else float(slope))
+    operands = _operand_request(operands)
+    if operands:
+        act, dst = _operand_destinations(operands, (b, cout, bd // b, h, wd), x.device)
+        _lib.call("genre_b200_conv3d_k4s2_forward_operands", *head, cgo, *dst, _lib.stream_ptr(xb))
+        return act
     out = torch.empty((bd, cgo, h, wd, 4), device=x.device, dtype=torch.float32)
-    _lib.call("genre_b200_conv3d_k4s2_forward", xb.data_ptr(), cpad // g, 3 if _x3() else 1, b, bd // b, h, wd, wpack.data_ptr(), npad,
-              _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
-              out.data_ptr(), cgo, _lib.stream_ptr(x))
+    _lib.call("genre_b200_conv3d_k4s2_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(xb))
     return from_blocked(out, b, cout)
 
 
@@ -898,7 +1016,7 @@ def _flat_common(m):
 
 
 def _flat_source_ok(x):
-    return torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and x.shape[1] % 8 == 0
+    return (torch.is_tensor(x) or isinstance(x, OperandActivation)) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and x.shape[1] % 8 == 0
 
 
 def _flat_convt_supported(sources, m):
@@ -915,6 +1033,7 @@ def _flat_conv_supported(x, m):
 
 
 def _flat_run(sources, m, bn, slope, transposed):
+    _fp32_only(*sources)
     cout = m.out_channels
     npad = flat_npad(cout)
     dev = sources[0].device
@@ -1214,11 +1333,17 @@ def _train_forward(x, m, supported):
     return _ConvForward.apply(x, m.weight, m.bias, m)
 
 
-def conv3d(x, m, bn=None, slope=None):
+def conv3d(x, m, bn=None, slope=None, operands=None):
     """Conv3d on the tensor-core kernel [+ folded eval BatchNorm3d + LeakyReLU]: k=8,s=2,p=3 on few input channels
-    (Unet_3D.enc1) via space-to-depth, or k=4,s=2,p=1 (discriminator, Unet_3D.enc2/enc3) via parity sub-volumes."""
+    (Unet_3D.enc1) via space-to-depth, or k=4,s=2,p=1 (discriminator, Unet_3D.enc2/enc3) via parity sub-volumes.
+    operands: [(layout, cpad)] of the consumers (conv_operand_layout / deconv_operand_layout): enc1 and the k4 s2 layers then
+    return the output as an OperandActivation."""
     if not x.is_cuda:
         return None
+    if isinstance(x, OperandActivation):
+        if _flat_conv_supported(x, m) or not (_no_autograd(x, m.weight, m.bias) and _conv_k4s2_supported(x, m)):
+            _fp32_only(x)
+        return _conv_k4s2(x, m, bn, slope, operands)
     if _needs_grad(x, m.weight, m.bias):
         if bn is not None or slope is not None:
             return None     # fused epilogues are inference-only; the caller falls back to module-by-module
@@ -1230,7 +1355,7 @@ def conv3d(x, m, bn=None, slope=None):
     if _flat_conv_supported(x, m):
         return _flat_run((x,), m, bn, slope, False)
     if _conv_k4s2_supported(x, m):
-        return _conv_k4s2(x, m, bn, slope)
+        return _conv_k4s2(x, m, bn, slope, operands)
     if _conv_k4s2_s2d_supported(x, m):
         return _conv_k4s2_s2d(x, m, bn, slope)
     if not _conv_k8s2_supported(x, m):
@@ -1250,10 +1375,15 @@ def conv3d(x, m, bn=None, slope=None):
             xb = _finish_operand(space_to_depth4_blocked(x, _act_group(), torch.float16 if _f16() else None))
         bd, cg, h, w, _ = xb.shape
         cgo = (cout + 3) // 4
+        head = (xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(), 80 if split_z else 160, _op_flag(),
+                aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope))
+        operands = _operand_request(operands)
+        if operands:   # output class q at coarse position j is enc2's parity sub-volume q at j
+            act, dst = _operand_destinations(operands, (b, cout, 2 * (bd // b), 2 * h, 2 * w), x.device)
+            _lib.call("genre_b200_conv3d_k8s2_s4d_forward_operands", *head, cgo, *dst, _lib.stream_ptr(x))
+            return act
         out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=x.device, dtype=torch.float32)
-        _lib.call("genre_b200_conv3d_k8s2_s4d_forward", xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(), 80 if split_z else 160,
-                  _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
-                  out.data_ptr(), cgo, _lib.stream_ptr(x))
+        _lib.call("genre_b200_conv3d_k8s2_s4d_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(x))
         return from_blocked(out, b, cout)
     cout, npad = m.out_channels, 32
     aff = _affine(m, bn, npad, x.device)
@@ -1276,26 +1406,28 @@ def conv3d(x, m, bn=None, slope=None):
 
 
 def _operand_of(x):
-    """blocked operand of the tensor-core kernels for activation x (NCDHW tensor or BlockedActivation) in the current
-    PRECISION, reusing the fp32 blocked twin a previous custom layer left behind; (operand, padded channels) or None"""
+    """blocked operand of the tensor-core kernels for activation x (NCDHW tensor, BlockedActivation or OperandActivation) in
+    the current PRECISION, reusing the fp32 blocked twin a previous custom layer left behind; (operand, padded channels) or None"""
+    if isinstance(x, OperandActivation):
+        return x.operand(PLAIN, -(-x.shape[1] // 8) * 8)
     c = x.shape[1]
     twin = _cached_blocked(x)
     if _x2():       # fp16 hi/lo parts of the (zero-padded) fp32 blocked tensor
         if twin is None:
-            if c % 4 != 0 or isinstance(x, BlockedActivation):
+            if c % 4 != 0:
                 return None
             twin = to_blocked(x, 4)
         return _split2(twin), ((twin.shape[1] + 1) // 2) * 8
     if not _f16():
         if twin is not None:
             return twin, twin.shape[1] * 4
-        return (to_blocked(x, 4), c) if c % 4 == 0 and not isinstance(x, BlockedActivation) else None
+        return (to_blocked(x, 4), c) if c % 4 == 0 else None
     if twin is not None:
         bd, cg4, h, w, _ = twin.shape
         out = torch.empty((bd, (cg4 + 1) // 2, h, w, 8), device=twin.device, dtype=torch.float16)
         _lib.call("genre_b200_blocked_f32_to_f16", twin.data_ptr(), cg4, bd, h, w, out.data_ptr(), _lib.stream_ptr(twin))
         return out, out.shape[1] * 8
-    return (to_blocked(x, 8, torch.float16), c) if c % 8 == 0 and not isinstance(x, BlockedActivation) else None
+    return (to_blocked(x, 8, torch.float16), c) if c % 8 == 0 else None
 
 
 def convt_c1_tc(inputs, m, sigmoid=False):
@@ -1334,15 +1466,20 @@ def convt_c1_tc(inputs, m, sigmoid=False):
     return out
 
 
+def _convt_c1_col2im_supported(inputs, m):
+    x0 = inputs[0]
+    return ("convt_c1_col2im" in POLICY and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
+            and tuple(m.padding) == (1, 1, 1) and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1)
+            and m.groups == 1 and m.out_channels == 1 and len(inputs) <= 2
+            and all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 5 and t.shape[2:] == x0.shape[2:] for t in inputs)
+            and x0.shape[4] == 64 and x0.shape[3] % 8 == 0 and x0.shape[0] <= 65535 and _no_autograd(*inputs, m.weight, m.bias))
+
+
 def convt_c1_col2im(inputs, m):
     """ConvTranspose3d(Cin -> 1, k4, s2, p1) over the channel concatenation of `inputs` on 64-wide volumes: tap GEMM + col2im
     (csrc/convt_c1_col2im.cu); NCDHW [B,1,2D,2H,128] or None if not covered."""
     x0 = inputs[0]
-    if not ("convt_c1_col2im" in POLICY and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
-            and tuple(m.padding) == (1, 1, 1) and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1)
-            and m.groups == 1 and m.out_channels == 1 and len(inputs) <= 2
-            and all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 5 and t.shape[2:] == x0.shape[2:] for t in inputs)
-            and x0.shape[4] == 64 and x0.shape[3] % 8 == 0 and x0.shape[0] <= 65535 and _no_autograd(*inputs, m.weight, m.bias)):
+    if not _convt_c1_col2im_supported(inputs, m):
         return None
     ops = [_operand_of(t) for t in inputs]
     if any(o is None for o in ops):
@@ -1402,6 +1539,7 @@ def convt_c1(src0, src1, batch, m):
 def conv_transpose3d(x, m, bn=None, slope=None):
     """ConvTranspose3d [-> eval-mode BatchNorm3d folded into the epilogue -> ReLU / LeakyReLU(slope)]; None if not covered
     (the caller then runs the plain modules)."""
+    _fp32_only(x)
     if x.is_cuda and not isinstance(x, BlockedActivation) and _needs_grad(x, m.weight, m.bias):
         if bn is not None or slope is not None or x.dim() != 5:
             return None
@@ -1414,9 +1552,9 @@ def conv_transpose3d(x, m, bn=None, slope=None):
             y = convt_c1_tc((x,), m)
         if y is not None:
             return y
-    if not isinstance(x, BlockedActivation) and _skinny_convt_supported(x, m):
+    if _skinny_convt_supported(x, m):
         return _skinny_run(x, m, bn, slope, True)
-    if not isinstance(x, BlockedActivation) and _flat_convt_supported((x,), m):
+    if _flat_convt_supported((x,), m):
         return _flat_run((x,), m, bn, slope, True)
     if (bn is None and slope is None and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
             and _convt_c1_supported(x.shape[1], x.shape[2:], m, (x,)) and _no_autograd(x, m.weight, m.bias)):
@@ -1521,9 +1659,17 @@ def fused_block(x, conv, bn, act):
     return conv3d(x, conv, bn, slope)
 
 
-def deconv_skip(x, skip, conv, bn=None, slope=None, keep_blocked=False):
+def _deconv_kernel_supported(x, skip, conv):
+    """deconv_skip's condition for the halo kernel (convt3d_s2_blocked)"""
+    return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and skip.shape[2:] == x.shape[2:]
+            and x.shape[1] % _group() == 0 and skip.shape[1] % _group() == 0
+            and _convt_supported((x.shape[0], x.shape[1] + skip.shape[1]) + tuple(x.shape[2:]), conv)
+            and _no_autograd(x, skip, conv.weight, conv.bias))
+
+
+def deconv_skip(x, skip, conv, bn=None, slope=None, operands=None):
     """cat(x, skip) -> ConvTranspose3d [-> eval-mode BatchNorm3d folded into the epilogue -> LeakyReLU(slope)] with the
-    concatenation walked as two K ranges instead of being materialised.  None if not covered."""
+    concatenation walked as two K ranges instead of being materialised.  None if not covered.  operands: as conv3d's."""
     if bn is None and conv.out_channels == 1:
         y = convt_c1_col2im((x, skip), conv)
         if y is None:
@@ -1543,17 +1689,16 @@ def deconv_skip(x, skip, conv, bn=None, slope=None, keep_blocked=False):
         return _skinny_run(xc, conv, bn, slope, True) if _skinny_convt_supported(xc, conv) else None
     if _flat_convt_supported((x, skip), conv):
         return _flat_run((x, skip), conv, bn, slope, True)
-    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and skip.shape[2:] == x.shape[2:]
-            and x.shape[1] % _group() == 0 and skip.shape[1] % _group() == 0
-            and _convt_supported((x.shape[0], x.shape[1] + skip.shape[1]) + tuple(x.shape[2:]), conv)
-            and _no_autograd(x, skip, conv.weight, conv.bias)):
+    if not _deconv_kernel_supported(x, skip, conv):
+        _fp32_only(x, skip)
         return None
     if bn is not None and (bn.training or not bn.track_running_stats):
+        _fp32_only(x, skip)
         return None  # batch statistics need the un-normalised output first
     # the concatenation stays two K ranges (a K chunk of 2 channel groups may straddle them: the halo producer picks the
     # source per channel group)
     a, bsrc = _to_operand(x), _to_operand(skip)
-    y = convt3d_s2_blocked(a, bsrc, x.shape[0], conv, bn, 1.0 if slope is None else slope)
-    if keep_blocked:
-        return BlockedActivation(y, x.shape[0], conv.out_channels)
+    y = convt3d_s2_blocked(a, bsrc, x.shape[0], conv, bn, 1.0 if slope is None else slope, operands)
+    if isinstance(y, OperandActivation):
+        return y
     return from_blocked(y, x.shape[0], conv.out_channels)

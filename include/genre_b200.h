@@ -190,6 +190,38 @@ int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, i
                                   const float *scale, const float *shift, float slope,
                                   float *out, int cgo, void *stream);
 
+/* Operand outputs.  The *_forward_operands variants of genre_b200_convt3d_s2_forward, genre_b200_convt3d_s2_merged_forward,
+ * genre_b200_conv3d_k8s2_s4d_forward and genre_b200_conv3d_k4s2_forward take the same arguments with `out` replaced by up to
+ * two destinations (dst1 may be NULL) of the fp16 operand the NEXT layers read, so that no layout pass runs between them.
+ * f16 = 2: parts = 2, hi = fp16(a) | lo' = fp16((a - hi) * 2^11) (the fp32-accurate mode; bit-identical to
+ * genre_b200_blocked_split2_f16 of the fp32 output); f16 = 1: parts = 1, fp16(a).  With the output extent Do, Ho, Wo:
+ *   layout 1 (plain)   dst [B*Do][parts][cpad/8][Ho][Wo][8 fp16]
+ *   layout 2 (parity)  dst [B*Do/2][parts][8 s][cpad/8][Ho/2][Wo/2][8 fp16], s = ((z&1)*2 + (y&1))*2 + (x&1): the parity
+ *                      sub-volumes of a following conv3d_k4s2 (= genre_b200_ncdhw_to_blocked mode 2 with group 16)
+ * Channels from 4*cgo up to cpad (a multiple of 8, >= 4*cgo) are written as zeros on every call. */
+int genre_b200_convt3d_s2_forward_operands(const void *src0, int cg0, const void *src1, int cg1,
+                                           int64_t B, int64_t D, int64_t H, int64_t W,
+                                           const void *wpack, int ksize, int npad, int f16,
+                                           const float *scale, const float *shift, float slope, int cgo,
+                                           void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                           void *stream);
+int genre_b200_convt3d_s2_merged_forward_operands(const void *src0, int cg0, const void *src1, int cg1,
+                                                  int64_t B, int64_t D, int64_t H, int64_t W,
+                                                  const void *wpack, int ksize, int npad, int f16,
+                                                  const float *scale, const float *shift, float slope, int cgo,
+                                                  void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                                  void *stream);
+int genre_b200_conv3d_k8s2_s4d_forward_operands(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
+                                                const void *wpack, int npad, int f16,
+                                                const float *scale, const float *shift, float slope, int cgo,
+                                                void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                                void *stream);
+int genre_b200_conv3d_k4s2_forward_operands(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
+                                            const void *wpack, int npad, int f16,
+                                            const float *scale, const float *shift, float slope, int cgo,
+                                            void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                            void *stream);
+
 /* Stride-1 convolution with `taps` (3 or 5) taps per dimension on channel-blocked activations, same wgmma kernel:
  *   out[b,z,y,x,n] = act(scale[n] * sum_{t,c} in[b, z+base-tz, y+base-ty, x+base-tx, c] * W[t][c][n] + shift[n])
  * Replaces the cuDNN call behind nn.Conv3d of Unet_3D.enc1 (networks/networks.py:151,197: Conv3d(2->20, k=8, s=2, p=3))

@@ -94,6 +94,7 @@ _SIGNATURES = {
     "genre_b200_voxel_stats": [_ptr, _ptr, _i64, _int, _int, _int, _int, _int, _f64, _f64, _ptr, _ptr, _ptr],
     "genre_b200_voxel_downsample": [_ptr, _i64, _int, _int, _int, _ptr, _ptr],
     "genre_b200_voxel_translate": [_ptr, _i64, _int, _int, _int, _ptr, _ptr, _ptr, _ptr],
+    "genre_b200_surface_sample": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _size, _ptr],
 }
 
 # every symbol include/genre_b200.h declares (tests check the library exports all of them)
@@ -102,7 +103,8 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_convt_c1_wgrad_workspace_bytes", "genre_b200_conv_k8s2_wgrad_workspace_bytes",
     "genre_b200_bn_workspace_bytes", "genre_b200_render_spherical_workspace_bytes",
     "genre_b200_voxel_surface_workspace_bytes", "genre_b200_conv_set_tma", "genre_b200_conv_set_cluster", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
-    "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes"])
+    "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
+    "genre_b200_surface_sample_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
@@ -126,6 +128,7 @@ _LAUNCHES = {
     "genre_b200_raycast_count": 3, "genre_b200_raycast_build": 2, "genre_b200_raycast_first_hit": 1,
     "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
     "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,
+    "genre_b200_surface_sample": 3,
 }
 
 
@@ -172,6 +175,8 @@ def load():
     lib.genre_b200_raycast_workspace_bytes.argtypes = [_i64, _int]
     lib.genre_b200_voxel_fill_workspace_bytes.restype = _size
     lib.genre_b200_voxel_fill_workspace_bytes.argtypes = [_i64, _int, _int, _int]
+    lib.genre_b200_surface_sample_workspace_bytes.restype = _size
+    lib.genre_b200_surface_sample_workspace_bytes.argtypes = [_i64, _i64]
     _lib = lib
     return lib
 

@@ -13,6 +13,9 @@ the device.
 ``voxel_fill`` / ``voxel_transform`` / ``find_bound`` / ``bounding_box_align`` / ``translate`` / ``downsample`` / ``voxel_iou``
 are the reference's voxel toolkit (util/util_voxel.py: exterior fill, affine resampling, bounding boxes, integer shifts and
 pooling) plus the IoU an evaluation computes from them, batched on the device.
+
+``sample_surface`` / ``chamfer_fscore`` / ``voxel_metrics`` evaluate predicted grids by the Chamfer distance and F-score of
+points drawn from their surfaces (the metric of the reference's nndistance op), batched on the device.
 """
 import numpy as np
 import torch
@@ -510,3 +513,121 @@ def voxel_iou(pred, gt, threshold=0.5, gt_threshold=0.5, pool=1, pool_mode="max"
     union = counts[:, 0] + counts[:, 1] - counts[:, 2]
     iou = torch.where(union > 0, counts[:, 2].double() / union.clamp(min=1).double(), torch.ones_like(union, dtype=torch.float64))
     return iou.float(), counts
+
+
+# ---- surface sampling and point-set metrics: Chamfer distance and F-score of predicted voxel grids -------------------------
+def _seeds(seed, n, device):
+    """[n] int64 on the device holding the uint64 seeds: seed + b (wrapping) for an int, else a [n] integer tensor"""
+    if isinstance(seed, torch.Tensor):
+        if seed.shape != (n,) or seed.dtype != torch.int64:
+            raise ValueError("seed: expected an int or a [%d] int64 tensor, got %s %s" % (n, seed.dtype, tuple(seed.shape)))
+        return seed.to(device).contiguous()
+    s = int(seed) % (1 << 64)
+    return torch.arange(n, dtype=torch.int64, device=device).add_(s - (1 << 64) if s >= 1 << 63 else s)
+
+
+def sample_surface(verts, faces, vert_off, face_off, n, seed=0):
+    """``n`` points per sample drawn uniformly by area from every sample's triangle mesh, on the device.
+
+    verts [V,3] fp32, faces [F,3] int32 (indices into the sample's own vertex block), vert_off / face_off [B+1] int64: the
+    packed meshes ``marching_cubes`` returns.  ``seed`` is an int (sample b uses seed + b) or a [B] int64 tensor of per-sample
+    seeds (read as uint64).  Returns (points [B,n,3] fp32, face [B,n] int32 local to the sample).  A face is drawn with
+    probability proportional to its area, quantised to 32 bits relative to the sample's largest face, so a face of zero area
+    is never drawn; the point is uniform inside it.  A sample without a face of non-zero area gets NaN points and face -1.
+
+    Every step is in integers or in fp64 / fp32 with one stated rounding per operation (include/genre_b200.h), so the result
+    is deterministic, does not depend on the rest of the batch, and equals the numpy restatement in
+    tests/surface_sample_ref.py bit for bit.  Nothing is copied to the host."""
+    _lib.require_cuda(verts, faces, vert_off, face_off)
+    _lib.require_f32(verts)
+    if faces.dtype != torch.int32 or vert_off.dtype != torch.int64 or face_off.dtype != torch.int64:
+        raise TypeError("sample_surface expects int32 faces and int64 offsets, got %s, %s, %s" % (faces.dtype, vert_off.dtype,
+                                                                                                 face_off.dtype))
+    b = vert_off.numel() - 1
+    if b < 1 or face_off.numel() != b + 1 or verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("sample_surface: verts [V,3], faces [F,3] and offsets [B+1] expected, got %s, %s, %s, %s"
+                         % (tuple(verts.shape), tuple(faces.shape), tuple(vert_off.shape), tuple(face_off.shape)))
+    n = int(n)
+    if n < 1:
+        raise ValueError("sample_surface: n = %d points per sample, at least 1 expected" % n)
+    nbytes = _lib.load().genre_b200_surface_sample_workspace_bytes(b, faces.shape[0])
+    if nbytes == 0:
+        raise ValueError("sample_surface: %d meshes with %d faces unsupported (1 <= B <= 65535, fewer than 2^31 faces)"
+                         % (b, faces.shape[0]))
+    dev = verts.device
+    verts, faces, vert_off, face_off = verts.contiguous(), faces.contiguous(), vert_off.contiguous(), face_off.contiguous()
+    seeds = _seeds(seed, b, dev)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    points = torch.empty((b, n, 3), dtype=torch.float32, device=dev)
+    face = torch.empty((b, n), dtype=torch.int32, device=dev)
+    _lib.call("genre_b200_surface_sample", verts.data_ptr(), verts.shape[0], faces.data_ptr(), faces.shape[0],
+              vert_off.data_ptr(), face_off.data_ptr(), b, seeds.data_ptr(), n, points.data_ptr(), face.data_ptr(),
+              ws.data_ptr(), nbytes, _lib.stream_ptr(verts))
+    return points, face
+
+
+def chamfer_fscore(p, q, tau=0.01):
+    """Per-sample Chamfer distance and F-score of two batches of point sets, by the nearest-neighbour kernel of ``nndistance``.
+
+    p [B,N,3] (e.g. points on the prediction) and q [B,M,3] (points on the ground truth), fp32 on CUDA, no NaNs.  With d the
+    fp32 squared distance from a point to its nearest neighbour in the other set (exactly ``nndistance``'s), and its square
+    root and everything after it in fp64, returns a dict of [B] fp64 tensors:
+      acc = mean sqrt(d(p -> q)),  comp = mean sqrt(d(q -> p)),  chamfer = (acc + comp) / 2,
+      precision = (the number of p's points with sqrt(d) <= tau) / N,  recall = the same for q's points over M,
+      fscore = 2 precision recall / (precision + recall), 0 when both are 0.
+    The reference's ``nndistance_score`` (toolbox/nndistance/functions/nnd.py) is acc + comp = 2 * chamfer, up to its
+    eps = 1e-10 under the square root.  Nothing is copied to the host."""
+    _lib.require_cuda(p, q)
+    _lib.require_f32(p, q)
+    if p.dim() != 3 or q.dim() != 3 or p.shape[2] != 3 or q.shape[2] != 3 or p.shape[0] != q.shape[0]:
+        raise ValueError("chamfer_fscore: p [B,N,3] and q [B,M,3] expected, got %s and %s" % (tuple(p.shape), tuple(q.shape)))
+    b, n, m = p.shape[0], p.shape[1], q.shape[1]
+    p, q = p.contiguous(), q.contiguous()
+    d1 = torch.empty((b, n), dtype=torch.float32, device=p.device)
+    d2 = torch.empty((b, m), dtype=torch.float32, device=p.device)
+    i1 = torch.empty((b, n), dtype=torch.int32, device=p.device)
+    i2 = torch.empty((b, m), dtype=torch.int32, device=p.device)
+    _lib.call("genre_b200_nnd_forward", p.data_ptr(), q.data_ptr(), b, n, m, d1.data_ptr(), d2.data_ptr(), i1.data_ptr(),
+              i2.data_ptr(), _lib.stream_ptr(p))
+    s1, s2 = d1.double().sqrt(), d2.double().sqrt()
+    acc, comp = s1.mean(1), s2.mean(1)
+    c1, c2 = (s1 <= tau).sum(1).double(), (s2 <= tau).sum(1).double()
+    prec, rec = c1 / torch.full_like(c1, n), c2 / torch.full_like(c2, m)   # a true division (by a scalar, torch multiplies)
+    both = prec + rec
+    fscore = torch.where(both > 0, 2 * prec * rec / torch.where(both > 0, both, torch.ones_like(both)), torch.zeros_like(both))
+    return {"acc": acc, "comp": comp, "chamfer": (acc + comp) / 2, "precision": prec, "recall": rec, "fscore": fscore}
+
+
+def voxel_metrics(pred, gt, level=0.5, gt_level=0.5, n_points=1024, tau=0.01, seed=0):
+    """Surface metrics of predicted voxel grids against ground-truth grids, batched on the device.
+
+    pred, gt [B,1,D,H,W] or [B,D,H,W] fp32 values (not logits) of the same shape.  The protocol, stated because it is not
+    the one behind any published table (the Pix3D evaluation's point count, normalisation, alignment and iso level are not
+    known here):
+      * meshes: ``marching_cubes`` of pred at ``level`` and of gt at ``gt_level``, spacing 1/dim and shift 0.5 - 0.5/dim per
+        axis, so the voxel centres sit in the centred unit cube [-0.5, 0.5]^3;
+      * points: ``sample_surface`` with ``n_points`` per mesh and the same seeds for both meshes (``seed`` as there), so
+        identical grids give identical points and a Chamfer distance of exactly 0;
+      * metrics: ``chamfer_fscore(points on pred, points on gt, tau)`` (tau in the unit cube's units), plus ``iou`` of
+        pred > level and gt > gt_level from ``voxel_iou``.
+    Returns the dict of ``chamfer_fscore`` with ``iou`` added (all [B] fp64) and ``valid`` [B] bool, False where either surface
+    is empty (no face of non-zero area); those samples get NaN surface metrics (their IoU is still defined) and their NaN
+    points never reach the nearest-neighbour kernel.  The two marching-cubes calls synchronise once each, as documented
+    there; nothing else does."""
+    a, g = _volumes(pred, "voxel_metrics"), _volumes(gt, "voxel_metrics")
+    if a.shape != g.shape:
+        raise ValueError("voxel_metrics: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(g.shape)))
+    b, dims = a.shape[0], a.shape[1:]
+    spacing = [1.0 / s for s in dims]
+    shift = [0.5 - 0.5 / s for s in dims]
+    seeds = _seeds(seed, b, a.device)
+    pp, fp = sample_surface(*marching_cubes(a, level, spacing, shift), n_points, seeds)
+    pg, fg = sample_surface(*marching_cubes(g, gt_level, spacing, shift), n_points, seeds)
+    valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
+    keep = valid[:, None, None]
+    out = chamfer_fscore(torch.where(keep, pp, torch.zeros_like(pp)), torch.where(keep, pg, torch.zeros_like(pg)), tau)
+    nan = torch.full((b,), float("nan"), dtype=torch.float64, device=a.device)
+    out = {k: torch.where(valid, v, nan) for k, v in out.items()}
+    out["iou"] = voxel_iou(a, g, level, gt_level)[0].double()
+    out["valid"] = valid
+    return out

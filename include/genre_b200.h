@@ -577,6 +577,30 @@ int genre_b200_voxel_downsample(const float *vol, int64_t N, int R, int times, i
 int genre_b200_voxel_translate(const float *vol, int64_t N, int D, int H, int W, const int32_t *bounds, const int32_t *offsets,
                                float *out, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Area-weighted uniform surface sampling of batched triangle meshes: n points per sample, the step from a marching-cubes mesh
+ * to a Chamfer / F-score evaluation (the reference's nndistance op) without leaving the device.
+ *   meshes  the packed output of genre_b200_isosurface_*: verts [V, 3] fp32, faces [F, 3] int32 indexing the sample's own
+ *           vertex block, vert_off / face_off [N+1] int64 on the device.  F (the total) < 2^31, 1 <= N <= 65535.
+ *   weight  per face, fp64 from the fp32 vertices a, b, c, one rounding per operation, no contraction: e1 = b - a, e2 = c - a,
+ *           n = (e1y*e2z - e1z*e2y, e1z*e2x - e1x*e2z, e1x*e2y - e1y*e2x), s = sqrt((nx*nx + ny*ny) + nz*nz), a non-finite s
+ *           counting as 0.  smax_b = the sample's largest s; w = floor(ldexp(s / smax_b, 32)) as uint64 (all 0 when
+ *           smax_b = 0).  P = the inclusive prefix sums of w per sample (exact in uint64), T_b = the last one (0 without faces).
+ *   point i of sample b: r_j = splitmix64(seed_b + (3i + j + 1) * 0x9E3779B97F4A7C15), j = 0, 1, 2, in wrapping uint64
+ *           arithmetic (splitmix64's output function, spelled out in csrc/surface_sample.cu); the face is the smallest f with
+ *           P_f > mulhi64(r_0, T_b); U = r_1 >> 40, V = r_2 >> 40, replaced by 2^24 - U, 2^24 - V when U + V > 2^24;
+ *           u = U * 2^-24, v = V * 2^-24; per axis p = fl(fl(a + fl(u * fl(b - a))) + fl(v * fl(c - a))), no FMA.
+ *   seeds   [N] uint64 on the device.  n in [1, 2^30].
+ *   output  points [N, n, 3] fp32, face [N, n] int32 local to the sample; a sample with T_b = 0 gets NaN points and face -1.
+ *           A point depends only on (seed_b, i) and its own mesh: deterministic and batch-equivariant.
+ *           tests/surface_sample_ref.py restates the whole contract in numpy, bit for bit.
+ *   workspace: genre_b200_surface_sample_workspace_bytes(N, F) bytes (0: unsupported), 16-byte aligned, caller-owned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_surface_sample_workspace_bytes(int64_t N, int64_t F);
+int genre_b200_surface_sample(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                              const int64_t *face_off, int64_t N, const uint64_t *seeds, int64_t n, float *points,
+                              int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

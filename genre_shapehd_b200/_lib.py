@@ -95,6 +95,10 @@ _SIGNATURES = {
     "genre_b200_voxel_downsample": [_ptr, _i64, _int, _int, _int, _ptr, _ptr],
     "genre_b200_voxel_translate": [_ptr, _i64, _int, _int, _int, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_surface_sample": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _size, _ptr],
+    "genre_b200_crop_to_render": [_ptr, _ptr, _int, _ptr, _ptr, _int, _i64, _int, _f64, _f64, _ptr, _ptr, _ptr, _ptr, _size,
+                                  _ptr],
+    "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
+                              _size, _ptr],
 }
 
 # every symbol include/genre_b200.h declares (tests check the library exports all of them)
@@ -104,12 +108,14 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_bn_workspace_bytes", "genre_b200_render_spherical_workspace_bytes",
     "genre_b200_voxel_surface_workspace_bytes", "genre_b200_conv_set_tma", "genre_b200_conv_set_cluster", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
     "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
-    "genre_b200_surface_sample_workspace_bytes"])
+    "genre_b200_surface_sample_workspace_bytes", "genre_b200_crop_to_render_workspace_bytes",
+    "genre_b200_preprocess_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
 
-# how many of this library's KERNELS one call of each entry point launches (memset nodes not counted)
+# how many of this library's KERNELS one call of each entry point launches (memset nodes not counted); a callable takes the
+# call's arguments
 _LAUNCHES = {
     "genre_b200_cam_bp_forward": 2, "genre_b200_cam_bp_backward": 1, "genre_b200_surface_mask": 1,
     "genre_b200_sph_bp_forward": 2, "genre_b200_sph_bp_backward": 1, "genre_b200_calc_prob_forward": 1,
@@ -128,7 +134,9 @@ _LAUNCHES = {
     "genre_b200_raycast_count": 3, "genre_b200_raycast_build": 2, "genre_b200_raycast_first_hit": 1,
     "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
     "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,
-    "genre_b200_surface_sample": 3,
+    "genre_b200_surface_sample": 3, "genre_b200_crop_to_render": 2,
+    # min/max (not rgb) + cubic, + gray, mean and jitter for train-mode rgb
+    "genre_b200_preprocess": lambda kind, train, *_: 1 + (kind != 0) + (3 if kind == 0 and train else 0),
 }
 
 
@@ -177,6 +185,10 @@ def load():
     lib.genre_b200_voxel_fill_workspace_bytes.argtypes = [_i64, _int, _int, _int]
     lib.genre_b200_surface_sample_workspace_bytes.restype = _size
     lib.genre_b200_surface_sample_workspace_bytes.argtypes = [_i64, _i64]
+    lib.genre_b200_crop_to_render_workspace_bytes.restype = _size
+    lib.genre_b200_crop_to_render_workspace_bytes.argtypes = [_i64]
+    lib.genre_b200_preprocess_workspace_bytes.restype = _size
+    lib.genre_b200_preprocess_workspace_bytes.argtypes = [_int, _int, _i64, _int]
     _lib = lib
     return lib
 
@@ -189,7 +201,8 @@ def call(name, *args):
     if rc != 0:
         msg = lib.genre_b200_last_error()
         raise RuntimeError("%s failed (status %d): %s" % (name, rc, msg.decode() if msg else "?"))
-    launch_count += _LAUNCHES.get(name, 0)
+    n = _LAUNCHES.get(name, 0)
+    launch_count += n(*args) if callable(n) else n
 
 
 def stream_ptr(t):

@@ -601,6 +601,42 @@ int genre_b200_surface_sample(const float *verts, int64_t V, const int32_t *face
                               const int64_t *face_off, int64_t N, const uint64_t *seeds, int64_t n, float *points,
                               int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Input preprocessing: the test-time silhouette crop (util_img.get_bbox + util_img.crop of every preprocess_wrapper) and
+ * MarrnetBaseModel.preprocess (models/marrnetbase.py:71-126), batched.  fp64 in the reference's operation order, one
+ * rounding per operation, no FMA (fp32 only where stated); outputs rounded once to fp32, as convert_to_float32 does.
+ *   sources  packed: data (bytes) and desc [B, 4] int64 on the device, (byte offset, H, W, C) per sample, dtype 0 uint8 or
+ *            1 uint16, read as x / 255.0 or x / 65535.0; dense (desc NULL): [B, H, W, C] dtype 2 float32 or 3 float64.
+ *            C in {1, 3, 4}: masks, depth and silhou read channel 0, rgb and normal channels 0..2.  Descriptors are trusted.
+ *   crop     bbox = min / max row and column of mask > th (fp64); no such pixel: valid[b] = 0 and the sample's crops NaN.
+ *            Window as util_img.crop with pad_zero=False: y1, x1, y2, x2 = (min col, min row, max col, max row),
+ *            l = max(x2 - x1, y2 - y1) * out / (out - 2 pad), x1' = rint((x1 + x2) / 2 - l / 2), x2' = rint(... + l / 2),
+ *            likewise y; the window reads clamped image rows and columns (edge padding).  cv2 INTER_LINEAR of the
+ *            window (rows and columns scaled separately) to out x out: s = (d + 0.5) (n / out) - 0.5, taps floor(s) and
+ *            floor(s) + 1 clamped into the window, weights (1 - f, f), horizontal pass then vertical.  The photo's three
+ *            channels -> rgb [B, out, out, 3] fp64, the mask's channel 0 -> silhou [B, out, out] fp64 (or NULL).
+ *   preprocess  kind 0 rgb, 1 depth, 2 silhou, 3 normal -> out [B, 3 or 1, S, S] fp32, S = im_size.  Square sources only.
+ *            cv2 INTER_CUBIC n -> S: fx = (float)((d + 0.5) (1 / (S / n)) - 0.5), i = floor(fx), fx -= i, the four
+ *            A = -0.75 coefficients in fp32 (c3 = 1 - c0 - c1 - c2), taps i-1 .. i+2 clamped, fp64 sums in tap order,
+ *            horizontal then vertical.  depth / normal: clamp to the source's min and max (none if it holds a NaN), *
+ *            scale_25d; silhou: clamp, 1 if > 0.999 else 0, * scale_25d; rgb: (x - mean_c) / std_c (ImageNet), and in
+ *            train mode first the jitter steps order[b][k] (0 brightness, 1 contrast, 2 saturation) with alpha[b][k]:
+ *            x = a x + (1 - a) * {0, m, gray(x)}, gray = (0.299 r + 0.587 g) + 0.114 b, then x_c += noise[b][c].  m = the mean
+ *            of gray at the contrast step, summed in a fixed order (csrc/preprocess.cu).  order int32, alpha and noise fp64,
+ *            [B, 3] each on the device.  Results depend only on the sample's own inputs.
+ *            tests/preprocess_ref.py restates the whole contract in numpy, bit for bit.
+ *   workspace: the _workspace_bytes query's bytes (0: unsupported), 16-byte aligned, caller-owned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_crop_to_render_workspace_bytes(int64_t B);
+int genre_b200_crop_to_render(const void *img, const int64_t *img_desc, int img_dtype, const void *mask,
+                              const int64_t *mask_desc, int mask_dtype, int64_t B, int out_size, double pad, double th,
+                              double *rgb, double *silhou, uint8_t *valid, void *workspace, size_t workspace_bytes,
+                              void *stream);
+size_t genre_b200_preprocess_workspace_bytes(int kind, int train, int64_t B, int im_size);
+int genre_b200_preprocess(int kind, int train, const void *src, const int64_t *desc, int dtype, int64_t B, int64_t H,
+                          int64_t W, int64_t C, int im_size, double scale_25d, const int32_t *order, const double *alpha,
+                          const double *noise, float *out, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

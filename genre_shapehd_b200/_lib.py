@@ -106,7 +106,7 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_last_error", "genre_b200_version", "genre_b200_voxelize_workspace_bytes",
     "genre_b200_convt_c1_wgrad_workspace_bytes", "genre_b200_conv_k8s2_wgrad_workspace_bytes",
     "genre_b200_bn_workspace_bytes", "genre_b200_render_spherical_workspace_bytes",
-    "genre_b200_voxel_surface_workspace_bytes", "genre_b200_conv_set_tma", "genre_b200_conv_set_cluster", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
+    "genre_b200_voxel_surface_workspace_bytes", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
     "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
     "genre_b200_surface_sample_workspace_bytes", "genre_b200_crop_to_render_workspace_bytes",
     "genre_b200_preprocess_workspace_bytes"])
@@ -167,10 +167,6 @@ def load():
     lib.genre_b200_bn_workspace_bytes.argtypes = [_i64]
     lib.genre_b200_render_spherical_workspace_bytes.restype = _size
     lib.genre_b200_render_spherical_workspace_bytes.argtypes = [_i64, _int]
-    lib.genre_b200_conv_set_tma.restype = _int
-    lib.genre_b200_conv_set_tma.argtypes = [_int]
-    lib.genre_b200_conv_set_cluster.restype = _int
-    lib.genre_b200_conv_set_cluster.argtypes = [_int]
     lib.genre_b200_skinny_gemm_workspace_bytes.restype = _size
     lib.genre_b200_skinny_gemm_workspace_bytes.argtypes = [_i64, _i64, _i64, _int]
     lib.genre_b200_convflat_positions.restype = _i64

@@ -16,17 +16,16 @@
 // materialised).  Weights are pre-packed on the host into the exact shared-memory image of each (parity, z-tap,
 // K-chunk) stage and arrive with ONE cp.async.bulk per stage.
 //
-// CTA = one (b, z, 16 y-rows, 8*MT x-columns) output slab of one parity class: MT M-tiles of 128 rows.  Warps 0-3: halo
-// producers (cp.async 16 B, zero-fill = padding, or one thread issuing tensor copies), then epilogue (shared-memory
-// accumulator image -> scale/shift/LeakyReLU -> blocked store).  Warps 4-11: two consumer warpgroups, each issuing the
-// m64 wgmma of one half (8 y-rows) of every M-tile and holding its MT x NACC / 2 fp32 accumulators in registers, so
-// MT * NACC <= 256 (launch_convt_impl narrows the x tile until it fits).  After the last K step they store the
-// accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.
+// CTA = one (b, z, 16 y-rows, 8*MT x-columns) output slab of one parity class: MT M-tiles of 128 rows.  Warps 0-3: one
+// thread issues the halo tensor copies (out-of-range elements zero-filled = padding) and the weight copy of every stage, then
+// all four run the epilogue (shared-memory accumulator image -> scale/shift/LeakyReLU -> blocked store).  Warps 4-11: two
+// consumer warpgroups, each issuing the m64 wgmma of one half (8 y-rows) of every M-tile and holding its MT x NACC / 2 fp32
+// accumulators in registers, so MT * NACC <= 256 (launch_convt_impl narrows the x tile until it fits).  After the last K
+// step they store the accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.
 // Pipeline: STAGES-deep ring of (halo chunk, weight chunk) with full/empty mbarriers; every consumer warp arrives on a slot's
 // empty barrier once its wgmma that read the slot have completed.  With 3 or more stages a stage's MMAs stay in flight while
 // the next stage is awaited and issued (wgmma.wait_group 1): its slot is released after the next stage's MMAs are committed.
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (the entry point is resolved through the runtime: no -lcuda)
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -36,7 +35,6 @@ namespace gb {
 constexpr int CT_THREADS = 384;       // 4 producer/epilogue warps + 2 consumer warpgroups
 constexpr int CT_CONSUMER_WARPS = 8;
 constexpr int CT_ACC_COLS = 256;      // accumulator columns per CTA (MT * NACC): 128 fp32 registers per consumer thread
-constexpr int CT_PRODUCERS = 128;
 constexpr int CT_BY = 16;             // y rows per CTA (16 core-matrix groups of 8 x positions = M 128)
 constexpr int CT_KCG = 2;             // channel groups (of 4) per stage = one K=8 TF32 MMA per tap and M-tile
 
@@ -104,18 +102,17 @@ __device__ __forceinline__ void store_operand(const ConvTParams &p, int k, int b
 // truncates: a step's error scales with the partial sum it joins, and the cross terms would otherwise ride on the big one),
 // and the epilogue returns acc_hi + 2^-11 * acc_cross.  The first two could be one N = 2*NPAD MMA, but the third would then
 // write into half of its registers, which makes ptxas serialize every wgmma of the kernel.
-// TMA: the halo of a channel group arrives as ONE cp.async.bulk.tensor (5-D tiled tensor map over [plane][cg][H][W][16 B], box
-// [1][1][PY][PX][16 B], out-of-bounds elements zero-filled = the convolution's padding) instead of PY*PX 16-byte cp.async
-// issued by 128 threads; each channel group then starts on a 128-byte boundary of shared memory (the LBO of the A descriptor
-// is that padded stride).
-template <int T, int NPAD, int MT, bool X2 = false, bool TMA = false>
+// The halo of a channel group arrives as ONE cp.async.bulk.tensor (5-D tiled tensor map over [plane][cg][H][W][16 B], box
+// [1][1][PY][PX][16 B], out-of-bounds elements zero-filled = the convolution's padding); each channel group starts on a
+// 128-byte boundary of shared memory (the LBO of the A descriptor is that padded stride).
+template <int T, int NPAD, int MT, bool X2 = false>
 struct ConvTCfg {
   static constexpr int W = 8 * MT;
   static constexpr int PY = CT_BY + T - 1, PX = W + T - 1;     // halo extent
   static constexpr int PARTS = X2 ? 2 : 1;
   static constexpr int NACC = PARTS * NPAD;                    // accumulator columns per M-tile = width of the B operand
   static constexpr int A_CG_BYTES = PY * PX * 16;              // one channel group of the halo
-  static constexpr int A_CG_STRIDE = TMA ? ((A_CG_BYTES + 127) / 128) * 128 : A_CG_BYTES;   // its pitch in shared memory = LBO of A
+  static constexpr int A_CG_STRIDE = ((A_CG_BYTES + 127) / 128) * 128;   // its pitch in shared memory = LBO of A
   static constexpr int A_BYTES = PARTS * CT_KCG * A_CG_STRIDE; // [part][channel group][halo]
   static constexpr int A_TX_BYTES = PARTS * CT_KCG * A_CG_BYTES;  // bytes the tensor copies of one stage deliver
   static constexpr int B_TAP_BYTES = 2 * (NACC / 8) * 128;     // one (y,x) tap: [2 kcore][NACC/8][8 rows][16 B]
@@ -136,8 +133,6 @@ struct ConvTCfg {
   static constexpr int STAGE_BYTES = stage_bytes(YS);
   // one CTA per SM (the accumulators take half the register file): the whole 227 KB of shared memory serves the ring
   static constexpr int STAGES = (218 * 1024) / STAGE_BYTES > 6 ? 6 : (218 * 1024) / STAGE_BYTES;
-  static constexpr int POS = PY * PX;
-  static constexpr int POS_PER_THREAD = (POS + CT_PRODUCERS - 1) / CT_PRODUCERS;
   // epilogue image of the accumulators, [128 rows][MT * NPAD (+ 4 pad) columns] fp32, over the drained ring
   static constexpr int ACC_LD = MT * NPAD + 4;
   static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
@@ -170,11 +165,11 @@ struct ConvTCfg {
 //     input gradient: 3 x 1280) that bias grows past 1e-4 of the result.  OP 3 hands each stage's MMA partial sums to a
 //     second register set with round-to-nearest fp32 adds and restarts the MMA accumulator from 0; the two sets take the
 //     register budget of twice the columns (launch_convt_impl narrows the tile as for X2).
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP, bool TMA>
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1) {
   constexpr bool F16 = OP == 1 || OP == 2, X2 = OP == 2, FLUSH = OP == 3;
-  using Cfg = ConvTCfg<T, NPAD, MT, X2, TMA>;
+  using Cfg = ConvTCfg<T, NPAD, MT, X2>;
   constexpr int NACC = Cfg::NACC;
   static_assert(!FLUSH || 2 * MT * NACC <= CT_ACC_COLS, "two-level accumulators exceed the register budget");
   constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4;
@@ -221,139 +216,49 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     return zi >= 0 && zi < p.D;
   };
   const int n_qq = TZ * nchunk;
-  // Cluster of NCL CTAs along blockIdx.x (same parity class, hence the same weight sequence): every CTA fetches 1/NCL of each
-  // stage's weights and multicasts it to all of them, so the L2 serves the weights once per cluster instead of once per CTA.
-  // The CTAs then walk the SAME stage sequence in lockstep: a stage whose z-tap plane lies outside this CTA's volume is not
-  // skipped but walked without halo and without MMAs; a slot is free when every CTA's MMAs have released it.
-  const uint32_t ncl = cluster_nctarank(), crank = ncl > 1 ? cluster_ctarank() : 0;
-  const uint16_t cmask = (uint16_t)((1u << ncl) - 1);
 
   if (tid == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full[s], TMA ? 1 : CT_PRODUCERS + 1);  // cp.async path: 128 producer arrivals + the expect_tx arrival of the
-                                                        // weight copy; TMA path: the one expect_tx arrival (halo + weight bytes)
-      mbar_init(&empty[s], ncl * CT_CONSUMER_WARPS);   // every consumer warp of every CTA of the cluster
+      mbar_init(&full[s], 1);                    // the producer's expect_tx arrival (halo + weight bytes)
+      mbar_init(&empty[s], CT_CONSUMER_WARPS);   // every consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (ncl > 1) cluster_sync_all();   // every CTA's barriers exist before a peer's multicast can signal them
-  // weights of one stage: this CTA's slice, to every CTA of the cluster
-  auto load_weights = [&](uint8_t *dst, const float *wsrc, uint32_t bytes, uint64_t *bar) {
-    if (ncl == 1) {
-      bulk_g2s(dst, wsrc, bytes, bar);
-    } else {
-      const uint32_t slice = bytes / ncl;
-      bulk_g2s_multicast(dst + crank * slice, reinterpret_cast<const uint8_t *>(wsrc) + crank * slice, slice, bar, cmask);
-    }
-  };
 
   if (warp < 4) {
-    if constexpr (TMA) {
-      // ===================== producer: ONE thread issues the tensor copies of every stage ==========================
-      if (tid == 0) {
-        int it = 0;
-        for (int qq = 0; qq < n_qq; ++qq) {
-          int tz, kc, bz, by, bx;
-          const bool valid = stage_of(qq, tz, kc, bz, by, bx);
-          if (!valid && ncl == 1) continue;
+    // ===================== producer: ONE thread issues the tensor copies (halo) and the bulk copy (weights) of every stage ====
+    if (tid == 0) {
+      int it = 0;
+      for (int qq = 0; qq < n_qq; ++qq) {
+        int tz, kc, bz, by, bx;
+        if (!stage_of(qq, tz, kc, bz, by, bx)) continue;
 #pragma unroll
-          for (int ys = 0; ys < Cfg::YS; ++ys) {
-            const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-            ++it;
-            if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
-            uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
-            const uint32_t wbytes = (uint32_t)(Cfg::rows_of(ys) * T * Cfg::B_TAP_BYTES);
-            const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
-                                (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
-            mbar_arrive_expect_tx(&full[s], wbytes + (valid ? (uint32_t)Cfg::A_TX_BYTES : 0u));
-            load_weights(sa + Cfg::A_BYTES, wsrc, wbytes, &full[s]);
-            if (!valid) continue;
-            const int zi = zj + bz - tz;
-            const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);
-#pragma unroll
-            for (int part = 0; part < Cfg::PARTS; ++part) {
-#pragma unroll
-              for (int c = 0; c < CT_KCG; ++c) {
-                int cg = kc * CT_KCG + c;
-                const CUtensorMap *tm = &tmap0;
-                if (cg >= p.cg0) { cg -= p.cg0; tm = &tmap1; }
-                tma_load_5d(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE, tm, gx0, gy0, cg, (b * p.D + zi) * Cfg::PARTS + part, &full[s]);
-              }
-            }
-          }
-        }
-      }
-    } else {
-    // ===================== producers: halo (cp.async, zero-fill) + weights (one bulk copy per stage) ==========
-    // this thread's halo positions are the same for every stage: precompute (offset in the cg plane, halo row/col)
-    int hoff[Cfg::POS_PER_THREAD], hy[Cfg::POS_PER_THREAD], hx[Cfg::POS_PER_THREAD];
-#pragma unroll
-    for (int i = 0; i < Cfg::POS_PER_THREAD; ++i) {
-      const int idx = tid + i * CT_PRODUCERS;
-      hy[i] = idx / Cfg::PX;
-      hx[i] = idx - hy[i] * Cfg::PX;
-      hoff[i] = idx < Cfg::POS ? idx * 16 : -1;
-    }
-    // cp.async groups in flight before a stage is published: the slot a publication waits for must not be one the consumers
-    // still hold, so LAG + INFLIGHT < STAGES
-    constexpr int LAG = Cfg::STAGES - 1 - INFLIGHT < 2 ? Cfg::STAGES - 1 - INFLIGHT : 2;
-    int it = 0;                                        // stages issued so far
-    auto publish = [&]() {  // after committing group `it`: group it - LAG has landed -> hand it to the async proxy
-      cp_async_commit();
-      if (it >= LAG) {
-        cp_async_wait<LAG>();
-        fence_proxy_async_smem();
-        mbar_arrive(&full[(it - LAG) % Cfg::STAGES]);
-      }
-      ++it;
-    };
-    for (int qq = 0; qq < n_qq; ++qq) {
-      int tz, kc, bz, by, bx;
-      const bool valid = stage_of(qq, tz, kc, bz, by, bx);
-      if (!valid && ncl == 1) continue;
-#pragma unroll
-      for (int ys = 0; ys < Cfg::YS; ++ys) {
-        const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
-        if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
-        uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
-        if (tid == 0) {
+        for (int ys = 0; ys < Cfg::YS; ++ys) {
+          const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
+          ++it;
+          if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
+          uint8_t *sa = stages + (size_t)s * Cfg::STAGE_BYTES;
           // weights of tap rows [ys*ROWS, ...) of this (class, z tap, K chunk): a contiguous slice of its T*T-tap block
-          const uint32_t bytes = (uint32_t)(Cfg::rows_of(ys) * T * Cfg::B_TAP_BYTES);
+          const uint32_t wbytes = (uint32_t)(Cfg::rows_of(ys) * T * Cfg::B_TAP_BYTES);
           const float *wsrc = p.wpack + ((((size_t)par * TZ + tz) * nchunk + kc) * (size_t)(T * T * Cfg::B_TAP_BYTES / 4)) +
                               (size_t)ys * Cfg::ROWS * T * (Cfg::B_TAP_BYTES / 4);
-          mbar_arrive_expect_tx(&full[s], bytes);
-          load_weights(sa + Cfg::A_BYTES, wsrc, bytes, &full[s]);
-        }
-        const int zi = zj + bz - tz;
-        const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);  // halo row hy holds input row gy0 + hy
-        if (valid) {
+          mbar_arrive_expect_tx(&full[s], wbytes + (uint32_t)Cfg::A_TX_BYTES);
+          bulk_g2s(sa + Cfg::A_BYTES, wsrc, wbytes, &full[s]);
+          const int zi = zj + bz - tz;
+          const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);  // halo row r holds input row gy0 + r
 #pragma unroll
-        for (int part = 0; part < Cfg::PARTS; ++part) {
+          for (int part = 0; part < Cfg::PARTS; ++part) {
 #pragma unroll
-          for (int c = 0; c < CT_KCG; ++c) {
-            int cg = kc * CT_KCG + c;
-            const float *src = p.src0;
-            int ncg = p.cg0;
-            if (cg >= p.cg0) { cg -= p.cg0; src = p.src1; ncg = p.cg1; }
-            // X2: [B*D][part][cg][H][W][16 B]
-            const float *plane = src + (((((size_t)b * p.D + zi) * Cfg::PARTS + part) * ncg + cg) * p.H) * (size_t)p.W * 4;
-#pragma unroll
-            for (int i = 0; i < Cfg::POS_PER_THREAD; ++i) {
-              if (hoff[i] < 0) continue;
-              const int gy = gy0 + hy[i], gx = gx0 + hx[i];
-              const bool ok = (gy >= 0) & (gy < p.H) & (gx >= 0) & (gx < p.W);
-              const float *g = ok ? plane + ((size_t)gy * p.W + gx) * 4 : plane;
-              cp_async16_zfill(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE + hoff[i], g, ok);
+            for (int c = 0; c < CT_KCG; ++c) {
+              int cg = kc * CT_KCG + c;
+              const CUtensorMap *tm = &tmap0;
+              if (cg >= p.cg0) { cg -= p.cg0; tm = &tmap1; }
+              tma_load_5d(sa + (part * CT_KCG + c) * Cfg::A_CG_STRIDE, tm, gx0, gy0, cg, (b * p.D + zi) * Cfg::PARTS + part, &full[s]);
             }
           }
         }
-        }
-        publish();
       }
-    }
-    for (int e = 0; e < LAG; ++e) publish();  // drain: empty groups push the last real ones through
-
     }
   } else {
     // ===================== consumers: warpgroup wg issues the wgmma of rows [64 wg, 64 wg + 64) of every M-tile ===========
@@ -370,38 +275,21 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
         for (int j = 0; j < NACC / 2; ++j) tot[mt][j] = 0.0f;
     }
-    // frees a slot (in every CTA of the cluster): this warp's wgmma that read it are done
+    // frees a slot: this warp's wgmma that read it are done
     auto release = [&](int slot) {
       __syncwarp();
-      if (lane == 0) {
-        if (ncl == 1) mbar_arrive(&empty[slot]);
-        else
-          for (uint32_t c = 0; c < ncl; ++c) mbar_arrive_cluster(&empty[slot], c);
-      }
+      if (lane == 0) mbar_arrive(&empty[slot]);
     };
     int it = 0;
     int held = -1;   // the slot of the last committed stage, whose MMAs may still be running
     for (int qq = 0; qq < n_qq; ++qq) {
       int tz, kc, bz, by, bx;
-      const bool valid = stage_of(qq, tz, kc, bz, by, bx);
-      if (!valid && ncl == 1) continue;
+      if (!stage_of(qq, tz, kc, bz, by, bx)) continue;
 #pragma unroll
       for (int ys = 0; ys < Cfg::YS; ++ys) {
         const int s = it % Cfg::STAGES, use = it / Cfg::STAGES;
         ++it;
         mbar_wait(&full[s], use & 1);
-        if (!valid) {   // walked in lockstep with the cluster: the weights pass through, no MMAs
-          // the held slot belongs to the last stage WITH MMAs, which may lie several stages back: the producers need it
-          // (from every CTA of the cluster) before they can publish the stage STAGES later, possibly the next one this CTA
-          // waits for, so it is not kept across stages walked without MMAs
-          if (held >= 0) {
-            wgmma_wait<0>();
-            release(held);
-            held = -1;
-          }
-          release(s);
-          continue;
-        }
         wgmma_fence();
         const uint32_t sa = smem_u32(stages + (size_t)s * Cfg::STAGE_BYTES);
         const uint32_t sb = sa + Cfg::A_BYTES;
@@ -611,7 +499,6 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     }
     }
   }
-  if (ncl > 1) cluster_sync_all();   // no CTA leaves while a peer may still signal its barriers
 }
 
 
@@ -644,31 +531,11 @@ static bool make_halo_tmap(CUtensorMap *m, const void *base, long long planes, i
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<void *>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// halo producer: tensor copies (default) or the cp.async path (GENRE_B200_CONV_TMA=0, or genre_b200_conv_set_tma(0))
-static int g_conv_tma = -1;
-static bool conv_use_tma() {
-  if (g_conv_tma < 0) {
-    const char *e = getenv("GENRE_B200_CONV_TMA");
-    g_conv_tma = (e && e[0] == '0') ? 0 : 1;
-  }
-  return g_conv_tma == 1 && tmap_encoder() != nullptr;
-}
 
-// CTAs per cluster sharing each stage's weights by multicast (GENRE_B200_CONV_CLUSTER, or genre_b200_conv_set_cluster): 1 = off
-static int g_conv_cluster = -1;
-static int conv_cluster() {
-  if (g_conv_cluster < 0) {
-    const char *e = getenv("GENRE_B200_CONV_CLUSTER");
-    const int v = e ? atoi(e) : 1;
-    g_conv_cluster = (v == 2 || v == 4 || v == 8) ? v : 1;
-  }
-  return g_conv_cluster;
-}
-
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP, bool TMA>
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
 static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
-  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2, TMA>;
-  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP, TMA>;
+  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2>;
+  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP>;
   static bool configured[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -683,35 +550,18 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
   ConvTParams q = p;
   q.xtiles = p.W / Cfg::W;
   if (q.xtiles < 1 || q.xtiles * Cfg::W != p.W) return fail_arg(GENRE_B200_EINVAL, "convt3d: W=%d is not a multiple of the %d-wide tile", p.W, Cfg::W);
+  if (!tmap_encoder())
+    return fail_arg(GENRE_B200_EINVAL, "convt3d: the driver entry point cuTensorMapEncodeTiled could not be resolved (the halo "
+                                       "loads are tensor copies)");
   CUtensorMap tm0, tm1;
   memset(&tm0, 0, sizeof(tm0));
   memset(&tm1, 0, sizeof(tm1));
-  if (TMA) {
-    const long long planes = (long long)p.B * p.D * Cfg::PARTS;
-    if (!make_halo_tmap(&tm0, p.src0, planes, p.cg0, p.H, p.W, Cfg::PX, Cfg::PY))
-      return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the first operand");
-    if (p.cg1 > 0 && !make_halo_tmap(&tm1, p.src1, planes, p.cg1, p.H, p.W, Cfg::PX, Cfg::PY))
-      return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the second operand");
-  }
+  const long long planes = (long long)p.B * p.D * Cfg::PARTS;
+  if (!make_halo_tmap(&tm0, p.src0, planes, p.cg0, p.H, p.W, Cfg::PX, Cfg::PY))
+    return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the first operand");
+  if (p.cg1 > 0 && !make_halo_tmap(&tm1, p.src1, planes, p.cg1, p.H, p.W, Cfg::PX, Cfg::PY))
+    return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the second operand");
   dim3 grid((unsigned)(p.B * p.D * (p.H / CT_BY) * q.xtiles), MODE == 0 ? 8 : MODE == 2 ? 2 : 1);
-  int cl = conv_cluster();
-  while (cl > 1 && (grid.x % cl != 0 || (T * Cfg::B_TAP_BYTES) % (16 * cl) != 0)) cl /= 2;
-  if (cl > 1) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(CT_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cudaLaunchKernelEx(&cfg, kern, q, tm0, tm1) != cudaSuccess) return check_launch("convt3d_s2 cluster launch");
-    return check_launch("convt3d_s2 kernel");
-  }
   kern<<<grid, CT_THREADS, Cfg::SMEM, st>>>(q, tm0, tm1);
   return check_launch("convt3d_s2 kernel");
 }
@@ -722,8 +572,7 @@ static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
   if constexpr (MT > 1 && MT * (OP >= 2 ? 2 : 1) * NPAD > CT_ACC_COLS) {
     return launch_convt_impl<TZ, T, NPAD, MT / 2, MODE, OP>(p, st);
   } else {
-    if (conv_use_tma()) return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, true>(p, st);
-    return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, false>(p, st);
+    return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP>(p, st);
   }
 }
 
@@ -796,22 +645,6 @@ static int launch_conv_merged8(const ConvTParams &p, cudaStream_t st) {
 }  // namespace gb
 
 using namespace gb;
-
-// Select the halo producer of the convolution kernels: 1 = cp.async.bulk.tensor (TMA, default), 0 = 16-byte cp.async by 128
-// threads.  Returns the previous setting.  Process-wide; meant for A/B timing and for testing both producers in one process.
-extern "C" int genre_b200_conv_set_tma(int enable) {
-  const int prev = conv_use_tma() ? 1 : 0;
-  g_conv_tma = enable ? 1 : 0;
-  return prev;
-}
-
-// CTAs per thread-block cluster of the convolution kernels (1, 2, 4 or 8): the CTAs of a cluster share every stage's weights
-// through multicast bulk copies.  Returns the previous setting.  Process-wide; for A/B timing and tests.
-extern "C" int genre_b200_conv_set_cluster(int ctas) {
-  const int prev = conv_cluster();
-  g_conv_cluster = (ctas == 2 || ctas == 4 || ctas == 8) ? ctas : 1;
-  return prev;
-}
 
 // ConvTranspose3d(kernel K in {4, 8}, stride 2, padding K/2 - 1) forward on channel-blocked activations.
 //   src0 [B*D][cg0][H][W][4], src1 [B*D][cg1][H][W][4] or NULL: the two halves of the channel concatenation

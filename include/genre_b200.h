@@ -410,17 +410,6 @@ int genre_b200_sph_bp_forward_fused(const float *sph, int64_t N, int64_t C, int6
 int genre_b200_scale_clamp_strided(const float *src, int64_t maps, int64_t n, float scale, float lo, float hi,
                                    float *dst, int64_t dst_map_stride, void *stream);
 
-/* Halo producer of the convolution kernels: 1 = cp.async.bulk.tensor over a 5-D tiled tensor map (default), 0 = cp.async by 128
- * threads (round 1).  Returns the previous setting; process-wide (A/B timing, tests).  Env: GENRE_B200_CONV_TMA. */
-int genre_b200_conv_set_tma(int enable);
-
-/* CTAs per thread-block cluster of the convolution kernels of csrc/convt3d.cu (1 = no clusters, 2, 4 or 8): the CTAs of a cluster
- * walk the same weight sequence, each fetches 1/n of every stage's weights and multicasts it to all of them (cp.async.bulk
- * .multicast::cluster), and a pipeline slot is released once every consumer warp of every CTA of the cluster has arrived on
- * it (remote mbarrier.arrive).  Default: GENRE_B200_CONV_CLUSTER or 1.
- * Returns the previous setting.  Process-wide. */
-int genre_b200_conv_set_cluster(int ctas);
-
 /* blocked fp32 [BD][cg4][H][W][4] -> blocked fp16 [BD][(cg4+1)/2][H][W][8], channel padding zero-filled: turns the
  * fp32 output of one tensor-core layer into the fp16 operand of the next without going through NCDHW */
 int genre_b200_blocked_f32_to_f16(const float *src, int cg4, int64_t BD, int64_t H, int64_t W, void *dst, void *stream);

@@ -575,54 +575,3 @@ def test_direct_hi_lo_conversions_equal_convert_then_split():
     x4 = torch.randn(2, 2, 8, 4, 12, device=DEV)
     assert torch.equal(ops_conv.space_to_depth4_blocked(x4, 16, torch.float16),
                        ops_conv._split2(ops_conv.space_to_depth4_blocked(x4, 4, None)))
-
-
-def test_both_halo_producers_give_identical_results():
-    """the TMA producer (cp.async.bulk.tensor, zero-filled out-of-range box elements) and the cp.async producer feed the same MMAs:
-    bit-identical outputs, in one process (genre_b200_conv_set_tma)"""
-    from genre_shapehd_b200 import _lib
-    lib = _lib.load()
-    torch.manual_seed(8)
-    m = nets.ConvTranspose3d(80, 20, 8, 2, 3).to(DEV)
-    blk = nets.Conv3d(64, 128, 4, 2, 1).to(DEV)
-    x = torch.randn(2, 80, 3, 32, 32, device=DEV)
-    xc = torch.randn(1, 64, 4, 32, 32, device=DEV)
-    prev = lib.genre_b200_conv_set_tma(1)
-    try:
-        with torch.no_grad():
-            a, ac = ops_conv.conv_transpose3d(x, m), ops_conv.conv3d(xc, blk)
-            lib.genre_b200_conv_set_tma(0)
-            b, bc = ops_conv.conv_transpose3d(x, m), ops_conv.conv3d(xc, blk)
-    finally:
-        lib.genre_b200_conv_set_tma(prev)
-    assert a is not None and ac is not None
-    assert torch.equal(a, b) and torch.equal(ac, bc)
-
-
-@pytest.mark.parametrize("ctas", [2, 4, 8])
-def test_weight_multicast_clusters_give_identical_results(ctas):
-    """clusters of 2 / 4 / 8 CTAs sharing every stage's weights by multicast (stages outside a CTA's volume walked without MMAs)
-    against the single-CTA launch: bit-identical, for a transposed conv whose z taps leave the volume, a strided conv in
-    sub-volume form, the merged-parity k8 layer and the 4x space-to-depth k8 conv; both halo producers"""
-    from genre_shapehd_b200 import _lib
-    lib = _lib.load()
-    torch.manual_seed(9)
-    layers = [(nets.ConvTranspose3d(80, 20, 8, 2, 3).to(DEV), torch.randn(2, 80, 4, 32, 32, device=DEV), ops_conv.conv_transpose3d),
-              (nets.ConvTranspose3d(64, 32, 4, 2, 1).to(DEV), torch.randn(1, 64, 3, 32, 32, device=DEV), ops_conv.conv_transpose3d),
-              (nets.Conv3d(64, 128, 4, 2, 1).to(DEV), torch.randn(1, 64, 4, 32, 64, device=DEV), ops_conv.conv3d),
-              (nets.Conv3d(2, 20, 8, 2, 3).to(DEV), torch.rand(1, 2, 8, 64, 64, device=DEV), ops_conv.conv3d)]
-    prev_tma = lib.genre_b200_conv_set_tma(1)
-    prev = lib.genre_b200_conv_set_cluster(1)
-    try:
-        with torch.no_grad():
-            for tma in (1, 0):
-                lib.genre_b200_conv_set_tma(tma)
-                lib.genre_b200_conv_set_cluster(1)
-                ref = [f(x, m) for m, x, f in layers]
-                lib.genre_b200_conv_set_cluster(ctas)
-                got = [f(x, m) for m, x, f in layers]
-                for r, g in zip(ref, got):
-                    assert r is not None and torch.equal(r, g)
-    finally:
-        lib.genre_b200_conv_set_cluster(prev)
-        lib.genre_b200_conv_set_tma(prev_tma)

@@ -58,9 +58,11 @@ __device__ __forceinline__ uint4 pack_f16x8(const float (&x)[8]) {
 }
 
 // The activation operand of the fp32-accurate f16x2 convolution mode for 8 channels: hi = fp16(a), lo' = fp16((a - hi) * 2^11),
-// a = hi + lo' * 2^-11 to ~2^-22 |a|.  Every producer of this operand (the layout kernels and the convolution epilogues) calls this
+// a = hi + lo' * 2^-11 to 2^-22 |a| while |a| >= 2^-14 (fp16's smallest normal).  Below that, fp16's subnormal spacing (2^-24)
+// in lo' makes the error an absolute floor instead: |a - hi - lo' * 2^-11| <= 2^-22 |a| + 2^-36 for every finite |a| < 65520.
+// Every producer of this operand (the layout kernels and the convolution epilogues) calls this
 // function: the intrinsics are never contracted into an FMA with the code that computed `a`, so the same fp32 value gives the
-// same bits wherever it is split.  |a| > 65504 becomes inf (and stays visible in the output).
+// same bits wherever it is split.  |a| >= 65520 rounds hi to inf (and stays visible in the output); up to there hi is finite.
 __device__ __forceinline__ void split_hi_lo8(const float (&x)[8], uint4 &hi, uint4 &lo) {
   __half h[8], l[8];
 #pragma unroll

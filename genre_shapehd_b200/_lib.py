@@ -99,6 +99,7 @@ _SIGNATURES = {
                                   _ptr],
     "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
                               _size, _ptr],
+    "genre_b200_mesh_voxelize": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _int, _int, _ptr, _ptr, _size, _ptr],
 }
 
 # every symbol include/genre_b200.h declares (tests check the library exports all of them)
@@ -109,7 +110,7 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_voxel_surface_workspace_bytes", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
     "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
     "genre_b200_surface_sample_workspace_bytes", "genre_b200_crop_to_render_workspace_bytes",
-    "genre_b200_preprocess_workspace_bytes"])
+    "genre_b200_preprocess_workspace_bytes", "genre_b200_mesh_voxelize_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
@@ -137,6 +138,8 @@ _LAUNCHES = {
     "genre_b200_surface_sample": 3, "genre_b200_crop_to_render": 2,
     # min/max (not rgb) + cubic, + gray, mean and jitter for train-mode rgb
     "genre_b200_preprocess": lambda kind, train, *_: 1 + (kind != 0) + (3 if kind == 0 and train else 0),
+    # count, scan and columns only when there are faces, then the expand kernel
+    "genre_b200_mesh_voxelize": lambda verts, V, faces, F, *_: 4 if F > 0 else 1,
 }
 
 
@@ -185,6 +188,8 @@ def load():
     lib.genre_b200_crop_to_render_workspace_bytes.argtypes = [_i64]
     lib.genre_b200_preprocess_workspace_bytes.restype = _size
     lib.genre_b200_preprocess_workspace_bytes.argtypes = [_int, _int, _i64, _int]
+    lib.genre_b200_mesh_voxelize_workspace_bytes.restype = _size
+    lib.genre_b200_mesh_voxelize_workspace_bytes.argtypes = [_i64, _i64, _int, _int, _int]
     _lib = lib
     return lib
 

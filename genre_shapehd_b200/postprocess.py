@@ -16,6 +16,10 @@ pooling) plus the IoU an evaluation computes from them, batched on the device.
 
 ``sample_surface`` / ``chamfer_fscore`` / ``voxel_metrics`` evaluate predicted grids by the Chamfer distance and F-score of
 points drawn from their surfaces (the metric of the reference's nndistance op), batched on the device.
+
+``voxelize_mesh`` / ``mesh_metrics`` / ``read_obj`` / ``pack_meshes`` go the other way, from triangle meshes (ShapeNet and
+Pix3D ship their shapes as meshes) to grids: conservative voxelisation on the device, and the same metrics against
+ground-truth meshes.
 """
 import numpy as np
 import torch
@@ -617,17 +621,161 @@ def voxel_metrics(pred, gt, level=0.5, gt_level=0.5, n_points=1024, tau=0.01, se
     a, g = _volumes(pred, "voxel_metrics"), _volumes(gt, "voxel_metrics")
     if a.shape != g.shape:
         raise ValueError("voxel_metrics: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(g.shape)))
-    b, dims = a.shape[0], a.shape[1:]
+    seeds = _seeds(seed, a.shape[0], a.device)
+    pp, fp = _grid_surface_points(a, level, n_points, seeds)
+    pg, fg = _grid_surface_points(g, gt_level, n_points, seeds)
+    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, g, level, gt_level)[0].double())
+
+
+def _grid_surface_points(v, level, n_points, seeds):
+    """sample_surface of marching_cubes(v, level) with voxel centres in the centred unit cube (voxel_metrics' frame)"""
+    dims = v.shape[1:]
     spacing = [1.0 / s for s in dims]
     shift = [0.5 - 0.5 / s for s in dims]
-    seeds = _seeds(seed, b, a.device)
-    pp, fp = sample_surface(*marching_cubes(a, level, spacing, shift), n_points, seeds)
-    pg, fg = sample_surface(*marching_cubes(g, gt_level, spacing, shift), n_points, seeds)
+    return sample_surface(*marching_cubes(v, level, spacing, shift), n_points, seeds)
+
+
+def _point_metrics(pp, fp, pg, fg, tau, iou):
+    """chamfer_fscore of two point batches, NaN where either surface is empty (face -1), with ``iou`` and ``valid`` added"""
     valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
     keep = valid[:, None, None]
     out = chamfer_fscore(torch.where(keep, pp, torch.zeros_like(pp)), torch.where(keep, pg, torch.zeros_like(pg)), tau)
-    nan = torch.full((b,), float("nan"), dtype=torch.float64, device=a.device)
+    nan = torch.full((pp.shape[0],), float("nan"), dtype=torch.float64, device=pp.device)
     out = {k: torch.where(valid, v, nan) for k, v in out.items()}
-    out["iou"] = voxel_iou(a, g, level, gt_level)[0].double()
+    out["iou"] = iou
     out["valid"] = valid
     return out
+
+
+# ---- meshes to grids: conservative voxelisation, scoring against ground-truth meshes, .obj input ---------------------------
+def _mesh_args(name, verts, faces, vert_off, face_off):
+    _lib.require_cuda(verts, faces, vert_off, face_off)
+    _lib.require_f32(verts)
+    if faces.dtype != torch.int32 or vert_off.dtype != torch.int64 or face_off.dtype != torch.int64:
+        raise TypeError("%s expects int32 faces and int64 offsets, got %s, %s, %s" % (name, faces.dtype, vert_off.dtype,
+                                                                                      face_off.dtype))
+    b = vert_off.numel() - 1
+    if b < 1 or face_off.numel() != b + 1 or verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("%s: verts [V,3], faces [F,3] and offsets [B+1] expected, got %s, %s, %s, %s"
+                         % (name, tuple(verts.shape), tuple(faces.shape), tuple(vert_off.shape), tuple(face_off.shape)))
+    return b, verts.contiguous(), faces.contiguous(), vert_off.contiguous(), face_off.contiguous()
+
+
+def voxelize_mesh(verts, faces, vert_off, face_off, shape=128):
+    """Conservative voxelisation of every sample's triangle mesh, on the device: [B,1,D,H,W] fp32, 1.0 where a voxel is set.
+
+    verts [V,3] fp32, faces [F,3] int32 (indices into the sample's own vertex block, trusted: ``pack_meshes`` checks them),
+    vert_off / face_off [B+1] int64: the packed meshes ``marching_cubes`` returns.  ``shape`` is an int or (D, H, W), every
+    dimension in [1, 512].
+
+    Frame: voxel (i0, i1, i2) is the closed cube [i_a/n_a - 0.5, (i_a+1)/n_a - 0.5] on each axis, (n_0, n_1, n_2) = (D, H, W),
+    vertex coordinate 0 along the first array axis: the centred unit cube of ``voxel_metrics``, whose ``marching_cubes``
+    frame puts mesh vertices between voxel centres.  Rule: a voxel is set iff the closed triangle and the closed cube
+    intersect (touching counts, so a face on a grid plane sets both layers), by the separating-axis test in fp64 with the
+    order stated in include/genre_b200.h; tests/mesh_voxelize_ref.py restates it bit for bit.  Faces with a non-finite vertex
+    or an exactly zero normal set nothing (the faces ``sample_surface`` never draws); faces outside the grid are clipped.
+
+    The rule is conservative: every path of closed cubes from the inside of a closed mesh to the outside meets a set voxel,
+    so ``voxel_fill(voxelize_mesh(...))`` is the solid of a closed mesh.  An open mesh leaks: its fill is its shell plus
+    whatever it does enclose.  Deterministic, batch-equivariant, and nothing is copied to the host (graph-capturable)."""
+    b, verts, faces, vert_off, face_off = _mesh_args("voxelize_mesh", verts, faces, vert_off, face_off)
+    d, h, w = (int(shape),) * 3 if np.ndim(shape) == 0 else (int(s) for s in shape)
+    nbytes = _lib.load().genre_b200_mesh_voxelize_workspace_bytes(b, faces.shape[0], d, h, w)
+    if nbytes == 0:
+        raise ValueError("voxelize_mesh: %d meshes with %d faces into %dx%dx%d unsupported (1 <= B <= 65535, fewer than 2^31 "
+                         "faces, every dimension in [1, 512])" % (b, faces.shape[0], d, h, w))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=verts.device)
+    out = torch.empty((b, 1, d, h, w), dtype=torch.float32, device=verts.device)
+    _lib.call("genre_b200_mesh_voxelize", verts.data_ptr(), verts.shape[0], faces.data_ptr(), faces.shape[0],
+              vert_off.data_ptr(), face_off.data_ptr(), b, d, h, w, out.data_ptr(), ws.data_ptr(), nbytes,
+              _lib.stream_ptr(verts))
+    return out
+
+
+def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=1024, tau=0.01, seed=0, six_way=True):
+    """``voxel_metrics`` of predicted grids against ground-truth triangle meshes given in the same frame (the centred unit
+    cube, ``voxelize_mesh``'s; aligning and normalising the meshes is the caller's).
+
+    pred [B,1,D,H,W] or [B,D,H,W] fp32 values; the meshes packed as for ``voxelize_mesh``, one per sample.
+      * points on the prediction: ``marching_cubes(pred, level)`` in voxel_metrics' frame, then ``sample_surface``;
+      * points on the ground truth: ``sample_surface`` of the meshes, with the same seeds;
+      * chamfer / F-score, ``valid`` and the NaNs of invalid samples exactly as ``voxel_metrics``;
+      * iou = voxel_iou(pred, voxel_fill(voxelize_mesh(meshes, (D, H, W)), six_way), level, 0.5).
+    Given the ground truth as ``marching_cubes(gt)`` in voxel_metrics' frame, every metric but ``iou`` equals voxel_metrics'
+    bit for bit.  The marching-cubes call synchronises once; nothing else does."""
+    a = _volumes(pred, "mesh_metrics")
+    b = a.shape[0]
+    nb, verts, faces, vert_off, face_off = _mesh_args("mesh_metrics", verts, faces, vert_off, face_off)
+    if nb != b:
+        raise ValueError("mesh_metrics: %d predictions and %d meshes" % (b, nb))
+    seeds = _seeds(seed, b, a.device)
+    pp, fp = _grid_surface_points(a, level, n_points, seeds)
+    pg, fg = sample_surface(verts, faces, vert_off, face_off, n_points, seeds)
+    solid = voxel_fill(voxelize_mesh(verts, faces, vert_off, face_off, tuple(a.shape[1:])), six_way)
+    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, solid[:, 0].float(), level, 0.5)[0].double())
+
+
+def read_obj(path):
+    """A Wavefront .obj file -> (verts [V,3] float32, faces [F,3] int32, 0-based) as numpy arrays.
+
+    ``v`` lines give vertices (components past the third are ignored); ``f`` lines give polygons in the ``i``, ``i/j``,
+    ``i//k`` and ``i/j/k`` forms, 1-based, a negative index counting back from the vertices read so far; a polygon is
+    fan-triangulated as (v0, v_k, v_k+1).  Every other line is ignored.  An index out of range, or a face of fewer than 3
+    vertices, raises ValueError.  ``write_obj``'s files read back exactly."""
+    verts, faces, positive = [], [], []
+    with open(path) as fh:
+        for lineno, line in enumerate(fh, 1):
+            parts = line.split()
+            if not parts:
+                continue
+            if parts[0] == "v":
+                if len(parts) < 4:
+                    raise ValueError("%s:%d: a vertex needs 3 coordinates" % (path, lineno))
+                verts.append(parts[1:4])
+            elif parts[0] == "f":
+                idx = []
+                for tok in parts[1:]:
+                    i = int(tok.split("/")[0])
+                    if i < 0:
+                        i += len(verts)
+                        if i < 0:
+                            raise ValueError("%s:%d: vertex index %s before the first vertex" % (path, lineno, tok))
+                    elif i == 0:
+                        raise ValueError("%s:%d: vertex index 0 (indices are 1-based)" % (path, lineno))
+                    else:
+                        i -= 1
+                        positive.append((i, lineno))
+                    idx.append(i)
+                if len(idx) < 3:
+                    raise ValueError("%s:%d: a face needs at least 3 vertices" % (path, lineno))
+                faces.extend((idx[0], idx[k], idx[k + 1]) for k in range(1, len(idx) - 1))
+    for i, lineno in positive:   # forward references are legal: checked against the whole vertex list
+        if i >= len(verts):
+            raise ValueError("%s:%d: vertex index %d of %d vertices" % (path, lineno, i + 1, len(verts)))
+    v = np.array(verts, dtype=np.float64).astype(np.float32).reshape(-1, 3)
+    return v, np.array(faces, dtype=np.int32).reshape(-1, 3)
+
+
+def pack_meshes(meshes, device):
+    """[(verts [V_b,3], faces [F_b,3]), ...] (numpy arrays or tensors) -> (verts, faces, vert_off, face_off) on ``device``,
+    the packed format of ``marching_cubes``.  Every face index is checked on the host to lie in [0, V_b), because the
+    kernels trust them: ValueError otherwise."""
+    vs, fs = [], []
+    for b, (v, f) in enumerate(meshes):
+        v = np.asarray(v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v, dtype=np.float32).reshape(-1, 3)
+        f = np.asarray(f.detach().cpu().numpy() if isinstance(f, torch.Tensor) else f)
+        if f.size and not np.issubdtype(f.dtype, np.integer):
+            raise ValueError("pack_meshes: mesh %d has %s face indices, integers expected" % (b, f.dtype))
+        f = f.astype(np.int64).reshape(-1, 3)
+        if f.size and (f.min() < 0 or f.max() >= len(v)):
+            raise ValueError("pack_meshes: mesh %d has a face index outside [0, %d)" % (b, len(v)))
+        vs.append(v)
+        fs.append(f.astype(np.int32))
+    if not vs:
+        raise ValueError("pack_meshes: no meshes")
+    vo = np.cumsum([0] + [len(v) for v in vs]).astype(np.int64)
+    fo = np.cumsum([0] + [len(f) for f in fs]).astype(np.int64)
+    if fo[-1] >= 1 << 31:
+        raise ValueError("pack_meshes: %d faces, fewer than 2^31 expected" % fo[-1])
+    return (torch.from_numpy(np.concatenate(vs)).to(device), torch.from_numpy(np.concatenate(fs)).to(device),
+            torch.from_numpy(vo).to(device), torch.from_numpy(fo).to(device))

@@ -591,6 +591,37 @@ int genre_b200_surface_sample(const float *verts, int64_t V, const int32_t *face
                               int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Conservative voxelisation of batched triangle meshes, the inverse of genre_b200_isosurface_*: ground-truth meshes become
+ * grids for voxel_iou / voxel_fill and training targets without a CPU tool.
+ *   meshes  the packed format of genre_b200_isosurface_*: verts [V, 3] fp32, faces [F, 3] int32 indexing the sample's own
+ *           vertex block (trusted: in [0, V_n)), vert_off / face_off [N+1] int64 on the device.  F (the total) < 2^31,
+ *           1 <= N <= 65535, every dimension of the D x H x W grid in [1, 512].
+ *   frame   voxel (i0, i1, i2) is the closed cube [i_a/n_a - 0.5, (i_a+1)/n_a - 0.5] per axis, (n0, n1, n2) = (D, H, W), axis 0
+ *           = vertex coordinate 0 = the first array axis (as genre_b200_isosurface_*).  Grid units, fp64 from the fp32 vertex:
+ *           g_a = fl(fl(p_a + 0.5) * n_a); the voxel is then the box [i_a, i_a + 1].
+ *   rule    a voxel is set iff the closed triangle and the closed cube intersect (touching counts: a face on a grid plane sets
+ *           both layers, which makes voxel_fill sound on the result of a closed mesh).  Separating-axis test in grid units,
+ *           fp64, one rounding per operation, no contraction, separation only by a strict inequality:
+ *             box axes  i_a in [max(ceil(min_k g_ka) - 1, 0), min(floor(max_k g_ka), n_a - 1)];
+ *             v_ka = g_ka - (i_a + 0.5); f0 = g1 - g0, f1 = g2 - g1, f2 = g0 - g2, e = g2 - g0;
+ *             normal    m = (f0_1*e_2 - f0_2*e_1, f0_2*e_0 - f0_0*e_2, f0_0*e_1 - f0_1*e_0);
+ *                       separated iff |(m0*v00 + m1*v01) + m2*v02| > 0.5 * ((|m0| + |m1|) + |m2|);
+ *             edges     for each f_j and box axis a, the two non-zero components (A on s, B on t, s < t) of e_a x f_j:
+ *                       a = 0: (-f_j2, f_j1) on (1, 2); a = 1: (f_j2, -f_j0) on (0, 2); a = 2: (-f_j1, f_j0) on (0, 1);
+ *                       p_k = A*v_ks + B*v_kt, separated iff min_k p_k > 0.5*(|A| + |B|) or max_k p_k < -0.5*(|A| + |B|).
+ *           A face with a non-finite vertex coordinate, or whose fp64 normal (b - a) x (c - a) from the fp32 vertices (the
+ *           order of genre_b200_surface_sample's weight) is exactly 0, sets nothing.  Faces outside the grid are clipped.
+ *   output  out [N, D, H, W] fp32, 1.0 for a set voxel and 0.0 elsewhere, written once and dense.  Deterministic and
+ *           batch-equivariant; nothing is copied to the host (graph-capturable).  tests/mesh_voxelize_ref.py restates the
+ *           contract in numpy, bit for bit.
+ *   workspace: genre_b200_mesh_voxelize_workspace_bytes(N, F, D, H, W) bytes (0: unsupported), 16-byte aligned, caller-owned.
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_mesh_voxelize_workspace_bytes(int64_t N, int64_t F, int D, int H, int W);
+int genre_b200_mesh_voxelize(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                             const int64_t *face_off, int64_t N, int D, int H, int W, float *out, void *workspace,
+                             size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Input preprocessing: the test-time silhouette crop (util_img.get_bbox + util_img.crop of every preprocess_wrapper) and
  * MarrnetBaseModel.preprocess (models/marrnetbase.py:71-126), batched.  fp64 in the reference's operation order, one
  * rounding per operation, no FMA (fp32 only where stated); outputs rounded once to fp32, as convert_to_float32 does.

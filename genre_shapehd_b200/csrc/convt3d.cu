@@ -26,6 +26,7 @@
 // empty barrier once its wgmma that read the slot have completed.  With 3 or more stages a stage's MMAs stay in flight while
 // the next stage is awaited and issued (wgmma.wait_group 1): its slot is released after the next stage's MMAs are committed.
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (the entry point is resolved through the runtime: no -lcuda)
+#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -105,10 +106,14 @@ __device__ __forceinline__ void store_operand(const ConvTParams &p, int k, int b
 // The halo of a channel group arrives as ONE cp.async.bulk.tensor (5-D tiled tensor map over [plane][cg][H][W][16 B], box
 // [1][1][PY][PX][16 B], out-of-bounds elements zero-filled = the convolution's padding); each channel group starts on a
 // 128-byte boundary of shared memory (the LBO of the A descriptor is that padded stride).
-template <int T, int NPAD, int MT, bool X2 = false>
+// PW > 0: the paired form of MODE 5 over an input PW wide.  Its halo is flattened: rows of pitch PX = PW + 2 (input x from
+// -2, the two columns past the right edge of a row are the zero columns of the next), PY rows = enough for MT * 128
+// consecutive positions starting anywhere in a row plus the 3 rows and 3 columns the taps reach (see the kernel).
+template <int T, int NPAD, int MT, bool X2 = false, int PW = 0>
 struct ConvTCfg {
   static constexpr int W = 8 * MT;
-  static constexpr int PY = CT_BY + T - 1, PX = W + T - 1;     // halo extent
+  static constexpr int PY = PW ? (128 * MT + (T + 1) * (PW + 2) + 1) / (PW + 2) : CT_BY + T - 1;   // halo extent
+  static constexpr int PX = PW ? PW + 2 : W + T - 1;
   static constexpr int PARTS = X2 ? 2 : 1;
   static constexpr int NACC = PARTS * NPAD;                    // accumulator columns per M-tile = width of the B operand
   static constexpr int A_CG_BYTES = PY * PX * 16;              // one channel group of the halo
@@ -118,8 +123,11 @@ struct ConvTCfg {
   static constexpr int B_TAP_BYTES = 2 * (NACC / 8) * 128;     // one (y,x) tap: [2 kcore][NACC/8][8 rows][16 B]
   // A stage holds the halo of one (z tap, K chunk) and the weights of ROWS of its T tap rows; YS = T / ROWS (rounded up)
   // stages walk the same halo when all T*T taps do not fit twice into shared memory (X2 with 5x5 union taps: 128 KB).
-  // dec5 keeps 2 stages of 3 + 2 tap rows: 3 stages of 2 + 2 + 1 rows would let its MMAs stay in flight across stages (the
-  // kernel's INFLIGHT), but load each halo three times, and measured 5.40 ms per call against 4.97 (H100 80GB HBM3, 700 W).
+  // dec5's union form (MODE 2, X2) keeps 2 stages of 3 + 2 tap rows: 3 stages of 2 + 2 + 1 rows would let its MMAs stay in
+  // flight across stages (the kernel's INFLIGHT), but load each halo three times, and measured 5.40 ms per call against 4.97
+  // (H100 80GB HBM3, 700 W).  Its paired form (MODE 5, X2: 16 taps, 97 KB per stage) takes all 4 tap rows in one stage,
+  // a 2-stage ring that loads each halo once: 3.75 ms per call, against 4.25 ms for 2 + 2 rows in a 3-stage ring with MMAs
+  // in flight and every halo loaded twice (H100 80GB HBM3, 700 W, SM clock 1.92-1.98 GHz, B = 16).
   static constexpr int stage_bytes(int ys) { return ((A_BYTES + ((T + ys - 1) / ys) * T * B_TAP_BYTES + 127) / 128) * 128; }
   static constexpr int pick_ys() {
     for (int ys = 1; ys < T; ++ys)
@@ -142,6 +150,7 @@ struct ConvTCfg {
   static_assert(MT * NACC <= CT_ACC_COLS, "accumulators exceed the register budget");
   static_assert(SMEM <= 227 * 1024, "shared memory");
   static_assert(NACC <= 256 && NACC % 16 == 0 && NPAD % 16 == 0 || !X2, "X2: MMA N must be a multiple of 16, at most 256");
+  static_assert(PW == 0 || (T == 4 && PY <= 256 && PX <= 256), "paired form: 4 taps per dimension, tensor-copy box <= 256");
 };
 
 // MODE 0: 8 parity classes (blockIdx.y), output at 2*j + parity (ConvTranspose3d stride 2); TZ = T = K/2 taps
@@ -159,20 +168,34 @@ struct ConvTCfg {
 // MODE 4: ConvTranspose3d(k 4, s 2, p 1) to ONE output channel (the last layer of every decoder): MODE 3's geometry with
 //         N = 16 columns of which 8 are the output classes; the epilogue adds the bias (shift[0]), optionally applies
 //         the sigmoid, and writes the NCDHW fp32 volume directly.
+// MODE 5: MODE 2 with PAIRED classes (ConvTranspose3d k 8, s 2, p 3; the fp16 operand modes).  Output 2j (y parity 0 of
+//         coarse j) and output 2j - 1 (parity 1 of coarse j - 1) read the same four inputs j + 1 - t, t < 4, with their own
+//         tap t each, so coarse position j computes the pair (2j - 1, 2j) per dimension: 4 x 4 (y,x) taps, N = 4 * Cout, no
+//         zero columns (MODE 2 walks the 5 x 5 union, 9 of its 25 taps zero for some class).  Coarse j then runs over
+//         [0, H] x [0, W], which the 16 x 8 tiles cannot cover, so M is flattened per plane: position q = y * PX + x over a
+//         halo of pitch PX = W + 2 starting at input x = -2.  Tap (ty, tx) is the same shared-memory array shifted by
+//         ((3 - ty) * PX + 3 - tx) * 16 bytes; reads past a row's right edge land on the next row's two leading columns,
+//         which are input x = -2, -1: zeros, the padding they need.  The A operand's 8-row core groups are 8 consecutive
+//         positions (SBO = 128 B).  CTA = one (b, z parity, z plane, run of MT * 128 positions of the (H+1) x PX plane); the
+//         epilogue drops x = W + 1 (the pitch's spare column), y > H and outputs -1 and 2H / 2W.  Per output the MMAs that
+//         carry non-zero weights come in MODE 2's order (z tap, K chunk, y tap, x tap), and MODE 2's others add exact
+//         zeros, so the two modes give bit-identical results.
 // OP: operand type: 0 = TF32 (fp32 storage), 1 = fp16, 2 = fp16 hi/lo split (X2, see ConvTCfg), 3 = TF32 operands of the
 //     3xTF32 split (lo | hi | hi along K) with a two-level accumulator: the tensor core's fp32 accumulator truncates, so a
 //     step's error scales with the partial sum it joins, and over the thousands of K steps of a k=8 layer (Unet_3D.dec5's
 //     input gradient: 3 x 1280) that bias grows past 1e-4 of the result.  OP 3 hands each stage's MMA partial sums to a
 //     second register set with round-to-nearest fp32 adds and restarts the MMA accumulator from 0; the two sets take the
 //     register budget of twice the columns (launch_convt_impl narrows the tile as for X2).
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
+// PW: the input width of MODE 5 (its halo pitch is compile-time), 0 otherwise.
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1) {
   constexpr bool F16 = OP == 1 || OP == 2, X2 = OP == 2, FLUSH = OP == 3;
-  using Cfg = ConvTCfg<T, NPAD, MT, X2>;
+  using Cfg = ConvTCfg<T, NPAD, MT, X2, PW>;
   constexpr int NACC = Cfg::NACC;
   static_assert(!FLUSH || 2 * MT * NACC <= CT_ACC_COLS, "two-level accumulators exceed the register budget");
-  constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4;
+  constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4, PAIR = MODE == 5;
+  static_assert(PAIR == (PW > 0), "MODE 5 and only MODE 5 takes an input width");
   // a stage's MMAs stay in flight while the next stage is issued (its slot is released one stage late) only with a ring of 3
   // or more, where the producer still has a slot to fill meanwhile; OP 3 reads its accumulators after every stage
   constexpr int INFLIGHT = Cfg::STAGES >= 3 && !FLUSH ? 1 : 0;
@@ -184,14 +207,17 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int par = blockIdx.y;  // parity class: bit 2 = z, bit 1 = y, bit 0 = x
-  const int pz = MERGE ? par : (par >> 2) & 1, py = (par >> 1) & 1, px = par & 1;
-  const int ytiles = p.H / CT_BY;
-  const int xt = blockIdx.x % p.xtiles;
+  const int pz = MERGE || PAIR ? par : (par >> 2) & 1, py = (par >> 1) & 1, px = par & 1;
+  const int ytiles = PAIR ? 1 : p.H / CT_BY;
+  const int xt = blockIdx.x % p.xtiles;   // MODE 5: the run of positions within the plane
   const int tile = blockIdx.x / p.xtiles;
   const int yt = tile % ytiles;
   const int zj = (tile / ytiles) % p.D;
   const int b = tile / (ytiles * p.D);
   const int y0 = yt * CT_BY, x0 = xt * Cfg::W;
+  // MODE 5: the CTA's first position q0, the plane row yq0 it lies in and its offset in that row; halo row r holds input row
+  // yq0 - 2 + r, so position q under tap (ty, tx) reads halo element q - yq0 * PX + (3 - ty) * PX + 3 - tx
+  const int q0 = xt * 128 * MT, yq0 = q0 / Cfg::PX, qoff = q0 - yq0 * Cfg::PX;
   const int nchunk = (p.cg0 + p.cg1) / CT_KCG;
 
   // (z tap, K chunk) enumeration shared by the producer and the MMA issuer: qq = tz * nchunk + kc, skipped when the z tap
@@ -246,7 +272,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
           mbar_arrive_expect_tx(&full[s], wbytes + (uint32_t)Cfg::A_TX_BYTES);
           bulk_g2s(sa + Cfg::A_BYTES, wsrc, wbytes, &full[s]);
           const int zi = zj + bz - tz;
-          const int gy0 = y0 + by - (T - 1), gx0 = x0 + bx - (T - 1);  // halo row r holds input row gy0 + r
+          const int gy0 = PAIR ? yq0 - 2 : y0 + by - (T - 1), gx0 = PAIR ? -2 : x0 + bx - (T - 1);  // halo row r = input row gy0 + r
 #pragma unroll
           for (int part = 0; part < Cfg::PARTS; ++part) {
 #pragma unroll
@@ -303,14 +329,17 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
             for (int mt = 0; mt < MT; ++mt) {
               // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x; this warpgroup's
-              // 64 rows are y = 8 wg .. 8 wg + 7
-              const uint32_t a0 = sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
-              const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+              // 64 rows are y = 8 wg .. 8 wg + 7.  MODE 5: positions q0 + 128 mt + 64 wg + [0, 64), consecutive in the
+              // flattened halo, so an 8-row core group is 8 consecutive 16-byte positions
+              constexpr uint32_t SBO = PAIR ? 128 : Cfg::PX * 16;
+              const uint32_t a0 = PAIR ? sa + (qoff + 128 * mt + 64 * wg + (T - 1 - ty) * Cfg::PX + (T - 1 - tx)) * 16
+                                       : sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
+              const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, SBO);
               if constexpr (X2) {
                 // A_hi x W_hi into the hi accumulator, then the cross terms A_hi x W_lo' and A_lo' x W_hi, in that order,
                 // into the cross accumulator: three N = NPAD MMAs on disjoint registers (an MMA that writes into part of
                 // another's accumulator registers makes ptxas serialize every wgmma)
-                const uint64_t adesc_lo = gmma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, Cfg::PX * 16);
+                const uint64_t adesc_lo = gmma_desc(a0 + CT_KCG * Cfg::A_CG_STRIDE, Cfg::A_CG_STRIDE, SBO);
                 wgmma_f16<NPAD>(acc[mt], adesc, bdesc);
                 wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc, gmma_desc(btap + (NPAD / 8) * 128, (NACC / 8) * 128, 128));
                 wgmma_f16<NPAD>(acc[mt] + NPAD / 2, adesc_lo, bdesc);
@@ -360,7 +389,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     const int m = warp * 32 + lane;  // accumulator row
     const float *arow = acc_img + (size_t)m * Cfg::ACC_LD;
     const int yy = m >> 3, xx = m & 7;
-    constexpr bool UP = PAR || MERGE || MERGE8 || C1;
+    constexpr bool UP = PAR || MERGE || MERGE8 || C1 || PAIR;
     const int Ho = UP ? 2 * p.H : p.H, Wo = UP ? 2 * p.W : p.W, Do = UP ? 2 * p.D : p.D;
     const int oz_plain = UP ? 2 * zj + pz : zj, oy = PAR ? 2 * (y0 + yy) + py : y0 + yy;
     auto act = [&](float a, int n) {
@@ -390,6 +419,54 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
         for (int qzy = 0; qzy < 4; ++qzy) {
           float *dst = p.out + (((size_t)b * Do + 2 * zj + (qzy >> 1)) * Ho + 2 * (y0 + yy) + (qzy & 1)) * (size_t)Wo + oxb;
           *reinterpret_cast<float2 *>(dst) = make_float2(v[qzy * 2], v[qzy * 2 + 1]);
+        }
+      }
+    } else if constexpr (PAIR) {
+      constexpr int CP = NPAD / 4;            // output channels per (y,x) class
+      static_assert(CP % 4 == 0, "merged classes must be whole channel groups");
+      const int oz = 2 * zj + pz;
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+        const int q = q0 + 128 * mt + m, y = q / Cfg::PX, x = q - y * Cfg::PX;
+        if (y > p.H || x > p.W) continue;     // past the plane, or the pitch's spare column x = W + 1
+#pragma unroll
+        for (int qy = 0; qy < 2; ++qy) {
+          const int oyy = 2 * y - qy;         // class y parity 1 is output 2y - 1, parity 0 is 2y
+          if (oyy < 0 || oyy >= Ho) continue;
+#pragma unroll
+          for (int qx = 0; qx < 2; ++qx) {
+            const int ox = 2 * x - qx;
+            if (ox < 0 || ox >= Wo) continue;
+            const float *cls = arow + mt * NPAD + (qy * 2 + qx) * CP;   // the CP channels of class (qy, qx)
+            if (to_operands) {
+#pragma unroll
+              for (int k = 0; k < (CP + 7) / 8; ++k) {
+                float v[8];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int c0 = 8 * k + 4 * h;
+                  float v4[4] = {0.f, 0.f, 0.f, 0.f};
+                  if (c0 < CP) ld_row<4>(cls + c0, v4);
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) v[4 * h + e] = c0 < CP && c0 + e < 4 * p.cgo ? act(v4[e], c0 + e) : 0.0f;
+                }
+                store_operand(p, k, b, oz, oyy, ox, Do, Ho, Wo, v);
+              }
+              store_zero_groups((CP + 7) / 8, oz, oyy, ox);
+              continue;
+            }
+#pragma unroll
+            for (int cgo = 0; cgo < CP / 4; ++cgo) {
+              if (cgo >= p.cgo) continue;  // uniform across the CTA
+              float v4[4];
+              ld_row<4>(cls + cgo * 4, v4);
+              float4 o;
+              float *po = &o.x;
+#pragma unroll
+              for (int e = 0; e < 4; ++e) po[e] = act(v4[e], cgo * 4 + e);
+              *reinterpret_cast<float4 *>(p.out + (((((size_t)b * Do + oz) * p.cgo + cgo) * Ho + oyy) * (size_t)Wo + ox) * 4) = o;
+            }
+          }
         }
       }
     } else if constexpr (MERGE || MERGE8) {
@@ -532,10 +609,10 @@ static bool make_halo_tmap(CUtensorMap *m, const void *base, long long planes, i
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0>
 static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
-  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2>;
-  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP>;
+  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2, PW>;
+  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP, PW>;
   static bool configured[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -548,8 +625,13 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
     configured[dev & 63] = true;
   }
   ConvTParams q = p;
-  q.xtiles = p.W / Cfg::W;
-  if (q.xtiles < 1 || q.xtiles * Cfg::W != p.W) return fail_arg(GENRE_B200_EINVAL, "convt3d: W=%d is not a multiple of the %d-wide tile", p.W, Cfg::W);
+  if constexpr (PW > 0) {
+    if (p.W != PW) return fail_arg(GENRE_B200_EINVAL, "convt3d: the paired kernel for W=%d got W=%d", PW, p.W);
+    q.xtiles = ((p.H + 1) * Cfg::PX + 128 * MT - 1) / (128 * MT);   // runs of MT * 128 positions per (H+1) x PX plane
+  } else {
+    q.xtiles = p.W / Cfg::W;
+    if (q.xtiles < 1 || q.xtiles * Cfg::W != p.W) return fail_arg(GENRE_B200_EINVAL, "convt3d: W=%d is not a multiple of the %d-wide tile", p.W, Cfg::W);
+  }
   if (!tmap_encoder())
     return fail_arg(GENRE_B200_EINVAL, "convt3d: the driver entry point cuTensorMapEncodeTiled could not be resolved (the halo "
                                        "loads are tensor copies)");
@@ -561,18 +643,18 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
     return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the first operand");
   if (p.cg1 > 0 && !make_halo_tmap(&tm1, p.src1, planes, p.cg1, p.H, p.W, Cfg::PX, Cfg::PY))
     return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the second operand");
-  dim3 grid((unsigned)(p.B * p.D * (p.H / CT_BY) * q.xtiles), MODE == 0 ? 8 : MODE == 2 ? 2 : 1);
+  dim3 grid((unsigned)(p.B * p.D * (PW ? 1 : p.H / CT_BY) * q.xtiles), MODE == 0 ? 8 : MODE == 2 || MODE == 5 ? 2 : 1);
   kern<<<grid, CT_THREADS, Cfg::SMEM, st>>>(q, tm0, tm1);
   return check_launch("convt3d_s2 kernel");
 }
 
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP>
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0>
 static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
   // narrower x tiles (more CTAs, each with fewer M-tiles) until the accumulators fit the consumers' registers
   if constexpr (MT > 1 && MT * (OP >= 2 ? 2 : 1) * NPAD > CT_ACC_COLS) {
-    return launch_convt_impl<TZ, T, NPAD, MT / 2, MODE, OP>(p, st);
+    return launch_convt_impl<TZ, T, NPAD, MT / 2, MODE, OP, PW>(p, st);
   } else {
-    return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP>(p, st);
+    return launch_convt_variant<TZ, T, NPAD, MT, MODE, OP, PW>(p, st);
   }
 }
 
@@ -605,6 +687,12 @@ static int launch_convt(const ConvTParams &p, cudaStream_t st) {
 template <int TZ, int T, int NPAD, int MT>
 static int launch_convt_merged(const ConvTParams &p, cudaStream_t st) {
   return launch_convt_op<TZ, T, NPAD, MT, 2>(p, st);
+}
+// MODE 5, the fp16 operand modes: three M-tiles per CTA in fp16 (240 accumulator columns), one in the hi/lo split (X2
+// narrows it), N = 80
+template <int PW>
+static int launch_convt_paired(const ConvTParams &p, cudaStream_t st) {
+  return g_conv_op == 2 ? launch_convt_impl<4, 4, 80, 3, 5, 2, PW>(p, st) : launch_convt_impl<4, 4, 80, 3, 5, 1, PW>(p, st);
 }
 // the operand destinations of the *_operands entry points
 struct OperandOut {
@@ -715,8 +803,11 @@ extern "C" int genre_b200_convt3d_s2_forward_operands(const void *src0, int cg0,
 // ConvTranspose3d(kernel 8, stride 2, padding 3) with the four (y,x) output parity classes merged along N (kernel MODE 2):
 // the layer that dominates Unet_3D, dec5 = ConvT(80 -> 20) on 32^3 (networks/networks.py:166).  Same operands as
 // genre_b200_convt3d_s2_forward except
-//   wpack [2 z-parity][4 z-tap][Cin chunk][5*5 union taps][2][npad/8][8][g], npad = 4 * cpad columns ordered
-//         n = (py*2+px)*cpad + co  (ops_conv.pack_convt_merged_weights);  scale, shift [cpad].
+//   wpack, npad = 4 * cpad columns ordered n = (py*2+px)*cpad + co;  scale, shift [cpad]:
+//     fp16 operands (f16 = 1, 2) and W in {16, 32}, GENRE_B200_CONVT_UNION unset or "0": paired classes (kernel MODE 5)
+//         [2 z-parity][4 z-tap][Cin chunk][4*4 taps][2][npad/8][8][8]  (ops_conv.pack_convt_paired_weights)
+//     otherwise: the 5 x 5 union of the classes' taps (kernel MODE 2)
+//         [2 z-parity][4 z-tap][Cin chunk][5*5 union taps][2][npad/8][8][g]  (ops_conv.pack_convt_merged_weights)
 // Supported: ksize 8, npad = 80 (Cout <= 20), W = 16 or a multiple of 32, H % 16 == 0.
 static int convt3d_s2_merged(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D, int64_t H,
                              int64_t W, const void *wpack_, int ksize, int npad, int f16, const float *scale,
@@ -750,6 +841,13 @@ static int convt3d_s2_merged(const void *src0_, int cg0, const void *src1_, int 
     p.base[par] = (par + pad - k0) / 2;
   }
   cudaStream_t st = as_stream(stream);
+  // paired classes (MODE 5) at the widths it is built for, unless GENRE_B200_CONVT_UNION is set (to anything but "0"): the
+  // union form, for comparing the two (ops_conv reads the same variable to pick the packer)
+  const char *union_env = getenv("GENRE_B200_CONVT_UNION");
+  if ((f16 == 1 || f16 == 2) && !(union_env && union_env[0] && strcmp(union_env, "0") != 0)) {
+    if (W == 32) return launch_convt_paired<32>(p, st);
+    if (W == 16) return launch_convt_paired<16>(p, st);
+  }
   if (W % 32 == 0) return launch_convt_merged<4, 5, 80, 4>(p, st);  // 32-wide x tiles
   return launch_convt_merged<4, 5, 80, 2>(p, st);
 }

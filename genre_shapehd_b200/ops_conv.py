@@ -68,8 +68,17 @@ PRECISION = os.environ.get("GENRE_B200_CONV_PRECISION", "exact")
 EXACT_IMPL = os.environ.get("GENRE_B200_CONV_EXACT_IMPL", "f16x2")
 # k=8 ConvTranspose3d with Cout <= 20 (Unet_3D.dec5): merge the four (y,x) parity classes into one N=80 MMA stream
 MERGE_PARITIES = os.environ.get("GENRE_B200_CONV_MERGE", "1") != "0"
+# ... and with fp16 operands at W in {16, 32} the library runs the merged classes PAIRED (4 x 4 taps, csrc/convt3d.cu MODE 5)
+# instead of over their 5 x 5 union of taps (MODE 2).  The library reads this variable on every call, so it is read here on
+# every call too: the packer has to match the form the kernel takes.  "1" keeps the union form (bit-identical, 28 % more MMAs).
+UNION_ENV = "GENRE_B200_CONVT_UNION"
 # Unet_3D.enc1 (4x space-to-depth form): z class on blockIdx.y (N = 80, two CTAs per SM) instead of all 8 classes in N = 160
 S4D_SPLIT_Z = os.environ.get("GENRE_B200_S4D_SPLIT_Z", "0") != "0"   # measured: 0.88 vs 0.80 ms, so off
+
+
+def _paired_classes(group, w):
+    """does genre_b200_convt3d_s2_merged_forward take the paired form (and the paired weight layout)?"""
+    return group == 8 and w in (16, 32) and os.environ.get(UNION_ENV, "0") in ("", "0")
 
 
 # With torch.backends.cudnn.allow_tf32 off the caller asks for fp32 convolutions: the kernels then run the 3xTF32 scheme
@@ -516,6 +525,26 @@ def pack_convt_merged_weights(weight, cpad, group=4):
     return _finish_pack(out, g)
 
 
+def pack_convt_paired_weights(weight, cpad, group=8):
+    """ConvTranspose3d weight [Cin, Cout, K, K, K] (stride 2, padding K/2-1) for the paired-class kernel (MODE 5):
+    [2 z-parity][T z-tap][Cin/(2g) chunk][T*T (y,x) taps][2 k-core][N/8][8][g],  N = 4*cpad, column n = (py*2+px)*cpad + co.
+    Coarse position j holds output 2j - p of class p per dimension; tap t reads input j + 1 - t, which is the class's own
+    tap t (kernel index k0_p + 2t) for both classes, so no column is zero (the union packer's tap u = t + 1 - p)."""
+    cin, cout, k = weight.shape[0], weight.shape[1], weight.shape[2]
+    t, pad, g = k // 2, k // 2 - 1, group
+    n = 4 * cpad
+    k0 = [(p + pad) % 2 for p in (0, 1)]
+    weq = weight.new_zeros((cin, n, 2, t, t, t))                         # (ci, n, pz, tz, ty, tx)
+    for py in (0, 1):
+        for px in (0, 1):
+            c0 = (py * 2 + px) * cpad
+            for pz in (0, 1):
+                weq[:, c0:c0 + cout, pz] = weight[:, :, k0[pz]::2, k0[py]::2, k0[px]::2]
+    sub = weq.reshape(cin // (2 * g), 2, g, n // 8, 8, 2, t, t, t)       # (kc, kk, e, ng, r, pz, tz, ty, tx)
+    out = sub.permute(5, 6, 0, 7, 8, 1, 3, 4, 2).contiguous()           # (pz, tz, kc, ty, tx, kk, ng, r, e)
+    return _finish_pack(out, g)
+
+
 def pack_convt_c1_tc_weights(weight, segments, group=4):
     """ConvTranspose3d weight [Cin, 1, 4, 4, 4] (stride 2, padding 1) for kernel MODE 4: [3 z-tap][chunk][9 taps][2][2][8][g].
     N = 16 columns, n = (qz*2+qy)*2+qx < 8 the output classes; union tap u reads input j + 1 - u and serves class q as its
@@ -642,8 +671,11 @@ def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0, operands=N
     src1_ptr = src1.data_ptr() if src1 is not None else None
     op = _op_flag() if g == 8 or _x3() else 0
     if merged:
-        # the four (y,x) parity classes share one MMA stream: N = 4 x 20 columns (csrc/convt3d.cu MODE 2)
-        wpack = _pack(module, ("convt_merged", 20, g), lambda wt: pack_convt_merged_weights(wt, 20, g), 2)
+        # the four (y,x) parity classes share one MMA stream: N = 4 x 20 columns (csrc/convt3d.cu MODE 5 paired, else MODE 2)
+        if _paired_classes(g, w):
+            wpack = _pack(module, ("convt_paired", 20, g), lambda wt: pack_convt_paired_weights(wt, 20, g), 2)
+        else:
+            wpack = _pack(module, ("convt_merged", 20, g), lambda wt: pack_convt_merged_weights(wt, 20, g), 2)
         head = (src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, op, aff[0].data_ptr(),
                 aff[1].data_ptr(), float(slope))
         if operands:

@@ -295,9 +295,16 @@ int genre_b200_convt_c1_forward(const float *src0, int cg0, const float *src1, i
                                 const float *weight, float bias, int act_sigmoid, float *out, void *stream);
 
 /* ConvTranspose3d(k 8, s 2, p 3), Cout <= 20, with the four (y,x) output parity classes merged along N (one N = 80 MMA
- * over the union of 5x5 taps instead of four N = 20 MMAs over 4x4): Unet_3D.dec5 = ConvT(80 -> 20) (networks/networks.py:166),
- * 53.7 of the refiner's 78 GFLOP.  Operands as genre_b200_convt3d_s2_forward except wpack
- * [2 z-parity][4][Cin chunk][25][2][npad/8][8][g] with npad = 80 columns n = (py*2+px)*20 + co; scale, shift [20]. */
+ * instead of four N = 20 MMAs): Unet_3D.dec5 = ConvT(80 -> 20) (networks/networks.py:166), 53.7 of the refiner's 78 GFLOP.
+ * Operands as genre_b200_convt3d_s2_forward except scale, shift [20] and wpack, npad = 80 columns n = (py*2+px)*20 + co, in
+ * one of two layouts:
+ *   fp16 operands (f16 = 1, 2) and W in {16, 32}: PAIRED classes, 4x4 taps (coarse position j computes outputs 2j - 1 and
+ *     2j per dimension, which read the same inputs): [2 z-parity][4][Cin chunk][16][2][npad/8][8][8]
+ *     (ops_conv.pack_convt_paired_weights);
+ *   otherwise (fp32 operands f16 = 0, 3; other W): the 5x5 UNION of the classes' taps, zero weights where a class does not
+ *     use a tap: [2 z-parity][4][Cin chunk][25][2][npad/8][8][g] (ops_conv.pack_convt_merged_weights).
+ * Setting the environment variable GENRE_B200_CONVT_UNION (to anything but "0") makes every call take the union layout
+ * (the two forms give bit-identical results; the paired one issues 28 % fewer MMAs at 32^2). */
 int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *src1, int cg1,
                                          int64_t B, int64_t D, int64_t H, int64_t W,
                                          const void *wpack, int ksize, int npad, int f16,

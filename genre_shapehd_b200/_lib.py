@@ -85,6 +85,7 @@ _SIGNATURES = {
     "genre_b200_voxelize_stage_splat": [_i64, _i64, _int, _ptr, _ptr, _f32, _f32, _f32, _ptr, _size, _ptr],
     "genre_b200_isosurface_count": [_ptr, _i64, _int, _int, _int, _f32, _ptr, _ptr, _size, _ptr],
     "genre_b200_isosurface_emit": [_ptr, _i64, _int, _int, _int, _f32] + [_f32] * 6 + [_ptr] * 5 + [_size, _ptr],
+    "genre_b200_isosurface_backward": [_ptr, _i64, _int, _int, _int, _f32] + [_f32] * 3 + [_ptr] * 4 + [_size, _ptr],
     "genre_b200_raycast_count": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _ptr, _ptr, _size, _ptr],
     "genre_b200_raycast_build": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_raycast_first_hit": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _ptr, _ptr, _ptr, _ptr, _i64, _i64, _ptr,
@@ -95,6 +96,7 @@ _SIGNATURES = {
     "genre_b200_voxel_downsample": [_ptr, _i64, _int, _int, _int, _ptr, _ptr],
     "genre_b200_voxel_translate": [_ptr, _i64, _int, _int, _int, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_surface_sample": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _size, _ptr],
+    "genre_b200_surface_sample_backward": [_ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _ptr],
     "genre_b200_crop_to_render": [_ptr, _ptr, _int, _ptr, _ptr, _int, _i64, _int, _f64, _f64, _ptr, _ptr, _ptr, _ptr, _size,
                                   _ptr],
     "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
@@ -131,7 +133,9 @@ _LAUNCHES = {
     "genre_b200_convt3d_s2_merged_forward": 1, "genre_b200_conv3d_k8s2_s4d_forward": 1, "genre_b200_ncdhw_to_blocked": 1, "genre_b200_blocked_to_ncdhw": 1,
     "genre_b200_convt3d_s2_forward_operands": 1, "genre_b200_convt3d_s2_merged_forward_operands": 1,
     "genre_b200_conv3d_k8s2_s4d_forward_operands": 1, "genre_b200_conv3d_k4s2_forward_operands": 1,
-    "genre_b200_isosurface_count": 2, "genre_b200_isosurface_emit": 2,
+    "genre_b200_isosurface_count": 2, "genre_b200_isosurface_emit": 2, "genre_b200_isosurface_backward": 1,
+    # the kernel only when there are vertices (after a memset)
+    "genre_b200_surface_sample_backward": lambda faces, F, vo, fo, N, seeds, n, face, gp, V, *_: 1 if V > 0 else 0,
     "genre_b200_raycast_count": 3, "genre_b200_raycast_build": 2, "genre_b200_raycast_first_hit": 1,
     "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
     "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,

@@ -34,6 +34,16 @@
 //   face  : block scan of ntri + tile offset; re-links the cell's nonempty faces and writes the fans.  The vertex of local edge
 //           e is base[owner] + popc(mask[owner] & ((1 << axis) - 1)).
 // The volume is read once by count (neighbour reads hit L1/L2) and again only around crossings by the emit kernels.
+//
+// Backward (genre_b200_isosurface_backward): the gradient of the vertex coordinates with respect to the volume.  Only x_a of
+// the vertex on the edge p -> q = p + e_a depends on the volume, through t; with g = grad_verts[v][a] (the other two
+// components are ignored), in fp64 from the fp32 operands, one rounding per operation, in this order:
+//           d = v1 - v0,  k = (g * s_a) / (d * d),  c0 = k * (level - v1) goes to p,  c1 = k * (v0 - level) goes to q.
+//           An edge with a non-finite end contributes 0.
+//   grad  : a gather, thread per grid point on the count kernel's tiling: the point sums its own crossing edges a = 0, 1, 2
+//           (their c0), then the incoming edges from p - e_a, a = 0, 1, 2 (their c1), in fp64 from 0, rounded once to fp32.
+//           The vertex of edge (owner, a) is vbase[owner] + popc(code[owner] & 7 & ((1 << a) - 1)), read only where the mask
+//           bit is set (vbase is written only there).  No atomics: deterministic.
 #include "common.cuh"
 
 namespace gb {
@@ -314,6 +324,60 @@ iso_face_kernel(const float *__restrict__ vol, int D, int H, int W, float level,
   }
 }
 
+// x is finite (not NaN, not +-inf)
+__device__ __forceinline__ bool iso_finite(float x) { return fabsf(x) <= 3.402823466e38f; }
+
+// the contribution of edge (owner, a) to one of its ends: c0 (to the owner, lo = true) or c1 (to the far end)
+__device__ __forceinline__ double iso_edge_grad(float v0, float v1, float level, float g, float s, bool lo) {
+  if (!iso_finite(v0) || !iso_finite(v1)) return 0.0;
+  const double d = __dsub_rn((double)v1, (double)v0);
+  const double k = __ddiv_rn(__dmul_rn((double)g, (double)s), __dmul_rn(d, d));
+  return lo ? __dmul_rn(k, __dsub_rn((double)level, (double)v1)) : __dmul_rn(k, __dsub_rn((double)v0, (double)level));
+}
+
+// grid (tiles, N): thread per grid point; grad_vol fully written
+__global__ void __launch_bounds__(ISO_THREADS)
+iso_grad_kernel(const float *__restrict__ vol, int D, int H, int W, float level, float3 spacing,
+                const unsigned char *__restrict__ codes, const unsigned *__restrict__ vbase,
+                const long long *__restrict__ vert_off, const float *__restrict__ grad_verts, float *__restrict__ grad_vol) {
+  const int n = blockIdx.y;
+  const long long P = (long long)D * H * W;
+  const int HW = H * W;
+  const long long p = (long long)blockIdx.x * ISO_THREADS + threadIdx.x;
+  if (p >= P) return;
+  const float *v = vol + (size_t)n * P;
+  const unsigned char *cd = codes + (size_t)n * P;
+  const unsigned *vb = vbase + (size_t)n * P;
+  const float *gv = grad_verts + 3 * (size_t)__ldg(vert_off + n);
+  const int k = (int)(p % W), j = (int)((p / W) % H), i = (int)(p / HW);
+  const float vp = __ldg(v + p);
+  double sum = 0.0;
+  const unsigned own = cd[p] & 7u;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const long long stride = a == 0 ? HW : a == 1 ? W : 1;
+    const float s = a == 0 ? spacing.x : a == 1 ? spacing.y : spacing.z;
+    if ((own >> a) & 1u) {
+      const unsigned vid = vb[p] + __popc(own & ((1u << a) - 1u));
+      sum = __dadd_rn(sum, iso_edge_grad(vp, __ldg(v + p + stride), level, __ldg(gv + 3 * (size_t)vid + a), s, true));
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const long long stride = a == 0 ? HW : a == 1 ? W : 1;
+    const float s = a == 0 ? spacing.x : a == 1 ? spacing.y : spacing.z;
+    if ((a == 0 ? i : a == 1 ? j : k) > 0) {
+      const long long o = p - stride;
+      const unsigned m = cd[o] & 7u;
+      if ((m >> a) & 1u) {
+        const unsigned vid = vb[o] + __popc(m & ((1u << a) - 1u));
+        sum = __dadd_rn(sum, iso_edge_grad(__ldg(v + o), vp, level, __ldg(gv + 3 * (size_t)vid + a), s, false));
+      }
+    }
+  }
+  grad_vol[(size_t)n * P + p] = __double2float_rn(sum);
+}
+
 struct IsoLayout {
   long long P;
   int tiles;
@@ -389,4 +453,17 @@ extern "C" int genre_b200_isosurface_emit(const float *vol, int64_t N, int D, in
   iso_face_kernel<<<grid, ISO_THREADS, 0, st>>>(vol, D, H, W, level, codes, tws, L.tiles, vbase, (const long long *)face_off,
                                                 faces);
   return check_launch("isosurface face kernel");
+}
+
+extern "C" int genre_b200_isosurface_backward(const float *vol, int64_t N, int D, int H, int W, float level, float sx, float sy,
+                                              float sz, const int64_t *vert_off, const float *grad_verts, float *grad_vol,
+                                              void *workspace, size_t workspace_bytes, void *stream) {
+  GB_REQUIRE(vert_off && grad_verts && grad_vol, GENRE_B200_EINVAL, "isosurface_backward: null pointer");
+  IsoLayout L;
+  if (int rc = iso_check("isosurface_backward", vol, N, D, H, W, level, workspace, workspace_bytes, &L)) return rc;
+  const char *ws = (const char *)workspace;
+  iso_grad_kernel<<<dim3((unsigned)L.tiles, (unsigned)N), ISO_THREADS, 0, as_stream(stream)>>>(
+      vol, D, H, W, level, make_float3(sx, sy, sz), (const unsigned char *)(ws + L.codes), (const unsigned *)(ws + L.vbase),
+      (const long long *)vert_off, grad_verts, grad_vol);
+  return check_launch("isosurface backward kernel");
 }

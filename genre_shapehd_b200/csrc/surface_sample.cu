@@ -29,6 +29,13 @@
 // Kernels: ss_weight_kernel (thread per face: s, the per-sample maximum), ss_scan_kernel (one CTA per sample: quantise and
 // scan in tiles of SS_SCAN_THREADS x SS_SCAN_ITEMS faces with a running carry), ss_sample_kernel (thread per point: three
 // splitmix64 draws, a binary search in P, the barycentric point).
+//
+// Backward (genre_b200_surface_sample_backward): the gradient of the points with respect to the vertices, with the drawn faces
+// and barycentric draws held fixed (the reparameterised sampling gradient; nothing flows through the area weights).  Point i
+// of sample b redraws (u, v) from (seed_b, i) with the forward's helper and reads its face from the forward's face output;
+// dp/da = 1 - u - v, dp/db = u, dp/dc = v, exact in fp32.  ss_sample_backward_kernel (thread per point) adds each
+// fl32(w * g) to grad_verts by fp32 atomicAdd after a memset: the order of the additions is unspecified, so the result is
+// not bitwise reproducible.  Points with face -1 contribute nothing.
 #include "common.cuh"
 
 namespace gb {
@@ -44,6 +51,20 @@ __device__ __forceinline__ unsigned long long ss_splitmix64(unsigned long long z
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
+}
+
+// the barycentric draw (u, v) of point i of a sample with seed `seed`: r_1, r_2 and the U + V > 2^24 fold
+__device__ __forceinline__ void ss_barycentric(unsigned long long seed, long long i, float &u, float &v) {
+  const unsigned long long k = 3ull * (unsigned long long)i;
+  const unsigned long long r1 = ss_splitmix64(seed + (k + 2ull) * SS_GOLDEN);
+  const unsigned long long r2 = ss_splitmix64(seed + (k + 3ull) * SS_GOLDEN);
+  unsigned U = (unsigned)(r1 >> 40), V = (unsigned)(r2 >> 40);
+  if (U + V > (1u << 24)) {
+    U = (1u << 24) - U;
+    V = (1u << 24) - V;
+  }
+  u = __fmul_rn((float)U, 0x1p-24f);
+  v = __fmul_rn((float)V, 0x1p-24f);
 }
 
 // largest n with off[n] <= i (empty samples are skipped over)
@@ -173,10 +194,8 @@ ss_sample_kernel(const float *__restrict__ verts, const int *__restrict__ faces,
     face[o] = -1;
     return;
   }
-  const unsigned long long seed = __ldg(seeds + b), k = 3ull * (unsigned long long)i;
-  const unsigned long long r0 = ss_splitmix64(seed + (k + 1ull) * SS_GOLDEN);
-  const unsigned long long r1 = ss_splitmix64(seed + (k + 2ull) * SS_GOLDEN);
-  const unsigned long long r2 = ss_splitmix64(seed + (k + 3ull) * SS_GOLDEN);
+  const unsigned long long seed = __ldg(seeds + b);
+  const unsigned long long r0 = ss_splitmix64(seed + (3ull * (unsigned long long)i + 1ull) * SS_GOLDEN);
   const unsigned long long x = __umul64hi(r0, T);
   long long lo = 0, hi = nf - 1;   // P[nf - 1] = T > x: the answer exists
   while (lo < hi) {
@@ -184,12 +203,8 @@ ss_sample_kernel(const float *__restrict__ verts, const int *__restrict__ faces,
     if (p[mid] > x) hi = mid;
     else lo = mid + 1;
   }
-  unsigned U = (unsigned)(r1 >> 40), V = (unsigned)(r2 >> 40);
-  if (U + V > (1u << 24)) {
-    U = (1u << 24) - U;
-    V = (1u << 24) - V;
-  }
-  const float u = __fmul_rn((float)U, 0x1p-24f), v = __fmul_rn((float)V, 0x1p-24f);
+  float u, v;
+  ss_barycentric(seed, i, u, v);
   const int *fp = faces + 3 * (fb + lo);
   const float *vb = verts + 3 * __ldg(vert_off + b);
   const float *A = vb + 3 * __ldg(fp), *B = vb + 3 * __ldg(fp + 1), *C = vb + 3 * __ldg(fp + 2);
@@ -199,6 +214,31 @@ ss_sample_kernel(const float *__restrict__ verts, const int *__restrict__ faces,
     points[3 * o + a] = __fadd_rn(__fadd_rn(va, __fmul_rn(u, __fsub_rn(__ldg(B + a), va))), __fmul_rn(v, __fsub_rn(__ldg(C + a), va)));
   }
   face[o] = (int)lo;
+}
+
+// grid (point blocks, N): thread per (point, sample); grad_verts zeroed beforehand
+__global__ void __launch_bounds__(SS_THREADS)
+ss_sample_backward_kernel(const int *__restrict__ faces, const long long *__restrict__ vert_off,
+                          const long long *__restrict__ face_off, const unsigned long long *__restrict__ seeds, long long n,
+                          const int *__restrict__ face, const float *__restrict__ grad_points, float *__restrict__ grad_verts) {
+  const int b = blockIdx.y;
+  const long long i = (long long)blockIdx.x * SS_THREADS + threadIdx.x;
+  if (i >= n) return;
+  const size_t o = (size_t)b * n + i;
+  const int f = __ldg(face + o);
+  if (f < 0) return;
+  float u, v;
+  ss_barycentric(__ldg(seeds + b), i, u, v);
+  const float w[3] = {__fsub_rn(__fsub_rn(1.0f, u), v), u, v};   // exact: u, v are multiples of 2^-24 with u + v <= 1
+  const int *fp = faces + 3 * (__ldg(face_off + b) + f);
+  float *gv = grad_verts + 3 * __ldg(vert_off + b);
+  const float g[3] = {__ldg(grad_points + 3 * o), __ldg(grad_points + 3 * o + 1), __ldg(grad_points + 3 * o + 2)};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float *dst = gv + 3 * (size_t)__ldg(fp + c);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) atomicAdd(dst + a, __fmul_rn(w[c], g[a]));
+  }
 }
 
 struct SsLayout {
@@ -258,4 +298,28 @@ extern "C" int genre_b200_surface_sample(const float *verts, int64_t V, const in
   ss_sample_kernel<<<dim3(ss_blocks(n, SS_THREADS), (unsigned)N), SS_THREADS, 0, st>>>(
       verts, faces, vo, fo, (const unsigned long long *)seeds, P, n, points, face);
   return check_launch("surface_sample kernel");
+}
+
+extern "C" int genre_b200_surface_sample_backward(const int32_t *faces, int64_t F, const int64_t *vert_off,
+                                                  const int64_t *face_off, int64_t N, const uint64_t *seeds, int64_t n,
+                                                  const int32_t *face, const float *grad_points, int64_t V, float *grad_verts,
+                                                  void *stream) {
+  GB_REQUIRE(vert_off && face_off && seeds && face && grad_points && (faces || F == 0) && (grad_verts || V == 0),
+             GENRE_B200_EINVAL, "surface_sample_backward: null pointer");
+  GB_REQUIRE(N >= 1 && N <= 65535, GENRE_B200_EINVAL, "surface_sample_backward: N=%lld out of range [1, 65535]", (long long)N);
+  GB_REQUIRE(V >= 0 && V <= ((int64_t)1 << 40) && F >= 0 && F < SS_MAX_FACES, GENRE_B200_EINVAL,
+             "surface_sample_backward: V=%lld, F=%lld out of range (F < 2^31)", (long long)V, (long long)F);
+  GB_REQUIRE(n >= 1 && n <= SS_MAX_POINTS, GENRE_B200_EINVAL, "surface_sample_backward: n=%lld out of range [1, 2^30]",
+             (long long)n);
+  if (V == 0) return 0;   // no vertex: no face was drawn either
+  cudaStream_t st = as_stream(stream);
+  const cudaError_t e = cudaMemsetAsync(grad_verts, 0, (size_t)V * 3 * sizeof(float), st);
+  if (e != cudaSuccess) {
+    set_error("surface_sample_backward: memset: %s", cudaGetErrorString(e));
+    return (int)e;
+  }
+  ss_sample_backward_kernel<<<dim3(ss_blocks(n, SS_THREADS), (unsigned)N), SS_THREADS, 0, st>>>(
+      faces, (const long long *)vert_off, (const long long *)face_off, (const unsigned long long *)seeds, n, face, grad_points,
+      grad_verts);
+  return check_launch("surface_sample backward kernel");
 }

@@ -73,8 +73,20 @@ def marching_cubes(volume, level, spacing=(1.0, 1.0, 1.0), shift=(0.0, 0.0, 0.0)
     crack-free but is not Lewiner's, so the faces differ from skimage's.
 
     The output size depends on the data: the per-sample counts are copied to the host once (a device synchronisation)
-    before the output is allocated, so the call cannot be captured in a CUDA graph."""
+    before the output is allocated, so the call cannot be captured in a CUDA graph.
+
+    Differentiable in ``volume``: when grad is enabled and ``volume.requires_grad``, ``verts`` carries a grad_fn whose
+    backward (``genre_b200_isosurface_backward``, deterministic) gives the volume the gradient of x_a = (p_a + t) s_a - shift_a
+    through t = (level - v0) / (v1 - v0); faces and offsets are not differentiable.  Only then is the volume saved and the
+    workspace (about 5 B per grid point) kept until the graph is freed.  The outputs are the same either way."""
     v = _volumes(volume, "marching_cubes")
+    if torch.is_grad_enabled() and v.requires_grad:
+        return _MarchingCubes.apply(v, float(level), spacing, shift)
+    return _marching_cubes(v, float(level), spacing, shift)[:4]
+
+
+def _marching_cubes(v, level, spacing, shift):
+    """marching_cubes of the [B,D,H,W] volumes v -> (verts, faces, vert_off, face_off, workspace)"""
     n, d, h, w = v.shape
     lib = _lib.load()
     nbytes = lib.genre_b200_isosurface_workspace_bytes(n, d, h, w)
@@ -83,7 +95,6 @@ def marching_cubes(volume, level, spacing=(1.0, 1.0, 1.0), shift=(0.0, 0.0, 0.0)
                          % (n, d, h, w))
     dev = v.device
     stream = _lib.stream_ptr(v)
-    level = float(level)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     counts = torch.empty((n, 2), dtype=torch.int64, device=dev)
     _lib.call("genre_b200_isosurface_count", v.data_ptr(), n, d, h, w, level, counts.data_ptr(), ws.data_ptr(), nbytes, stream)
@@ -97,7 +108,31 @@ def marching_cubes(volume, level, spacing=(1.0, 1.0, 1.0), shift=(0.0, 0.0, 0.0)
         sh = [float(x) for x in shift]
         _lib.call("genre_b200_isosurface_emit", v.data_ptr(), n, d, h, w, level, *sp, *sh, offsets[0].data_ptr(),
                   offsets[1].data_ptr(), verts.data_ptr(), faces.data_ptr(), ws.data_ptr(), nbytes, stream)
-    return verts, faces, offsets[0], offsets[1]
+    return verts, faces, offsets[0], offsets[1], ws
+
+
+class _MarchingCubes(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, v, level, spacing, shift):
+        verts, faces, vo, fo, ws = _marching_cubes(v, level, spacing, shift)
+        ctx.save_for_backward(v, vo)
+        ctx.ws, ctx.level, ctx.spacing = ws, level, [float(x) for x in spacing]
+        ctx.mark_non_differentiable(faces, vo, fo)
+        return verts, faces, vo, fo
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_verts, *_):
+        v, vo = ctx.saved_tensors
+        n, d, h, w = v.shape
+        if grad_verts.shape[0] == 0:   # no vertex: nothing depends on the volume
+            return torch.zeros_like(v), None, None, None
+        g = grad_verts.contiguous()
+        _lib.require_f32(g)
+        grad = torch.empty_like(v)
+        _lib.call("genre_b200_isosurface_backward", v.data_ptr(), n, d, h, w, ctx.level, *ctx.spacing, vo.data_ptr(),
+                  g.data_ptr(), grad.data_ptr(), ctx.ws.data_ptr(), ctx.ws.numel(), _lib.stream_ptr(v))
+        return grad, None, None, None
 
 
 # Visualizer._to_obj_str prints every coordinate with "{}".format(x).  For a float32 x, numpy 1.x formats str(x) (the
@@ -541,7 +576,13 @@ def sample_surface(verts, faces, vert_off, face_off, n, seed=0):
 
     Every step is in integers or in fp64 / fp32 with one stated rounding per operation (include/genre_b200.h), so the result
     is deterministic, does not depend on the rest of the batch, and equals the numpy restatement in
-    tests/surface_sample_ref.py bit for bit.  Nothing is copied to the host."""
+    tests/surface_sample_ref.py bit for bit.  Nothing is copied to the host.
+
+    Differentiable in ``verts``: when grad is enabled and ``verts.requires_grad``, ``points`` carries a grad_fn whose backward
+    (``genre_b200_surface_sample_backward``) gives each vertex of a point's face its barycentric weight times the point's
+    gradient, with the drawn faces and barycentric coordinates held fixed (no gradient through the area weights).  The
+    backward redraws the coordinates from the seeds and accumulates by fp32 atomics, so its result is not bitwise
+    reproducible.  The outputs are the same either way."""
     _lib.require_cuda(verts, faces, vert_off, face_off)
     _lib.require_f32(verts)
     if faces.dtype != torch.int32 or vert_off.dtype != torch.int64 or face_off.dtype != torch.int64:
@@ -561,6 +602,14 @@ def sample_surface(verts, faces, vert_off, face_off, n, seed=0):
     dev = verts.device
     verts, faces, vert_off, face_off = verts.contiguous(), faces.contiguous(), vert_off.contiguous(), face_off.contiguous()
     seeds = _seeds(seed, b, dev)
+    if torch.is_grad_enabled() and verts.requires_grad:
+        return _SampleSurface.apply(verts, faces, vert_off, face_off, seeds, n, nbytes)
+    return _sample_surface(verts, faces, vert_off, face_off, seeds, n, nbytes)
+
+
+def _sample_surface(verts, faces, vert_off, face_off, seeds, n, nbytes):
+    b = vert_off.numel() - 1
+    dev = verts.device
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     points = torch.empty((b, n, 3), dtype=torch.float32, device=dev)
     face = torch.empty((b, n), dtype=torch.int32, device=dev)
@@ -568,6 +617,29 @@ def sample_surface(verts, faces, vert_off, face_off, n, seed=0):
               vert_off.data_ptr(), face_off.data_ptr(), b, seeds.data_ptr(), n, points.data_ptr(), face.data_ptr(),
               ws.data_ptr(), nbytes, _lib.stream_ptr(verts))
     return points, face
+
+
+class _SampleSurface(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, verts, faces, vert_off, face_off, seeds, n, nbytes):
+        points, face = _sample_surface(verts, faces, vert_off, face_off, seeds, n, nbytes)
+        ctx.save_for_backward(faces, vert_off, face_off, seeds, face)
+        ctx.nv = verts.shape[0]
+        ctx.mark_non_differentiable(face)
+        return points, face
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_points, _):
+        faces, vert_off, face_off, seeds, face = ctx.saved_tensors
+        g = grad_points.contiguous()
+        _lib.require_f32(g)
+        b, n = face.shape
+        grad = torch.empty((ctx.nv, 3), dtype=torch.float32, device=g.device)
+        _lib.call("genre_b200_surface_sample_backward", faces.data_ptr(), faces.shape[0], vert_off.data_ptr(),
+                  face_off.data_ptr(), b, seeds.data_ptr(), n, face.data_ptr(), g.data_ptr(), ctx.nv, grad.data_ptr(),
+                  _lib.stream_ptr(g))
+        return grad, None, None, None, None, None, None
 
 
 def chamfer_fscore(p, q, tau=0.01):
@@ -645,6 +717,51 @@ def _point_metrics(pp, fp, pg, fg, tau, iou):
     out["iou"] = iou
     out["valid"] = valid
     return out
+
+
+def chamfer_loss(pred, gt, level=0.5, n_points=1024, seed=0, eps=1e-10):
+    """Differentiable Chamfer loss of predicted grids against ground-truth grids or points, for training.
+
+    pred [B,1,D,H,W] or [B,D,H,W] fp32 values, not logits (pass ``torch.sigmoid(logits)``).  Its points are exactly those of
+    ``voxel_metrics``: ``marching_cubes(pred, level)`` with voxel centres in the centred unit cube, then ``sample_surface``
+    with ``n_points`` per sample and ``seed`` as there.  ``gt`` is either a grid of pred's shape, meshed and sampled the same
+    way at level 0.5 with the same seeds, or points [B,M,3] in that frame (e.g. ``sample_surface`` of ``pack_meshes`` output,
+    the frame of ``mesh_metrics``).
+      loss_b = mean_i sqrt(d1_i + eps) + mean_j sqrt(d2_j + eps)
+    with d1, d2 the squared nearest-neighbour distances of ``nndistance`` (the reference's ``nndistance_score``, i.e. about
+    2 x ``voxel_metrics``' chamfer).  Returns (loss [B] fp32, valid [B] bool).  Where either side has no surface (face -1 on
+    pred or a grid gt, or NaN ground-truth points) valid is False, the loss is 0 and no gradient flows from that sample; NaN
+    points never reach the nearest-neighbour kernel.
+
+    The gradient reaches pred through the sampled points (faces and barycentric draws fixed) and the marching-cubes vertices:
+    it only moves the surface the prediction already has.  It cannot create surface where none exists, so the term belongs
+    next to the BCE losses, not instead of them.  On an
+    edge whose two values both lie close to ``level`` the gradient grows like 1 / (v1 - v0)^2; no clipping is built in.
+    Marching cubes on pred synchronises once; a grid gt adds its own."""
+    from .toolbox.nndistance.functions.nnd import NNDFunction
+    a = _volumes(pred, "chamfer_loss")
+    b = a.shape[0]
+    seeds = _seeds(seed, b, a.device)
+    pp, fp = _grid_surface_points(a, level, n_points, seeds)
+    if gt.dim() == 3:
+        _lib.require_cuda(gt)
+        _lib.require_f32(gt)
+        if gt.shape[0] != b or gt.shape[2] != 3:
+            raise ValueError("chamfer_loss: gt points [%d,M,3] expected, got %s" % (b, tuple(gt.shape)))
+        pg = gt
+        valid = (fp[:, 0] >= 0) & ~torch.isnan(gt).any(2).any(1)
+    else:
+        g = _volumes(gt, "chamfer_loss")
+        if g.shape != a.shape:
+            raise ValueError("chamfer_loss: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(g.shape)))
+        pg, fg = _grid_surface_points(g, 0.5, n_points, seeds)
+        valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
+    keep = valid[:, None, None]
+    p1 = torch.where(keep, pp, torch.zeros_like(pp))
+    p2 = torch.where(keep, pg, torch.zeros_like(pg))
+    d1, d2, _, _ = NNDFunction.apply(p1, p2)
+    loss = torch.sqrt(d1 + eps).mean(1) + torch.sqrt(d2 + eps).mean(1)
+    return torch.where(valid, loss, torch.zeros_like(loss)), valid
 
 
 # ---- meshes to grids: conservative voxelisation, scoring against ground-truth meshes, .obj input ---------------------------

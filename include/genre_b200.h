@@ -475,6 +475,18 @@ int genre_b200_isosurface_count(const float *vol, int64_t N, int D, int H, int W
 int genre_b200_isosurface_emit(const float *vol, int64_t N, int D, int H, int W, float level, float sx, float sy, float sz,
                                float shx, float shy, float shz, const int64_t *vert_off, const int64_t *face_off, float *verts,
                                int32_t *faces, void *workspace, size_t workspace_bytes, void *stream);
+/* backward: grad_vol [N, D, H, W] fp32 (fully written, no memset needed) = the gradient of the emitted vertex coordinates with
+ * respect to vol, given grad_verts [sum V, 3] fp32.  Same vol, N, D, H, W, level and workspace as the count and emit calls,
+ * the workspace untouched since emit; the spacing and vert_off of the emit call.  Only x_a of the vertex on the edge from p
+ * (value v0) to q = p + e_a (value v1) depends on vol; with g = grad_verts[v][a] (the other two components are ignored),
+ * in fp64 from the fp32 operands, one rounding per operation, in this order:
+ *     d = v1 - v0,  k = (g * s_a) / (d * d),  c0 = k * (level - v1) to p,  c1 = k * (v0 - level) to q.
+ * An edge with a non-finite end contributes 0.  Grid point p sums in fp64, from 0, its own crossing edges a = 0, 1, 2 (c0),
+ * then the edges arriving from p - e_a, a = 0, 1, 2 (c1), and rounds once to fp32; a point on no crossing edge gets 0.
+ * A gather without atomics: deterministic, bit-equal to the numpy restatement in tests/surface_grad_ref.py. */
+int genre_b200_isosurface_backward(const float *vol, int64_t N, int D, int H, int W, float level, float sx, float sy, float sz,
+                                   const int64_t *vert_off, const float *grad_verts, float *grad_vol, void *workspace,
+                                   size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * First-hit ray casting of batched triangle meshes (SURVEY 8f-4).  Replaces trimesh's
@@ -596,6 +608,15 @@ size_t genre_b200_surface_sample_workspace_bytes(int64_t N, int64_t F);
 int genre_b200_surface_sample(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
                               const int64_t *face_off, int64_t N, const uint64_t *seeds, int64_t n, float *points,
                               int32_t *face, void *workspace, size_t workspace_bytes, void *stream);
+/* backward: grad_verts [V, 3] fp32 (fully written: the call clears it first) = the gradient of the points with respect to the
+ * vertices, the drawn faces and barycentric draws held fixed (no gradient through the area weights).  faces, vert_off,
+ * face_off, seeds, N and n as in the forward call; face [N, n] the forward's output (trusted); grad_points [N, n, 3] fp32.
+ * Point i of sample b redraws (u, v) from (seed_b, i) as above and adds fl32(w * g) for w = 1 - u - v, u, v (exact in fp32)
+ * to its face's three vertices by fp32 atomicAdd: the order is unspecified, so the result is not bitwise reproducible.
+ * Points with face -1 contribute nothing.  No workspace. */
+int genre_b200_surface_sample_backward(const int32_t *faces, int64_t F, const int64_t *vert_off, const int64_t *face_off,
+                                       int64_t N, const uint64_t *seeds, int64_t n, const int32_t *face,
+                                       const float *grad_points, int64_t V, float *grad_verts, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Conservative voxelisation of batched triangle meshes, the inverse of genre_b200_isosurface_*: ground-truth meshes become

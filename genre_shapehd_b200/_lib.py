@@ -38,25 +38,17 @@ _SIGNATURES = {
     "genre_b200_nnd_forward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_nnd_backward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_convt3d_s2_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr, _ptr,
-                                      _f32, _ptr, _int, _ptr],
-    "genre_b200_convt3d_s2_forward_operands": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr,
-                                               _ptr, _f32, _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
-    "genre_b200_convt3d_s2_merged_forward_operands": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int,
-                                                      _ptr, _ptr, _f32, _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
-    "genre_b200_conv3d_k8s2_s4d_forward_operands": [_ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _ptr, _ptr, _f32,
-                                                    _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
-    "genre_b200_conv3d_k4s2_forward_operands": [_ptr, _int, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _ptr, _ptr, _f32,
-                                                _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
+                                      _f32, _ptr, _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
     "genre_b200_conv3d_taps_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _int, _ptr,
                                        _ptr, _f32, _ptr, _int, _ptr],
     "genre_b200_convt_c1_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _f32, _int, _ptr, _ptr],
     "genre_b200_conv3d_k4s2_forward": [_ptr, _int, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _ptr, _ptr, _f32, _ptr, _int,
-                                       _ptr],
+                                       _ptr, _int, _int, _ptr, _int, _int, _ptr],
     "genre_b200_blocked_split3": [_ptr, _int, _i64, _i64, _i64, _ptr, _ptr],
-    "genre_b200_convt3d_s2_merged_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr,
-                                             _ptr, _f32, _ptr, _int, _ptr],
+    "genre_b200_convt3d_s2_merged_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _int,
+                                             _ptr, _ptr, _f32, _ptr, _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
     "genre_b200_conv3d_k8s2_s4d_forward": [_ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _ptr, _ptr, _f32, _ptr,
-                                           _int, _ptr],
+                                           _int, _ptr, _int, _int, _ptr, _int, _int, _ptr],
     "genre_b200_convt_c1_tc_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _ptr, _int, _ptr, _ptr],
     "genre_b200_blocked_f32_to_f16": [_ptr, _int, _i64, _i64, _i64, _ptr, _ptr],
     "genre_b200_blocked_split2_f16": [_ptr, _int, _i64, _i64, _i64, _ptr, _ptr],
@@ -131,8 +123,6 @@ _LAUNCHES = {
     "genre_b200_bn_act_train_forward": 3, "genre_b200_bn_act_train_backward": 2, "genre_b200_conv_k8s2_wgrad": 2, "genre_b200_convt_c1_wgrad": 2, "genre_b200_convt_c1_dgrad": 1,
     "genre_b200_blocked_split3": 1, "genre_b200_blocked_split2_f16": 1, "genre_b200_voxel_surface": 2, "genre_b200_convt_c1_col2im_forward": 1, "genre_b200_skinny_gemm": 2, "genre_b200_convflat_pack": 1, "genre_b200_convflat_forward": 1, "genre_b200_convt_c1_tc_forward": 1, "genre_b200_blocked_f32_to_f16": 1,
     "genre_b200_convt3d_s2_merged_forward": 1, "genre_b200_conv3d_k8s2_s4d_forward": 1, "genre_b200_ncdhw_to_blocked": 1, "genre_b200_blocked_to_ncdhw": 1,
-    "genre_b200_convt3d_s2_forward_operands": 1, "genre_b200_convt3d_s2_merged_forward_operands": 1,
-    "genre_b200_conv3d_k8s2_s4d_forward_operands": 1, "genre_b200_conv3d_k4s2_forward_operands": 1,
     "genre_b200_isosurface_count": 2, "genre_b200_isosurface_emit": 2, "genre_b200_isosurface_backward": 1,
     # the kernel only when there are vertices (after a memset)
     "genre_b200_surface_sample_backward": lambda faces, F, vo, fo, N, seeds, n, face, gp, V, *_: 1 if V > 0 else 0,

@@ -26,7 +26,6 @@
 // empty barrier once its wgmma that read the slot have completed.  With 3 or more stages a stage's MMAs stay in flight while
 // the next stage is awaited and issued (wgmma.wait_group 1): its slot is released after the next stage's MMAs are committed.
 #include <cuda.h>   // CUtensorMap + the cuTensorMapEncodeTiled prototype (the entry point is resolved through the runtime: no -lcuda)
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -658,8 +657,6 @@ static int launch_convt_impl(const ConvTParams &p, cudaStream_t st) {
   }
 }
 
-// operand type of the next launch (set by the C ABI entry points): 0 TF32, 1 fp16, 2 fp16 hi/lo, 3 3xTF32 (two-level accumulator)
-static thread_local int g_conv_op = 0;
 // X2 doubles the accumulator columns (launch_convt_impl narrows the tile to fit them)
 template <int TZ, int T, int NPAD, int MT, int MODE>
 static int launch_convt_x2(const ConvTParams &p, cudaStream_t st) {
@@ -669,39 +666,39 @@ static int launch_convt_x2(const ConvTParams &p, cudaStream_t st) {
     return launch_convt_impl<TZ, T, NPAD, MT, MODE, 2>(p, st);
   }
 }
+// op: the operand type of the entry point's f16 argument, 0 TF32, 1 fp16, 2 fp16 hi/lo, 3 3xTF32 (two-level accumulator)
 template <int TZ, int T, int NPAD, int MT, int MODE>
-static int launch_convt_op(const ConvTParams &p, cudaStream_t st) {
-  if (g_conv_op == 2) return launch_convt_x2<TZ, T, NPAD, MT, MODE>(p, st);
-  if (g_conv_op == 3) {
+static int launch_convt_op(const ConvTParams &p, int op, cudaStream_t st) {
+  if (op == 2) return launch_convt_x2<TZ, T, NPAD, MT, MODE>(p, st);
+  if (op == 3) {
     if constexpr (2 * NPAD > CT_ACC_COLS)   // N > 128: no room for the second register set, one-level accumulation
       return launch_convt_impl<TZ, T, NPAD, MT, MODE, 0>(p, st);
     else
       return launch_convt_impl<TZ, T, NPAD, MT, MODE, 3>(p, st);
   }
-  return g_conv_op == 1 ? launch_convt_impl<TZ, T, NPAD, MT, MODE, 1>(p, st) : launch_convt_impl<TZ, T, NPAD, MT, MODE, 0>(p, st);
+  return op == 1 ? launch_convt_impl<TZ, T, NPAD, MT, MODE, 1>(p, st) : launch_convt_impl<TZ, T, NPAD, MT, MODE, 0>(p, st);
 }
 template <int T, int NPAD, int MT, bool PAR>
-static int launch_convt(const ConvTParams &p, cudaStream_t st) {
-  return launch_convt_op<T, T, NPAD, MT, PAR ? 0 : 1>(p, st);
+static int launch_convt(const ConvTParams &p, int op, cudaStream_t st) {
+  return launch_convt_op<T, T, NPAD, MT, PAR ? 0 : 1>(p, op, st);
 }
 template <int TZ, int T, int NPAD, int MT>
-static int launch_convt_merged(const ConvTParams &p, cudaStream_t st) {
-  return launch_convt_op<TZ, T, NPAD, MT, 2>(p, st);
+static int launch_convt_merged(const ConvTParams &p, int op, cudaStream_t st) {
+  return launch_convt_op<TZ, T, NPAD, MT, 2>(p, op, st);
 }
 // MODE 5, the fp16 operand modes: three M-tiles per CTA in fp16 (240 accumulator columns), one in the hi/lo split (X2
 // narrows it), N = 80
 template <int PW>
-static int launch_convt_paired(const ConvTParams &p, cudaStream_t st) {
-  return g_conv_op == 2 ? launch_convt_impl<4, 4, 80, 3, 5, 2, PW>(p, st) : launch_convt_impl<4, 4, 80, 3, 5, 1, PW>(p, st);
+static int launch_convt_paired(const ConvTParams &p, int op, cudaStream_t st) {
+  return op == 2 ? launch_convt_impl<4, 4, 80, 3, 5, 2, PW>(p, st) : launch_convt_impl<4, 4, 80, 3, 5, 1, PW>(p, st);
 }
-// the operand destinations of the *_operands entry points
+// the operand destinations dst0, layout0, cpad0, dst1, layout1, cpad1 of an entry point
 struct OperandOut {
   void *dst[2];
   int layout[2], cpad[2];
 };
 static int set_operand_outputs(ConvTParams &p, const OperandOut &o, int f16, int64_t Do, int64_t Ho, int64_t Wo, const char *who) {
   GB_REQUIRE(f16 == 1 || f16 == 2, GENRE_B200_EINVAL, "%s: operand outputs need fp16 operands (f16 = 1 or 2), not %d", who, f16);
-  GB_REQUIRE(o.dst[0], GENRE_B200_EINVAL, "%s: null pointer (first operand destination)", who);
   for (int d = 0; d < 2; ++d) {
     if (!o.dst[d]) continue;
     GB_REQUIRE(o.layout[d] == OP_PLAIN || o.layout[d] == OP_PARITY, GENRE_B200_EINVAL,
@@ -718,16 +715,37 @@ static int set_operand_outputs(ConvTParams &p, const OperandOut &o, int f16, int
   p.oparts = f16 == 2 ? 2 : 1;
   return 0;
 }
+// The checks every entry point of the halo kernel shares, and the ConvTParams they fill (the entry point sets base and
+// its own fields).  `who` prefixes the messages.  Exactly one of out and ops.dst[0] is set; the operand destinations are
+// those of an output extent `up` (1 or 2) times the input's.  out_align: the alignment the epilogue's stores to out need.
+static int halo_params(ConvTParams &p, const char *who, const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                       int64_t D, int64_t H, int64_t W, const void *wpack, int f16, const float *scale, const float *shift,
+                       float slope, float *out, int cgo, const OperandOut &ops, int up, int out_align = 16) {
+  GB_REQUIRE(src0 && wpack && scale && shift, GENRE_B200_EINVAL, "%s: null pointer", who);
+  GB_REQUIRE(out || ops.dst[0], GENRE_B200_EINVAL, "%s: null pointer (out, or the first operand destination)", who);
+  GB_REQUIRE(!(out && ops.dst[0]), GENRE_B200_EINVAL, "%s: both out and an operand destination given (one or the other)", who);
+  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "%s: bad extent", who);
+  GB_REQUIRE(cg0 > 0 && cg1 >= 0 && (cg0 + cg1) % CT_KCG == 0 && (cg1 == 0 || src1), GENRE_B200_EINVAL,
+             "%s: channel groups (%d + %d) must be even in total", who, cg0, cg1);
+  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "%s: grid too large", who);
+  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && (!src1 || aligned16(src1)) && ((uintptr_t)out & (out_align - 1)) == 0,
+             GENRE_B200_EALIGN, "%s: buffers must be 16-byte aligned, out %d-byte aligned", who, out_align);
+  p.src0 = (const float *)src0; p.src1 = (const float *)src1; p.cg0 = cg0; p.cg1 = cg1;
+  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
+  p.wpack = (const float *)wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
+  p.srcpar_cgs = 0;
+  return ops.dst[0] ? set_operand_outputs(p, ops, f16, up * D, up * H, up * W, who) : 0;
+}
 
 template <int MT>
-static int launch_convt_c1(const ConvTParams &p, cudaStream_t st) {
-  if (g_conv_op == 2)   // not routed (ops_conv.convt_c1_tc): the exact FP32-pipe stencil serves the fp32-accurate modes
+static int launch_convt_c1(const ConvTParams &p, int op, cudaStream_t st) {
+  if (op == 2)   // not routed (ops_conv.convt_c1_tc): the exact FP32-pipe stencil serves the fp32-accurate modes
     return fail_arg(GENRE_B200_EINVAL, "convt_c1_tc: the fp16 hi/lo operand mode is not supported for the 1-channel layer");
-  return g_conv_op == 1 ? launch_convt_impl<3, 3, 16, MT, 4, 1>(p, st) : launch_convt_impl<3, 3, 16, MT, 4, 0>(p, st);
+  return op == 1 ? launch_convt_impl<3, 3, 16, MT, 4, 1>(p, st) : launch_convt_impl<3, 3, 16, MT, 4, 0>(p, st);
 }
 template <int T, int NPAD, int MT>
-static int launch_conv_merged8(const ConvTParams &p, cudaStream_t st) {
-  return launch_convt_op<T, T, NPAD, MT, 3>(p, st);
+static int launch_conv_merged8(const ConvTParams &p, int op, cudaStream_t st) {
+  return launch_convt_op<T, T, NPAD, MT, 3>(p, op, st);
 }
 
 }  // namespace gb
@@ -738,33 +756,21 @@ using namespace gb;
 //   src0 [B*D][cg0][H][W][4], src1 [B*D][cg1][H][W][4] or NULL: the two halves of the channel concatenation
 //   wpack: weights packed by genre_shapehd_b200.ops_conv.pack_convt_weights (layout in the kernel header)
 //   scale, shift [npad]: per-channel affine applied to the accumulator (bias and folded eval-mode BatchNorm),
-//   slope: LeakyReLU slope (1 = none).   out [B*2D][cgo][2H][2W][4]
+//   slope: LeakyReLU slope (1 = none).   out [B*2D][cgo][2H][2W][4], or the operand destinations (OP_PLAIN / OP_PARITY)
 // Supported: W in {16, 32}, H % 16 == 0, cg0 + cg1 even, 4*cgo <= npad, npad in {32, 64}.
-static int convt3d_s2(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D, int64_t H, int64_t W,
-                      const void *wpack_, int ksize, int npad, int f16, const float *scale, const float *shift, float slope,
-                      float *out, int cgo, const OperandOut *ops, void *stream) {
-  const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "convt3d: null pointer");
+extern "C" int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B, int64_t D,
+                                             int64_t H, int64_t W, const void *wpack, int ksize, int npad, int f16,
+                                             const float *scale, const float *shift, float slope, float *out, int cgo,
+                                             void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                             void *stream) {
+  ConvTParams p;
+  const int rc = halo_params(p, "convt3d", src0, cg0, src1, cg1, B, D, H, W, wpack, f16, scale, shift, slope, out, cgo,
+                             {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}}, 2);
+  if (rc) return rc;
   GB_REQUIRE(ksize == 4 || ksize == 8, GENRE_B200_EINVAL, "convt3d: kernel size %d unsupported (4 or 8)", ksize);
   GB_REQUIRE(npad == 32 || npad == 64, GENRE_B200_EINVAL, "convt3d: npad %d unsupported (32 or 64)", npad);
   GB_REQUIRE(W == 16 || W == 32, GENRE_B200_EINVAL, "convt3d: input width %lld unsupported (16 or 32)", (long long)W);
-  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "convt3d: bad extent");
-  GB_REQUIRE(cg0 > 0 && cg1 >= 0 && (cg0 + cg1) % CT_KCG == 0 && (cg1 == 0 || src1), GENRE_B200_EINVAL,
-             "convt3d: channel groups (%d + %d) must be even in total", cg0, cg1);
   GB_REQUIRE(cgo > 0 && 4 * cgo <= npad, GENRE_B200_EINVAL, "convt3d: %d output channels exceed npad %d", 4 * cgo, npad);
-  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "convt3d: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && (!out || aligned16(out)) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
-             "convt3d: buffers must be 16-byte aligned");
-  ConvTParams p;
-  p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
-  p.srcpar_cgs = 0;
-  if (ops) {
-    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "convt3d");
-    if (rc) return rc;
-  }
   const int pad = ksize / 2 - 1;
   for (int par = 0; par < 2; ++par) {
     const int k0 = (par + pad) % 2;
@@ -772,7 +778,7 @@ static int convt3d_s2(const void *src0_, int cg0, const void *src1_, int cg1, in
   }
   cudaStream_t st = as_stream(stream);
   const int T = ksize / 2;
-#define GB_CT(TT, NN, MM) return launch_convt<TT, NN, MM, true>(p, st)
+#define GB_CT(TT, NN, MM) return launch_convt<TT, NN, MM, true>(p, f16, st)
   if (T == 4 && npad == 32 && W == 32) GB_CT(4, 32, 4);
   if (T == 4 && npad == 32 && W == 16) GB_CT(4, 32, 2);
   if (T == 2 && npad == 32 && W == 32) GB_CT(2, 32, 4);
@@ -784,87 +790,44 @@ static int convt3d_s2(const void *src0_, int cg0, const void *src1_, int cg1, in
 #undef GB_CT
   return fail_arg(GENRE_B200_EINVAL, "convt3d: no kernel instance for k=%d npad=%d W=%lld", ksize, npad, (long long)W);
 }
-extern "C" int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B, int64_t D,
-                                             int64_t H, int64_t W, const void *wpack, int ksize, int npad, int f16,
-                                             const float *scale, const float *shift, float slope, float *out, int cgo,
-                                             void *stream) {
-  return convt3d_s2(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
-}
-// The same layer writing the fp16 operand(s) of the next layers (layouts OP_PLAIN / OP_PARITY above) instead of `out`.
-extern "C" int genre_b200_convt3d_s2_forward_operands(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
-                                                      int64_t D, int64_t H, int64_t W, const void *wpack, int ksize, int npad,
-                                                      int f16, const float *scale, const float *shift, float slope, int cgo,
-                                                      void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
-                                                      void *stream) {
-  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
-  return convt3d_s2(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
-}
 
 // ConvTranspose3d(kernel 8, stride 2, padding 3) with the four (y,x) output parity classes merged along N (kernel MODE 2):
 // the layer that dominates Unet_3D, dec5 = ConvT(80 -> 20) on 32^3 (networks/networks.py:166).  Same operands as
 // genre_b200_convt3d_s2_forward except
 //   wpack, npad = 4 * cpad columns ordered n = (py*2+px)*cpad + co;  scale, shift [cpad]:
-//     fp16 operands (f16 = 1, 2) and W in {16, 32}, GENRE_B200_CONVT_UNION unset or "0": paired classes (kernel MODE 5)
+//     paired = 1 (fp16 operands f16 = 1, 2 and W in {16, 32} only): paired classes (kernel MODE 5)
 //         [2 z-parity][4 z-tap][Cin chunk][4*4 taps][2][npad/8][8][8]  (ops_conv.pack_convt_paired_weights)
-//     otherwise: the 5 x 5 union of the classes' taps (kernel MODE 2)
+//     paired = 0: the 5 x 5 union of the classes' taps (kernel MODE 2)
 //         [2 z-parity][4 z-tap][Cin chunk][5*5 union taps][2][npad/8][8][g]  (ops_conv.pack_convt_merged_weights)
 // Supported: ksize 8, npad = 80 (Cout <= 20), W = 16 or a multiple of 32, H % 16 == 0.
-static int convt3d_s2_merged(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D, int64_t H,
-                             int64_t W, const void *wpack_, int ksize, int npad, int f16, const float *scale,
-                             const float *shift, float slope, float *out, int cgo, const OperandOut *ops, void *stream) {
-  const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "convt3d_merged: null pointer");
+extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                                                    int64_t D, int64_t H, int64_t W, const void *wpack, int ksize,
+                                                    int npad, int f16, int paired, const float *scale, const float *shift,
+                                                    float slope, float *out, int cgo, void *dst0, int layout0, int cpad0,
+                                                    void *dst1, int layout1, int cpad1, void *stream) {
+  ConvTParams p;
+  const int rc = halo_params(p, "convt3d_merged", src0, cg0, src1, cg1, B, D, H, W, wpack, f16, scale, shift, slope, out, cgo,
+                             {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}}, 2);
+  if (rc) return rc;
   GB_REQUIRE(ksize == 8, GENRE_B200_EINVAL, "convt3d_merged: kernel size %d unsupported (8)", ksize);
   GB_REQUIRE(npad == 80, GENRE_B200_EINVAL, "convt3d_merged: npad %d unsupported (80 = 4 classes x 20 channels)", npad);
   GB_REQUIRE(W == 16 || (W > 0 && W % 32 == 0), GENRE_B200_EINVAL,
              "convt3d_merged: input width %lld unsupported (16, or a multiple of 32 walked in 32-wide tiles)", (long long)W);
-  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "convt3d_merged: bad extent");
-  GB_REQUIRE(cg0 > 0 && cg1 >= 0 && (cg0 + cg1) % CT_KCG == 0 && (cg1 == 0 || src1), GENRE_B200_EINVAL,
-             "convt3d_merged: channel groups (%d + %d) must be even in total", cg0, cg1);
   GB_REQUIRE(cgo > 0 && 16 * cgo <= npad, GENRE_B200_EINVAL, "convt3d_merged: %d output channels exceed npad/4", 4 * cgo);
-  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "convt3d_merged: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && (!out || aligned16(out)) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
-             "convt3d_merged: buffers must be 16-byte aligned");
-  ConvTParams p;
-  p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
-  p.srcpar_cgs = 0;
-  if (ops) {
-    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "convt3d_merged");
-    if (rc) return rc;
-  }
+  GB_REQUIRE(paired == 0 || paired == 1, GENRE_B200_EINVAL,
+             "convt3d_merged: paired = %d unknown (1 = paired classes, 0 = the union of their taps)", paired);
+  GB_REQUIRE(!paired || ((f16 == 1 || f16 == 2) && (W == 16 || W == 32)), GENRE_B200_EINVAL,
+             "convt3d_merged: the paired classes need fp16 operands (f16 = 1 or 2) and W = 16 or 32, not f16 = %d, W = %lld",
+             f16, (long long)W);
   const int pad = ksize / 2 - 1;
   for (int par = 0; par < 2; ++par) {
     const int k0 = (par + pad) % 2;
     p.base[par] = (par + pad - k0) / 2;
   }
   cudaStream_t st = as_stream(stream);
-  // paired classes (MODE 5) at the widths it is built for, unless GENRE_B200_CONVT_UNION is set (to anything but "0"): the
-  // union form, for comparing the two (ops_conv reads the same variable to pick the packer)
-  const char *union_env = getenv("GENRE_B200_CONVT_UNION");
-  if ((f16 == 1 || f16 == 2) && !(union_env && union_env[0] && strcmp(union_env, "0") != 0)) {
-    if (W == 32) return launch_convt_paired<32>(p, st);
-    if (W == 16) return launch_convt_paired<16>(p, st);
-  }
-  if (W % 32 == 0) return launch_convt_merged<4, 5, 80, 4>(p, st);  // 32-wide x tiles
-  return launch_convt_merged<4, 5, 80, 2>(p, st);
-}
-extern "C" int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
-                                                    int64_t D, int64_t H, int64_t W, const void *wpack, int ksize,
-                                                    int npad, int f16, const float *scale, const float *shift,
-                                                    float slope, float *out, int cgo, void *stream) {
-  return convt3d_s2_merged(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
-}
-extern "C" int genre_b200_convt3d_s2_merged_forward_operands(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
-                                                             int64_t D, int64_t H, int64_t W, const void *wpack, int ksize,
-                                                             int npad, int f16, const float *scale, const float *shift,
-                                                             float slope, int cgo, void *dst0, int layout0, int cpad0,
-                                                             void *dst1, int layout1, int cpad1, void *stream) {
-  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
-  return convt3d_s2_merged(src0, cg0, src1, cg1, B, D, H, W, wpack, ksize, npad, f16, scale, shift, slope, nullptr, cgo, &ops,
-                           stream);
+  if (paired) return W == 32 ? launch_convt_paired<32>(p, f16, st) : launch_convt_paired<16>(p, f16, st);
+  if (W % 32 == 0) return launch_convt_merged<4, 5, 80, 4>(p, f16, st);  // 32-wide x tiles
+  return launch_convt_merged<4, 5, 80, 2>(p, f16, st);
 }
 
 // Conv3d(kernel 8, stride 2, padding 3), few input channels, Cout <= 20, on a 4x space-to-depth input (kernel MODE 3):
@@ -872,47 +835,26 @@ extern "C" int genre_b200_convt3d_s2_merged_forward_operands(const void *src0, i
 //   src [B*D][cg][H][W][16 B]: D,H,W = input extent / 4, channels ((c*4+rz)*4+ry)*4+rx (genre_b200_ncdhw_to_blocked mode 3)
 //   wpack [3 z-tap][chunk][9 taps][2][npad/8][8][g], npad = 160 columns n = ((qz*2+qy)*2+qx)*20 + co
 //         (ops_conv.pack_conv_k8s2_s4d_weights);  scale, shift [20];  out [B*2D][cgo][2H][2W][4] fp32
-// Supported: W % 16 == 0, H % 16 == 0, cg even.
-static int conv3d_k8s2_s4d(const void *src_, int cg, int64_t B, int64_t D, int64_t H, int64_t W, const void *wpack_, int npad,
-                           int f16, const float *scale, const float *shift, float slope, float *out, int cgo,
-                           const OperandOut *ops, void *stream) {
-  const float *src = (const float *)src_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "conv3d_k8s2_s4d: null pointer");
+// Supported: W % 16 == 0, H % 16 == 0, cg even.  The operand outputs of enc1 are those of enc2 (OP_PARITY: output class q at
+// coarse position j IS sub-volume q at j) and dec6.
+extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
+                                                  const void *wpack, int npad, int f16, const float *scale,
+                                                  const float *shift, float slope, float *out, int cgo, void *dst0, int layout0,
+                                                  int cpad0, void *dst1, int layout1, int cpad1, void *stream) {
+  ConvTParams p;
+  const int rc = halo_params(p, "conv3d_k8s2_s4d", src, cg, nullptr, 0, B, D, H, W, wpack, f16, scale, shift, slope, out, cgo,
+                             {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}}, 2);
+  if (rc) return rc;
   GB_REQUIRE(npad == 160 || npad == 80, GENRE_B200_EINVAL,
              "conv3d_k8s2_s4d: npad %d unsupported (160 = 8 classes x 20 channels, or 80 = 4 (y,x) classes per z class)", npad);
-  GB_REQUIRE(W > 0 && W % 16 == 0 && H > 0 && H % CT_BY == 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: bad extent");
-  GB_REQUIRE(cg > 0 && cg % CT_KCG == 0, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: channel groups must be even");
+  GB_REQUIRE(W > 0 && W % 16 == 0, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: bad extent");
   GB_REQUIRE(cgo > 0 && cgo <= 5, GENRE_B200_EINVAL, "conv3d_k8s2_s4d: too many output channels");
   GB_REQUIRE(B * D * (H / CT_BY) * (W / 16) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_k8s2_s4d: grid too large");
-  GB_REQUIRE(aligned16(src) && aligned16(wpack) && (!out || aligned16(out)), GENRE_B200_EALIGN, "conv3d_k8s2_s4d: alignment");
-  ConvTParams p;
-  p.src0 = src; p.src1 = nullptr; p.cg0 = cg; p.cg1 = 0;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
-  p.srcpar_cgs = 0;
-  if (ops) {
-    const int rc = set_operand_outputs(p, *ops, f16, 2 * D, 2 * H, 2 * W, "conv3d_k8s2_s4d");
-    if (rc) return rc;
-  }
   p.base[0] = p.base[1] = 1;  // input cell = j + 1 - t
   // npad 80: the z class moves to blockIdx.y (MODE 2 with 3 z taps per class; wpack [2 qz][3][chunk][9][2][10][8][g]):
   // twice the MMAs of the 8-class form, but half the accumulator columns and weight bytes per stage
-  if (npad == 80) return launch_convt_merged<3, 3, 80, 2>(p, as_stream(stream));
-  return launch_conv_merged8<3, 160, 2>(p, as_stream(stream));
-}
-extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
-                                                  const void *wpack, int npad, int f16, const float *scale,
-                                                  const float *shift, float slope, float *out, int cgo, void *stream) {
-  return conv3d_k8s2_s4d(src, cg, B, D, H, W, wpack, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
-}
-// enc1 writing the fp16 operands of enc2 (OP_PARITY: output class q at coarse position j IS sub-volume q at j) and dec6
-extern "C" int genre_b200_conv3d_k8s2_s4d_forward_operands(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
-                                                           const void *wpack, int npad, int f16, const float *scale,
-                                                           const float *shift, float slope, int cgo, void *dst0, int layout0,
-                                                           int cpad0, void *dst1, int layout1, int cpad1, void *stream) {
-  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
-  return conv3d_k8s2_s4d(src, cg, B, D, H, W, wpack, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
+  if (npad == 80) return launch_convt_merged<3, 3, 80, 2>(p, f16, as_stream(stream));
+  return launch_conv_merged8<3, 160, 2>(p, f16, as_stream(stream));
 }
 
 // ConvTranspose3d(Cin -> 1, k 4, s 2, p 1) on the tensor cores (kernel MODE 4): the last layer of every decoder
@@ -921,30 +863,20 @@ extern "C" int genre_b200_conv3d_k8s2_s4d_forward_operands(const void *src, int 
 //   src0/src1 blocked operands [B*D][cg][H][W][16 B] (two halves of a skip concatenation; src1 may be NULL)
 //   wpack [3][chunk][9][2][2][8][g] (ops_conv.pack_convt_c1_tc_weights), bias, act_sigmoid;  out [B][2D][2H][2W] fp32
 // Supported: W in {16, 32, 64}, H % 16 == 0, cg0 + cg1 even.
-extern "C" int genre_b200_convt_c1_tc_forward(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B, int64_t D,
-                                              int64_t H, int64_t W, const void *wpack_, int f16, const float *bias,
+extern "C" int genre_b200_convt_c1_tc_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B, int64_t D,
+                                              int64_t H, int64_t W, const void *wpack, int f16, const float *bias,
                                               int act_sigmoid, float *out, void *stream) {
-  const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && bias && out, GENRE_B200_EINVAL, "convt_c1_tc: null pointer");
+  ConvTParams p;   // out takes float2 stores: 8-byte aligned
+  const int rc = halo_params(p, "convt_c1_tc", src0, cg0, src1, cg1, B, D, H, W, wpack, f16, bias, bias, 1.0f, out, 1,
+                             OperandOut{}, 2, 8);
+  if (rc) return rc;
   GB_REQUIRE(W == 16 || W == 32 || W == 64, GENRE_B200_EINVAL, "convt_c1_tc: input width %lld unsupported", (long long)W);
-  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "convt_c1_tc: bad extent");
-  GB_REQUIRE(cg0 > 0 && cg1 >= 0 && (cg0 + cg1) % CT_KCG == 0 && (cg1 == 0 || src1), GENRE_B200_EINVAL,
-             "convt_c1_tc: channel groups (%d + %d) must be even in total", cg0, cg1);
-  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "convt_c1_tc: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && ((uintptr_t)out & 7) == 0 && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
-             "convt_c1_tc: alignment");
-  ConvTParams p;
-  p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = bias; p.shift = bias; p.slope = 1.0f; p.out = out; p.cgo = 1;
-  p.srcpar_cgs = 0;
   p.act_sigmoid = act_sigmoid;
   p.base[0] = p.base[1] = 1;
   cudaStream_t st = as_stream(stream);
-  if (W == 64) return launch_convt_c1<8>(p, st);
-  if (W == 32) return launch_convt_c1<4>(p, st);
-  return launch_convt_c1<2>(p, st);
+  if (W == 64) return launch_convt_c1<8>(p, f16, st);
+  if (W == 32) return launch_convt_c1<4>(p, f16, st);
+  return launch_convt_c1<2>(p, f16, st);
 }
 
 // Stride-1 convolution with T taps per dimension on channel-blocked activations (same kernel, one output class):
@@ -953,43 +885,33 @@ extern "C" int genre_b200_convt_c1_tc_forward(const void *src0_, int cg0, const 
 // Conv3d(2 -> 20, k=8, s=2, p=3) (networks/networks.py:151) is a 5-tap stride-1 convolution over the 16 s2d channels.
 //   wpack [T z-tap][C/8 chunk][T*T taps][2][npad/8][8][4];  out [B*D][cgo][H][W][4]
 // Supported: T in {3, 5}, W in {16, 32, 64}, H % 16 == 0, npad = 32 (or 64 with T = 3, 96 with T = 5).
-extern "C" int genre_b200_conv3d_taps_forward(const void *src0_, int cg0, const void *src1_, int cg1, int64_t B,
-                                              int64_t D, int64_t H, int64_t W, const void *wpack_, int taps, int base,
+extern "C" int genre_b200_conv3d_taps_forward(const void *src0, int cg0, const void *src1, int cg1, int64_t B,
+                                              int64_t D, int64_t H, int64_t W, const void *wpack, int taps, int base,
                                               int npad, int f16, const float *scale, const float *shift, float slope,
                                               float *out, int cgo, void *stream) {
-  const float *src0 = (const float *)src0_, *src1 = (const float *)src1_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src0 && wpack && scale && shift && out, GENRE_B200_EINVAL, "conv3d_taps: null pointer");
+  ConvTParams p;
+  const int rc = halo_params(p, "conv3d_taps", src0, cg0, src1, cg1, B, D, H, W, wpack, f16, scale, shift, slope, out, cgo,
+                             OperandOut{}, 1);
+  if (rc) return rc;
   GB_REQUIRE(taps == 3 || taps == 5, GENRE_B200_EINVAL, "conv3d_taps: %d taps unsupported (3 or 5)", taps);
   GB_REQUIRE(npad == 32 || (npad == 64 && taps == 3) || (npad == 96 && taps == 5), GENRE_B200_EINVAL,
              "conv3d_taps: npad %d unsupported (32; 64 with 3 taps; 96 with 5 taps)", npad);
   GB_REQUIRE(W == 16 || W == 32 || W == 64, GENRE_B200_EINVAL, "conv3d_taps: width %lld unsupported", (long long)W);
-  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "conv3d_taps: bad extent");
-  GB_REQUIRE(cg0 > 0 && cg1 >= 0 && (cg0 + cg1) % CT_KCG == 0 && (cg1 == 0 || src1), GENRE_B200_EINVAL,
-             "conv3d_taps: channel groups (%d + %d) must be even in total", cg0, cg1);
   GB_REQUIRE(cgo > 0 && 4 * cgo <= npad, GENRE_B200_EINVAL, "conv3d_taps: too many output channels");
-  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_taps: grid too large");
-  GB_REQUIRE(aligned16(src0) && aligned16(wpack) && aligned16(out) && (!src1 || aligned16(src1)), GENRE_B200_EALIGN,
-             "conv3d_taps: buffers must be 16-byte aligned");
-  ConvTParams p;
-  p.src0 = src0; p.src1 = src1; p.cg0 = cg0; p.cg1 = cg1;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
-  p.srcpar_cgs = 0;
   p.base[0] = p.base[1] = base;
   cudaStream_t st = as_stream(stream);
   // 3 taps, N = 64: Conv3d(1 -> 64, k4, s2, p1) over the 2x space-to-depth input (VoxelDiscriminator's first layer)
   if (taps == 3 && npad == 64) {
-    if (W % 32 == 0) return launch_convt<3, 64, 4, false>(p, st);
-    return launch_convt<3, 64, 2, false>(p, st);
+    if (W % 32 == 0) return launch_convt<3, 64, 4, false>(p, f16, st);
+    return launch_convt<3, 64, 2, false>(p, f16, st);
   }
   // 5 taps, N = 96: Conv3d(20 -> 80, k8, s2, p3) over the 2x space-to-depth input = the input gradient of Unet_3D.dec5
   // (ConvTranspose3d 80 -> 20)
   if (taps == 5 && npad == 96) {
-    if (W % 32 == 0) return launch_convt<5, 96, 4, false>(p, st);
-    return launch_convt<5, 96, 2, false>(p, st);
+    if (W % 32 == 0) return launch_convt<5, 96, 4, false>(p, f16, st);
+    return launch_convt<5, 96, 2, false>(p, f16, st);
   }
-#define GB_CV(TT, MM) return launch_convt<TT, 32, MM, false>(p, st)
+#define GB_CV(TT, MM) return launch_convt<TT, 32, MM, false>(p, f16, st)
   if (taps == 5 && W == 64) GB_CV(5, 8);
   if (taps == 5 && W == 32) GB_CV(5, 4);
   if (taps == 5 && W == 16) GB_CV(5, 2);
@@ -1007,31 +929,22 @@ extern "C" int genre_b200_conv3d_taps_forward(const void *src0_, int cg0, const 
 //   wpack [2 z-tap][kblocks*8*cgs/2 chunk][4 taps][2][npad/8][8][g];  out [B*D'][cgo][H'][W'][4] fp32
 //   kblocks (1, or 3 for the hi|lo|hi operand of the 3xTF32 mode): how many such 8-sub-volume blocks the K range holds
 // Supported: W' in {16, 32}, H' % 16 == 0, cgs even, npad in {32, 64, 96, 128}.
-static int conv3d_k4s2(const void *src_, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W, const void *wpack_,
-                       int npad, int f16, const float *scale, const float *shift, float slope, float *out, int cgo,
-                       const OperandOut *ops, void *stream) {
-  const float *src = (const float *)src_, *wpack = (const float *)wpack_;
-  g_conv_op = f16;
-  GB_REQUIRE(src && wpack && scale && shift && (out || ops), GENRE_B200_EINVAL, "conv3d_k4s2: null pointer");
+extern "C" int genre_b200_conv3d_k4s2_forward(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
+                                              const void *wpack, int npad, int f16, const float *scale, const float *shift,
+                                              float slope, float *out, int cgo, void *dst0, int layout0, int cpad0, void *dst1,
+                                              int layout1, int cpad1, void *stream) {
+  ConvTParams p;
+  const int rc = halo_params(p, "conv3d_k4s2", src, 8 * cgs * (kblocks > 0 ? kblocks : 1), nullptr, 0, B, D, H, W, wpack, f16,
+                             scale, shift, slope, out, cgo, {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}}, 1);
+  if (rc) return rc;
   GB_REQUIRE(npad == 32 || npad == 64 || npad == 96 || npad == 128, GENRE_B200_EINVAL, "conv3d_k4s2: npad %d", npad);
   GB_REQUIRE(W == 16 || W == 32, GENRE_B200_EINVAL, "conv3d_k4s2: output width %lld unsupported (16 or 32)", (long long)W);
-  GB_REQUIRE(H % CT_BY == 0 && H > 0 && D > 0 && B > 0, GENRE_B200_EINVAL, "conv3d_k4s2: bad extent");
   GB_REQUIRE(cgs > 0 && cgs % CT_KCG == 0, GENRE_B200_EINVAL, "conv3d_k4s2: channel groups per sub-volume must be even");
   GB_REQUIRE(cgo > 0 && 4 * cgo <= npad, GENRE_B200_EINVAL, "conv3d_k4s2: too many output channels");
-  GB_REQUIRE(B * D * (H / CT_BY) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_k4s2: grid too large");
-  GB_REQUIRE(aligned16(src) && aligned16(wpack) && (!out || aligned16(out)), GENRE_B200_EALIGN, "conv3d_k4s2: alignment");
-  ConvTParams p;
-  p.src0 = src; p.src1 = nullptr; p.cg0 = 8 * cgs * (kblocks > 0 ? kblocks : 1); p.cg1 = 0;
-  p.B = (int)B; p.D = (int)D; p.H = (int)H; p.W = (int)W;
-  p.wpack = wpack; p.scale = scale; p.shift = shift; p.slope = slope; p.out = out; p.cgo = cgo;
   p.srcpar_cgs = cgs;
-  if (ops) {
-    const int rc = set_operand_outputs(p, *ops, f16, D, H, W, "conv3d_k4s2");
-    if (rc) return rc;
-  }
   p.base[0] = p.base[1] = 0;
   cudaStream_t st = as_stream(stream);
-#define GB_CS(NN, MM) return launch_convt<2, NN, MM, false>(p, st)
+#define GB_CS(NN, MM) return launch_convt<2, NN, MM, false>(p, f16, st)
   if (W == 32) {
     if (npad == 32) GB_CS(32, 4);
     if (npad == 64) GB_CS(64, 4);
@@ -1045,16 +958,4 @@ static int conv3d_k4s2(const void *src_, int cgs, int kblocks, int64_t B, int64_
   }
 #undef GB_CS
   return fail_arg(GENRE_B200_EINVAL, "conv3d_k4s2: no kernel instance");
-}
-extern "C" int genre_b200_conv3d_k4s2_forward(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
-                                              const void *wpack, int npad, int f16, const float *scale, const float *shift,
-                                              float slope, float *out, int cgo, void *stream) {
-  return conv3d_k4s2(src, cgs, kblocks, B, D, H, W, wpack, npad, f16, scale, shift, slope, out, cgo, nullptr, stream);
-}
-extern "C" int genre_b200_conv3d_k4s2_forward_operands(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H,
-                                                       int64_t W, const void *wpack, int npad, int f16, const float *scale,
-                                                       const float *shift, float slope, int cgo, void *dst0, int layout0,
-                                                       int cpad0, void *dst1, int layout1, int cpad1, void *stream) {
-  const OperandOut ops = {{dst0, dst1}, {layout0, layout1}, {cpad0, cpad1}};
-  return conv3d_k4s2(src, cgs, kblocks, B, D, H, W, wpack, npad, f16, scale, shift, slope, nullptr, cgo, &ops, stream);
 }

@@ -68,17 +68,15 @@ PRECISION = os.environ.get("GENRE_B200_CONV_PRECISION", "exact")
 EXACT_IMPL = os.environ.get("GENRE_B200_CONV_EXACT_IMPL", "f16x2")
 # k=8 ConvTranspose3d with Cout <= 20 (Unet_3D.dec5): merge the four (y,x) parity classes into one N=80 MMA stream
 MERGE_PARITIES = os.environ.get("GENRE_B200_CONV_MERGE", "1") != "0"
-# ... and with fp16 operands at W in {16, 32} the library runs the merged classes PAIRED (4 x 4 taps, csrc/convt3d.cu MODE 5)
-# instead of over their 5 x 5 union of taps (MODE 2).  The library reads this variable on every call, so it is read here on
-# every call too: the packer has to match the form the kernel takes.  "1" keeps the union form (bit-identical, 28 % more MMAs).
-UNION_ENV = "GENRE_B200_CONVT_UNION"
 # Unet_3D.enc1 (4x space-to-depth form): z class on blockIdx.y (N = 80, two CTAs per SM) instead of all 8 classes in N = 160
 S4D_SPLIT_Z = os.environ.get("GENRE_B200_S4D_SPLIT_Z", "0") != "0"   # measured: 0.88 vs 0.80 ms, so off
 
 
 def _paired_classes(group, w):
-    """does genre_b200_convt3d_s2_merged_forward take the paired form (and the paired weight layout)?"""
-    return group == 8 and w in (16, 32) and os.environ.get(UNION_ENV, "0") in ("", "0")
+    """run the merged classes of genre_b200_convt3d_s2_merged_forward PAIRED (4 x 4 taps, csrc/convt3d.cu MODE 5) rather than
+    over their 5 x 5 union of taps (MODE 2)?  The fp16 operands at W in {16, 32}; the answer picks the packer and is the
+    entry point's `paired` argument."""
+    return group == 8 and w in (16, 32)
 
 
 # With torch.backends.cudnn.allow_tf32 off the caller asks for fp32 convolutions: the kernels then run the 3xTF32 scheme
@@ -412,9 +410,12 @@ def deconv_operand_layout(x_shape, skip_shape, conv, bn=None):
     return PLAIN, x_shape[1]
 
 
-def _operand_request(operands):
-    """the operand outputs a producer is asked for, if the current mode writes fp16 operands"""
-    return operands if operands and _mode() in ("f16x2", "f16") else None
+def _operand_request(operands, shape, device):
+    """the operand outputs a producer is asked for, if the current mode writes fp16 operands, as _operand_destinations
+    allocates them; else (None, no destinations): the producer writes its fp32 output"""
+    if operands and _mode() in ("f16x2", "f16"):
+        return _operand_destinations(operands, shape, device)
+    return None, [None, 0, 0] * 2
 
 
 def _operand_destinations(operands, shape, device):
@@ -663,34 +664,27 @@ def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0, operands=N
     aff = _affine(module, bn, npad, dev)
     if aff is None:
         return None
-    operands = _operand_request(operands)
-    if operands:
-        act, dst = _operand_destinations(operands, (batch, cout, 2 * (bd // batch), 2 * h, 2 * w), dev)
-    else:
-        out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=dev, dtype=torch.float32)
+    act, dst = _operand_request(operands, (batch, cout, 2 * (bd // batch), 2 * h, 2 * w), dev)
+    out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=dev, dtype=torch.float32) if act is None else None
     src1_ptr = src1.data_ptr() if src1 is not None else None
     op = _op_flag() if g == 8 or _x3() else 0
+    out_ptr = out.data_ptr() if out is not None else None
     if merged:
         # the four (y,x) parity classes share one MMA stream: N = 4 x 20 columns (csrc/convt3d.cu MODE 5 paired, else MODE 2)
-        if _paired_classes(g, w):
+        paired = _paired_classes(g, w)
+        if paired:
             wpack = _pack(module, ("convt_paired", 20, g), lambda wt: pack_convt_paired_weights(wt, 20, g), 2)
         else:
             wpack = _pack(module, ("convt_merged", 20, g), lambda wt: pack_convt_merged_weights(wt, 20, g), 2)
-        head = (src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w, wpack.data_ptr(), 8, 80, op, aff[0].data_ptr(),
-                aff[1].data_ptr(), float(slope))
-        if operands:
-            _lib.call("genre_b200_convt3d_s2_merged_forward_operands", *head, cgo, *dst, _lib.stream_ptr(src0))
-            return act
-        _lib.call("genre_b200_convt3d_s2_merged_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(src0))
-        return out
-    wpack = _pack(module, ("convt", npad, g), lambda wt: pack_convt_weights(wt, npad, g), 4)
-    head = (src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w, wpack.data_ptr(), module.kernel_size[0], npad, op,
-            aff[0].data_ptr(), aff[1].data_ptr(), float(slope))
-    if operands:
-        _lib.call("genre_b200_convt3d_s2_forward_operands", *head, cgo, *dst, _lib.stream_ptr(src0))
-        return act
-    _lib.call("genre_b200_convt3d_s2_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(src0))
-    return out
+        _lib.call("genre_b200_convt3d_s2_merged_forward", src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w,
+                  wpack.data_ptr(), 8, 80, op, int(paired), aff[0].data_ptr(), aff[1].data_ptr(), float(slope), out_ptr, cgo,
+                  *dst, _lib.stream_ptr(src0))
+    else:
+        wpack = _pack(module, ("convt", npad, g), lambda wt: pack_convt_weights(wt, npad, g), 4)
+        _lib.call("genre_b200_convt3d_s2_forward", src0.data_ptr(), cg0, src1_ptr, cg1, batch, bd // batch, h, w,
+                  wpack.data_ptr(), module.kernel_size[0], npad, op, aff[0].data_ptr(), aff[1].data_ptr(), float(slope), out_ptr,
+                  cgo, *dst, _lib.stream_ptr(src0))
+    return out if act is None else act
 
 
 def _no_autograd(*tensors):
@@ -972,16 +966,12 @@ def _conv_k4s2(x, m, bn, slope, operands=None):
     b = x.shape[0]
     bd, _, h, wd, _ = xb.shape
     cgo = (cout + 3) // 4
-    head = (xb.data_ptr(), cpad // g, 3 if _x3() else 1, b, bd // b, h, wd, wpack.data_ptr(), npad, _op_flag(), aff[0].data_ptr(),
-            aff[1].data_ptr(), 1.0 if slope is None else float(slope))
-    operands = _operand_request(operands)
-    if operands:
-        act, dst = _operand_destinations(operands, (b, cout, bd // b, h, wd), x.device)
-        _lib.call("genre_b200_conv3d_k4s2_forward_operands", *head, cgo, *dst, _lib.stream_ptr(xb))
-        return act
-    out = torch.empty((bd, cgo, h, wd, 4), device=x.device, dtype=torch.float32)
-    _lib.call("genre_b200_conv3d_k4s2_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(xb))
-    return from_blocked(out, b, cout)
+    act, dst = _operand_request(operands, (b, cout, bd // b, h, wd), x.device)
+    out = torch.empty((bd, cgo, h, wd, 4), device=x.device, dtype=torch.float32) if act is None else None
+    _lib.call("genre_b200_conv3d_k4s2_forward", xb.data_ptr(), cpad // g, 3 if _x3() else 1, b, bd // b, h, wd, wpack.data_ptr(),
+              npad, _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
+              out.data_ptr() if out is not None else None, cgo, *dst, _lib.stream_ptr(xb))
+    return from_blocked(out, b, cout) if act is None else act
 
 
 # ---- small volumes: the flattened, zero-separated implicit GEMM (csrc/convflat.cu) ------------------------------------------
@@ -1246,7 +1236,8 @@ def dgrad_conv_k8s2(gy, m):
             one = m.__dict__["_gb_dgrad_affine"] = (torch.ones(96, device=gy.device), torch.zeros(96, device=gy.device))
         out = torch.empty((bd * 2, cgo, 2 * hh, 2 * ww, 4), device=gy.device, dtype=torch.float32)
         _lib.call("genre_b200_convt3d_s2_merged_forward", src.data_ptr(), cg, None, 0, b, bd // b, hh, ww, wpack.data_ptr(), 8, 80,
-                  _op_flag(), one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, _lib.stream_ptr(gy))
+                  _op_flag(), 0, one[0].data_ptr(), one[1].data_ptr(), 1.0, out.data_ptr(), cgo, None, 0, 0, None, 0, 0,
+                  _lib.stream_ptr(gy))
         dx = from_blocked(out, b, cin)
         dx.__dict__.pop("_gb_blocked", None)
         return dx
@@ -1407,16 +1398,13 @@ def conv3d(x, m, bn=None, slope=None, operands=None):
             xb = _finish_operand(space_to_depth4_blocked(x, _act_group(), torch.float16 if _f16() else None))
         bd, cg, h, w, _ = xb.shape
         cgo = (cout + 3) // 4
-        head = (xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(), 80 if split_z else 160, _op_flag(),
-                aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope))
-        operands = _operand_request(operands)
-        if operands:   # output class q at coarse position j is enc2's parity sub-volume q at j
-            act, dst = _operand_destinations(operands, (b, cout, 2 * (bd // b), 2 * h, 2 * w), x.device)
-            _lib.call("genre_b200_conv3d_k8s2_s4d_forward_operands", *head, cgo, *dst, _lib.stream_ptr(x))
-            return act
-        out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=x.device, dtype=torch.float32)
-        _lib.call("genre_b200_conv3d_k8s2_s4d_forward", *head, out.data_ptr(), cgo, _lib.stream_ptr(x))
-        return from_blocked(out, b, cout)
+        # operand outputs: output class q at coarse position j is enc2's parity sub-volume q at j
+        act, dst = _operand_request(operands, (b, cout, 2 * (bd // b), 2 * h, 2 * w), x.device)
+        out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=x.device, dtype=torch.float32) if act is None else None
+        _lib.call("genre_b200_conv3d_k8s2_s4d_forward", xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(),
+                  80 if split_z else 160, _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
+                  out.data_ptr() if out is not None else None, cgo, *dst, _lib.stream_ptr(x))
+        return from_blocked(out, b, cout) if act is None else act
     cout, npad = m.out_channels, 32
     aff = _affine(m, bn, npad, x.device)
     if aff is None:

@@ -181,46 +181,27 @@ int genre_b200_voxelize_stage_splat(int64_t n_maps, int64_t pixels_per_map, int 
  *           the kernels are bound by shared-memory operand bandwidth, so this path is ~2x faster)
  *   wpack   weights packed per (parity, z-tap, 8-channel chunk) stage: see genre_shapehd_b200/ops_conv.py
  *   scale, shift [npad]   y = act(acc * scale + shift): bias and folded eval-mode BatchNorm3d
- *   slope   LeakyReLU slope (1 = none);   out [B*2D][cgo][2H][2W][4]
+ *   slope   LeakyReLU slope (1 = none);   out [B*2D][cgo][2H][2W][4], or NULL with operand outputs (below)
  * Supported: W in {16,32}, H % 16 == 0, cg0 + cg1 even, 4*cgo <= npad, npad in {32,64}.
+ *
+ * Operand outputs.  genre_b200_convt3d_s2_forward, genre_b200_convt3d_s2_merged_forward, genre_b200_conv3d_k8s2_s4d_forward
+ * and genre_b200_conv3d_k4s2_forward write either `out` or, instead, up to two destinations dst0, dst1 (dst1 may be NULL) of
+ * the fp16 operand the NEXT layers read, so that no layout pass runs between them.  Exactly one of out and dst0 is non-NULL
+ * (anything else is GENRE_B200_EINVAL); without dst0 the layout and cpad arguments are ignored.  Operand outputs need fp16
+ * operands: f16 = 2: parts = 2, hi = fp16(a) | lo' = fp16((a - hi) * 2^11) (the fp32-accurate mode; bit-identical to
+ * genre_b200_blocked_split2_f16 of the fp32 output); f16 = 1: parts = 1, fp16(a).  With the output extent Do, Ho, Wo:
+ *   layout 1 (plain)   dst [B*Do][parts][cpad/8][Ho][Wo][8 fp16]
+ *   layout 2 (parity)  dst [B*Do/2][parts][8 s][cpad/8][Ho/2][Wo/2][8 fp16], s = ((z&1)*2 + (y&1))*2 + (x&1): the parity
+ *                      sub-volumes of a following conv3d_k4s2 (= genre_b200_ncdhw_to_blocked mode 2 with group 16)
+ * Channels from 4*cgo up to cpad (a multiple of 8, >= 4*cgo) are written as zeros on every call.
  * ------------------------------------------------------------------------------------------- */
 int genre_b200_convt3d_s2_forward(const void *src0, int cg0, const void *src1, int cg1,
                                   int64_t B, int64_t D, int64_t H, int64_t W,
                                   const void *wpack, int ksize, int npad, int f16,
                                   const float *scale, const float *shift, float slope,
-                                  float *out, int cgo, void *stream);
-
-/* Operand outputs.  The *_forward_operands variants of genre_b200_convt3d_s2_forward, genre_b200_convt3d_s2_merged_forward,
- * genre_b200_conv3d_k8s2_s4d_forward and genre_b200_conv3d_k4s2_forward take the same arguments with `out` replaced by up to
- * two destinations (dst1 may be NULL) of the fp16 operand the NEXT layers read, so that no layout pass runs between them.
- * f16 = 2: parts = 2, hi = fp16(a) | lo' = fp16((a - hi) * 2^11) (the fp32-accurate mode; bit-identical to
- * genre_b200_blocked_split2_f16 of the fp32 output); f16 = 1: parts = 1, fp16(a).  With the output extent Do, Ho, Wo:
- *   layout 1 (plain)   dst [B*Do][parts][cpad/8][Ho][Wo][8 fp16]
- *   layout 2 (parity)  dst [B*Do/2][parts][8 s][cpad/8][Ho/2][Wo/2][8 fp16], s = ((z&1)*2 + (y&1))*2 + (x&1): the parity
- *                      sub-volumes of a following conv3d_k4s2 (= genre_b200_ncdhw_to_blocked mode 2 with group 16)
- * Channels from 4*cgo up to cpad (a multiple of 8, >= 4*cgo) are written as zeros on every call. */
-int genre_b200_convt3d_s2_forward_operands(const void *src0, int cg0, const void *src1, int cg1,
-                                           int64_t B, int64_t D, int64_t H, int64_t W,
-                                           const void *wpack, int ksize, int npad, int f16,
-                                           const float *scale, const float *shift, float slope, int cgo,
-                                           void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
-                                           void *stream);
-int genre_b200_convt3d_s2_merged_forward_operands(const void *src0, int cg0, const void *src1, int cg1,
-                                                  int64_t B, int64_t D, int64_t H, int64_t W,
-                                                  const void *wpack, int ksize, int npad, int f16,
-                                                  const float *scale, const float *shift, float slope, int cgo,
-                                                  void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
-                                                  void *stream);
-int genre_b200_conv3d_k8s2_s4d_forward_operands(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
-                                                const void *wpack, int npad, int f16,
-                                                const float *scale, const float *shift, float slope, int cgo,
-                                                void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
-                                                void *stream);
-int genre_b200_conv3d_k4s2_forward_operands(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
-                                            const void *wpack, int npad, int f16,
-                                            const float *scale, const float *shift, float slope, int cgo,
-                                            void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
-                                            void *stream);
+                                  float *out, int cgo,
+                                  void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                  void *stream);
 
 /* Stride-1 convolution with `taps` (3 or 5) taps per dimension on channel-blocked activations, same wgmma kernel:
  *   out[b,z,y,x,n] = act(scale[n] * sum_{t,c} in[b, z+base-tz, y+base-ty, x+base-tx, c] * W[t][c][n] + shift[n])
@@ -244,7 +225,9 @@ int genre_b200_conv3d_taps_forward(const void *src0, int cg0, const void *src1, 
 int genre_b200_conv3d_k4s2_forward(const void *src, int cgs, int kblocks, int64_t B, int64_t D, int64_t H, int64_t W,
                                    const void *wpack, int npad, int f16,
                                    const float *scale, const float *shift, float slope,
-                                   float *out, int cgo, void *stream);
+                                   float *out, int cgo,
+                                   void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                   void *stream);
 
 /* The k 4 / s 2 / p 1 convolutions of the SMALL volumes (coarse side <= 8^3: Unet_3D.enc4, enc5, dec2, dec3,
  * networks/networks.py:157-165; the 4^3 / 8^3 stages of VoxelDecoder / VoxelGenerator / VoxelDiscriminator :40-57,:79-97,:247-256)
@@ -297,19 +280,21 @@ int genre_b200_convt_c1_forward(const float *src0, int cg0, const float *src1, i
 /* ConvTranspose3d(k 8, s 2, p 3), Cout <= 20, with the four (y,x) output parity classes merged along N (one N = 80 MMA
  * instead of four N = 20 MMAs): Unet_3D.dec5 = ConvT(80 -> 20) (networks/networks.py:166), 53.7 of the refiner's 78 GFLOP.
  * Operands as genre_b200_convt3d_s2_forward except scale, shift [20] and wpack, npad = 80 columns n = (py*2+px)*20 + co, in
- * one of two layouts:
- *   fp16 operands (f16 = 1, 2) and W in {16, 32}: PAIRED classes, 4x4 taps (coarse position j computes outputs 2j - 1 and
- *     2j per dimension, which read the same inputs): [2 z-parity][4][Cin chunk][16][2][npad/8][8][8]
+ * one of two layouts, chosen by `paired`:
+ *   paired = 1, valid only with fp16 operands (f16 = 1, 2) and W in {16, 32}: PAIRED classes, 4x4 taps (coarse position j
+ *     computes outputs 2j - 1 and 2j per dimension, which read the same inputs): [2 z-parity][4][Cin chunk][16][2][npad/8][8][8]
  *     (ops_conv.pack_convt_paired_weights);
- *   otherwise (fp32 operands f16 = 0, 3; other W): the 5x5 UNION of the classes' taps, zero weights where a class does not
- *     use a tap: [2 z-parity][4][Cin chunk][25][2][npad/8][8][g] (ops_conv.pack_convt_merged_weights).
- * Setting the environment variable GENRE_B200_CONVT_UNION (to anything but "0") makes every call take the union layout
- * (the two forms give bit-identical results; the paired one issues 28 % fewer MMAs at 32^2). */
+ *   paired = 0: the 5x5 UNION of the classes' taps, zero weights where a class does not use a tap:
+ *     [2 z-parity][4][Cin chunk][25][2][npad/8][8][g] (ops_conv.pack_convt_merged_weights).
+ * Any other `paired`, or paired = 1 outside its domain, is GENRE_B200_EINVAL.  The two forms give bit-identical results; the
+ * paired one issues 28 % fewer MMAs at 32^2. */
 int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *src1, int cg1,
                                          int64_t B, int64_t D, int64_t H, int64_t W,
-                                         const void *wpack, int ksize, int npad, int f16,
+                                         const void *wpack, int ksize, int npad, int f16, int paired,
                                          const float *scale, const float *shift, float slope,
-                                         float *out, int cgo, void *stream);
+                                         float *out, int cgo,
+                                         void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                         void *stream);
 
 /* Conv3d(k 8, s 2, p 3), Cout <= 20, as a 3-tap stride-1 convolution over the 4x space-to-depth input whose N = 160
  * columns are the 8 output classes of the 2x finer output grid: Unet_3D.enc1 = Conv3d(2 -> 20) on 128^3
@@ -318,7 +303,9 @@ int genre_b200_convt3d_s2_merged_forward(const void *src0, int cg0, const void *
 int genre_b200_conv3d_k8s2_s4d_forward(const void *src, int cg, int64_t B, int64_t D, int64_t H, int64_t W,
                                        const void *wpack, int npad, int f16,
                                        const float *scale, const float *shift, float slope,
-                                       float *out, int cgo, void *stream);
+                                       float *out, int cgo,
+                                       void *dst0, int layout0, int cpad0, void *dst1, int layout1, int cpad1,
+                                       void *stream);
 
 /* ConvTranspose3d(Cin -> 1, k 4, s 2, p 1) on the tensor cores: 3 union taps per dimension, the 8 output classes as
  * N columns, bias [1] (device) and optional sigmoid in the epilogue, NCDHW fp32 output [B][2D][2H][2W].  Same layers

@@ -62,21 +62,31 @@ def _d(v=4096):
     return ctypes.c_void_p(v)
 
 
+NO_DST = (None, 0, 0, None, 0, 0)   # no operand destinations: the fp32 `out` is written
+
+
 @pytest.mark.parametrize("call,code,needle", [
     # convolution entry points: shape support is part of the contract (include/genre_b200.h)
-    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 24, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5, None),
-     -1, b"width"),
-    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 3, None, 0, 1, 2, 16, 16, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5, None),
-     -1, b"even"),
-    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 6, 32, 1, _d(), _d(), 1.0, _d(), 5, None),
-     -1, b"kernel size"),
-    (lambda L: L.genre_b200_convt3d_s2_forward(_d(4100), 2, None, 0, 1, 2, 16, 16, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5, None),
-     -3, b"aligned"),
-    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 64, 1, _d(), _d(), 1.0, _d(), 5, None),
-     -1, b"npad"),
-    (lambda L: L.genre_b200_conv3d_k8s2_s4d_forward(_d(), 2, 1, 2, 16, 24, _d(), 160, 1, _d(), _d(), 1.0, _d(), 5, None),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 24, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5, *NO_DST,
+                                               None), -1, b"width"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 3, None, 0, 1, 2, 16, 16, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5, *NO_DST,
+                                               None), -1, b"even"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 6, 32, 1, _d(), _d(), 1.0, _d(), 5, *NO_DST,
+                                               None), -1, b"kernel size"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(4100), 2, None, 0, 1, 2, 16, 16, _d(), 8, 32, 1, _d(), _d(), 1.0, _d(), 5,
+                                               *NO_DST, None), -3, b"aligned"),
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 64, 1, 1, _d(), _d(), 1.0, _d(), 5,
+                                                      *NO_DST, None), -1, b"npad"),
+    # the paired form of the merged classes: fp16 operands at W in {16, 32} only, and `paired` is 0 or 1
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 80, 0, 1, _d(), _d(), 1.0, _d(), 5,
+                                                      *NO_DST, None), -1, b"paired"),
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 64, _d(), 8, 80, 1, 1, _d(), _d(), 1.0, _d(), 5,
+                                                      *NO_DST, None), -1, b"paired"),
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 32, _d(), 8, 80, 1, 2, _d(), _d(), 1.0, _d(), 5,
+                                                      *NO_DST, None), -1, b"paired"),
+    (lambda L: L.genre_b200_conv3d_k8s2_s4d_forward(_d(), 2, 1, 2, 16, 24, _d(), 160, 1, _d(), _d(), 1.0, _d(), 5, *NO_DST, None),
      -1, b"extent"),
-    (lambda L: L.genre_b200_conv3d_k4s2_forward(_d(), 3, 1, 1, 2, 16, 16, _d(), 64, 1, _d(), _d(), 1.0, _d(), 16, None),
+    (lambda L: L.genre_b200_conv3d_k4s2_forward(_d(), 3, 1, 1, 2, 16, 16, _d(), 64, 1, _d(), _d(), 1.0, _d(), 16, *NO_DST, None),
      -1, b"even"),
     (lambda L: L.genre_b200_convt_c1_tc_forward(_d(), 2, None, 0, 1, 2, 16, 48, _d(), 1, _d(), 0, _d(), None), -1, b"width"),
     (lambda L: L.genre_b200_convt_c1_forward(_d(), 2, None, 0, 1, 2, 16, 18, _d(), 0.0, 0, _d(), None), -1, b"extent"),
@@ -93,7 +103,7 @@ def _d(v=4096):
     # fused glue
     (lambda L: L.genre_b200_render_spherical_forward_pre(_d(), 1, 16, _d(), 8, 16, _d(), 50.0, 1.0, 0.0, _d(), None), -1, b"clamp"),
 ])
-def test_conv_and_layout_entry_points_validate_before_launching(call, code, needle):
+def test_entry_points_validate_before_launching(call, code, needle):
     """every unsupported shape / misaligned buffer is an argument error with a message, reported without touching a GPU"""
     lib = _lib.load()
     rc = call(lib)

@@ -127,11 +127,6 @@ def test_paired_pack_is_union_pack_without_zero_taps():
     assert bool((pc != 0).any(dim=-2).all())     # no all-zero (tap, column)
 
 
-def test_paired_form_follows_the_library_switch(monkeypatch):
-    monkeypatch.delenv(ops_conv.UNION_ENV, raising=False)
+def test_paired_form_domain():
     assert ops_conv._paired_classes(8, 32) and ops_conv._paired_classes(8, 16)
-    assert not ops_conv._paired_classes(4, 32) and not ops_conv._paired_classes(8, 64)
-    monkeypatch.setenv(ops_conv.UNION_ENV, "0")
-    assert ops_conv._paired_classes(8, 32)
-    monkeypatch.setenv(ops_conv.UNION_ENV, "1")
-    assert not ops_conv._paired_classes(8, 32)
+    assert not ops_conv._paired_classes(4, 32) and not ops_conv._paired_classes(4, 16) and not ops_conv._paired_classes(8, 64)

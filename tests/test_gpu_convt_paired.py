@@ -39,36 +39,37 @@ def nan_destinations(monkeypatch):
 
 
 def _run(blk, x, s, monkeypatch):
-    """(fp32 output, dec6's plain operand) through genre_b200_convt3d_s2_merged_forward[_operands]"""
+    """(fp32 output, dec6's plain operand) through genre_b200_convt3d_s2_merged_forward, without and with dst0"""
     calls = {}
     orig = _lib.call
 
     def call(name, *args):
-        calls[name] = calls.get(name, 0) + 1
+        key = (name, args[-7] is not None)       # dst0: the 7th argument from the end
+        calls[key] = calls.get(key, 0) + 1
         return orig(name, *args)
     with monkeypatch.context() as m:
         m.setattr(_lib, "call", call)
         y = blk(x, s)
         act = blk(x, s, [(ops_conv.PLAIN, 24)])
-    assert calls.get("genre_b200_convt3d_s2_merged_forward") == 1, calls
-    assert calls.get("genre_b200_convt3d_s2_merged_forward_operands") == 1, calls
+    assert calls.get(("genre_b200_convt3d_s2_merged_forward", False)) == 1, calls
+    assert calls.get(("genre_b200_convt3d_s2_merged_forward", True)) == 1, calls
     return y, act.operand(ops_conv.PLAIN, 24)[0]
 
 
 @pytest.mark.parametrize("mode", ["f16x2", "f16"])
 @pytest.mark.parametrize("b,d,n", [(2, 4, 32), (2, 2, 16)])
-def test_paired_classes_equal_the_union_walk(mode, b, d, n, nan_destinations, monkeypatch):
+def test_paired_argument_equals_the_union_walk(mode, b, d, n, nan_destinations, monkeypatch):
     blk = _dec5()
     g = torch.Generator(device=DEV).manual_seed(n + d)
     x = torch.randn(b, 40, d, n, n, device=DEV, generator=g)
     s = torch.randn(b, 40, d, n, n, device=DEV, generator=g)
     conv = blk._conv_bn()[0]
     with torch.no_grad(), ops_conv.precision(mode):
-        monkeypatch.delenv(ops_conv.UNION_ENV, raising=False)
         y_pair, op_pair = _run(blk, x, s, monkeypatch)
         assert any(k[0] == "convt_paired" for k in conv._gb_packed), "the paired form was not taken"
-        monkeypatch.setenv(ops_conv.UNION_ENV, "1")
-        y_union, op_union = _run(blk, x, s, monkeypatch)
+        with monkeypatch.context() as m:
+            m.setattr(ops_conv, "_paired_classes", lambda group, w: False)
+            y_union, op_union = _run(blk, x, s, monkeypatch)
         assert any(k[0] == "convt_merged" for k in conv._gb_packed), "the union form was not taken"
         torch.backends.cudnn.allow_tf32 = False
         try:

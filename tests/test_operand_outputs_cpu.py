@@ -113,18 +113,26 @@ def _d(v=4096):
 
 
 @pytest.mark.parametrize("call,code,needle", [
-    (lambda L: L.genre_b200_convt3d_s2_forward_operands(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 4, 32, 0, _d(), _d(), 1.0, 5,
-                                                        _d(), 1, 24, None, 0, 0, None), -1, b"fp16"),
-    (lambda L: L.genre_b200_convt3d_s2_forward_operands(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 4, 32, 2, _d(), _d(), 1.0, 5,
-                                                        None, 1, 24, None, 0, 0, None), -1, b"null"),
-    (lambda L: L.genre_b200_convt3d_s2_merged_forward_operands(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 80, 2, _d(), _d(), 1.0,
-                                                               5, _d(), 3, 24, None, 0, 0, None), -1, b"layout"),
-    (lambda L: L.genre_b200_conv3d_k8s2_s4d_forward_operands(_d(), 2, 1, 2, 16, 16, _d(), 80, 2, _d(), _d(), 1.0, 5,
-                                                             _d(), 2, 32, _d(), 1, 16, None), -1, b"cpad"),
-    (lambda L: L.genre_b200_conv3d_k4s2_forward_operands(_d(), 2, 1, 1, 2, 16, 16, _d(), 64, 2, _d(), _d(), 1.0, 10,
-                                                         _d(), 2, 48, _d(4104), 1, 40, None), -3, b"aligned"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 4, 32, 0, _d(), _d(), 1.0, None, 5,
+                                               _d(), 1, 24, None, 0, 0, None), -1, b"fp16"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 4, 32, 2, _d(), _d(), 1.0, None, 5,
+                                               None, 1, 24, None, 0, 0, None), -1, b"null"),
+    (lambda L: L.genre_b200_convt3d_s2_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 4, 32, 2, _d(), _d(), 1.0, _d(), 5,
+                                               _d(), 1, 24, None, 0, 0, None), -1, b"both"),
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 80, 2, 1, _d(), _d(), 1.0, None,
+                                                      5, _d(), 3, 24, None, 0, 0, None), -1, b"layout"),
+    (lambda L: L.genre_b200_convt3d_s2_merged_forward(_d(), 2, None, 0, 1, 2, 16, 16, _d(), 8, 80, 2, 1, _d(), _d(), 1.0, None,
+                                                      5, None, 0, 0, None, 0, 0, None), -1, b"first operand destination"),
+    (lambda L: L.genre_b200_conv3d_k8s2_s4d_forward(_d(), 2, 1, 2, 16, 16, _d(), 80, 2, _d(), _d(), 1.0, None, 5,
+                                                    _d(), 2, 32, _d(), 1, 16, None), -1, b"cpad"),
+    (lambda L: L.genre_b200_conv3d_k8s2_s4d_forward(_d(), 2, 1, 2, 16, 16, _d(), 80, 2, _d(), _d(), 1.0, _d(), 5,
+                                                    _d(), 2, 32, None, 0, 0, None), -1, b"both"),
+    (lambda L: L.genre_b200_conv3d_k4s2_forward(_d(), 2, 1, 1, 2, 16, 16, _d(), 64, 2, _d(), _d(), 1.0, None, 10,
+                                                _d(), 2, 48, _d(4104), 1, 40, None), -3, b"aligned"),
+    (lambda L: L.genre_b200_conv3d_k4s2_forward(_d(), 2, 1, 1, 2, 16, 16, _d(), 64, 2, _d(), _d(), 1.0, None, 10,
+                                                None, 0, 0, None, 0, 0, None), -1, b"first operand destination"),
 ])
-def test_operand_entry_points_validate_before_launching(call, code, needle):
+def test_operand_outputs_validate_before_launching(call, code, needle):
     from genre_shapehd_b200 import _lib
     lib = _lib.load()
     rc = call(lib)

@@ -21,7 +21,8 @@
 // all four run the epilogue (shared-memory accumulator image -> scale/shift/LeakyReLU -> blocked store).  Warps 4-11: two
 // consumer warpgroups, each issuing the m64 wgmma of one half (8 y-rows) of every M-tile and holding its MT x NACC / 2 fp32
 // accumulators in registers, so MT * NACC <= 256 (launch_convt_impl narrows the x tile until it fits).  After the last K
-// step they store the accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.
+// step they store the accumulators to shared memory (over the drained pipeline ring) for the epilogue warps.  MODE 5 in the
+// hi/lo split runs three consumer warpgroups (warps 4-15) on 192-position M-tiles (template parameter CW).
 // Pipeline: STAGES-deep ring of (halo chunk, weight chunk) with full/empty mbarriers; every consumer warp arrives on a slot's
 // empty barrier once its wgmma that read the slot have completed.  With 3 or more stages a stage's MMAs stay in flight while
 // the next stage is awaited and issued (wgmma.wait_group 1): its slot is released after the next stage's MMAs are committed.
@@ -32,8 +33,6 @@
 
 namespace gb {
 
-constexpr int CT_THREADS = 384;       // 4 producer/epilogue warps + 2 consumer warpgroups
-constexpr int CT_CONSUMER_WARPS = 8;
 constexpr int CT_ACC_COLS = 256;      // accumulator columns per CTA (MT * NACC): 128 fp32 registers per consumer thread
 constexpr int CT_BY = 16;             // y rows per CTA (16 core-matrix groups of 8 x positions = M 128)
 constexpr int CT_KCG = 2;             // channel groups (of 4) per stage = one K=8 TF32 MMA per tap and M-tile
@@ -60,6 +59,10 @@ struct ConvTParams {
   int olayout[2] = {0, 0};
   int ocg[2] = {0, 0};
   int oparts = 0;
+  // Unet_3D.enc1 in split-z MODE 2 over fp16 groups of 8 (conv3d_k8s2_s4d, npad 80): K chunk kc holds the 16 space-to-depth
+  // channels (c, rz) = (kc >> 2, kc & 3), and z tap tz of z class pz reads kernel tap 7 - 4 tz + rz - 2 pz, so the stages
+  // where that lies outside [0, 8) carry only zero weights and are skipped (a third of them)
+  int s4d_zskip = 0;
 };
 // operand output layouts (Do, Ho, Wo: the output extent)
 //   OP_PLAIN   [B*Do][oparts][ocg][Ho][Wo][8 fp16]: the blocked operand of a following ConvTranspose3d
@@ -106,12 +109,15 @@ __device__ __forceinline__ void store_operand(const ConvTParams &p, int k, int b
 // [1][1][PY][PX][16 B], out-of-bounds elements zero-filled = the convolution's padding); each channel group starts on a
 // 128-byte boundary of shared memory (the LBO of the A descriptor is that padded stride).
 // PW > 0: the paired form of MODE 5 over an input PW wide.  Its halo is flattened: rows of pitch PX = PW + 2 (input x from
-// -2, the two columns past the right edge of a row are the zero columns of the next), PY rows = enough for MT * 128
+// -2, the two columns past the right edge of a row are the zero columns of the next), PY rows = enough for MT * M
 // consecutive positions starting anywhere in a row plus the 3 rows and 3 columns the taps reach (see the kernel).
-template <int T, int NPAD, int MT, bool X2 = false, int PW = 0>
+// CW: consumer warpgroups, each issuing the m64 MMAs of 64 rows of every M-tile, so an M-tile is M = 64 * CW rows.  Only the
+// paired form takes CW = 3 (its positions are a flat run; the other modes' 128-row tiles are 16 y-rows x 8 x-columns).
+template <int T, int NPAD, int MT, bool X2 = false, int PW = 0, int CW = 2>
 struct ConvTCfg {
+  static constexpr int M = 64 * CW;
   static constexpr int W = 8 * MT;
-  static constexpr int PY = PW ? (128 * MT + (T + 1) * (PW + 2) + 1) / (PW + 2) : CT_BY + T - 1;   // halo extent
+  static constexpr int PY = PW ? (M * MT + (T + 1) * (PW + 2) + 1) / (PW + 2) : CT_BY + T - 1;   // halo extent
   static constexpr int PX = PW ? PW + 2 : W + T - 1;
   static constexpr int PARTS = X2 ? 2 : 1;
   static constexpr int NACC = PARTS * NPAD;                    // accumulator columns per M-tile = width of the B operand
@@ -126,7 +132,8 @@ struct ConvTCfg {
   // flight across stages (the kernel's INFLIGHT), but load each halo three times, and measured 5.40 ms per call against 4.97
   // (H100 80GB HBM3, 700 W).  Its paired form (MODE 5, X2: 16 taps, 97 KB per stage) takes all 4 tap rows in one stage,
   // a 2-stage ring that loads each halo once: 3.75 ms per call, against 4.25 ms for 2 + 2 rows in a 3-stage ring with MMAs
-  // in flight and every halo loaded twice (H100 80GB HBM3, 700 W, SM clock 1.92-1.98 GHz, B = 16).
+  // in flight and every halo loaded twice (H100 80GB HBM3, 700 W, SM clock 1.92-1.98 GHz, B = 16).  With CW = 3 (192
+  // positions, 10 halo rows at W = 32) a stage is 101 KB and the ring still holds 2.
   static constexpr int stage_bytes(int ys) { return ((A_BYTES + ((T + ys - 1) / ys) * T * B_TAP_BYTES + 127) / 128) * 128; }
   static constexpr int pick_ys() {
     for (int ys = 1; ys < T; ++ys)
@@ -140,9 +147,9 @@ struct ConvTCfg {
   static constexpr int STAGE_BYTES = stage_bytes(YS);
   // one CTA per SM (the accumulators take half the register file): the whole 227 KB of shared memory serves the ring
   static constexpr int STAGES = (218 * 1024) / STAGE_BYTES > 6 ? 6 : (218 * 1024) / STAGE_BYTES;
-  // epilogue image of the accumulators, [128 rows][MT * NPAD (+ 4 pad) columns] fp32, over the drained ring
+  // epilogue image of the accumulators, [M rows][MT * NPAD (+ 4 pad) columns] fp32, over the drained ring
   static constexpr int ACC_LD = MT * NPAD + 4;
-  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
+  static constexpr int ACC_BYTES = M * ACC_LD * 4;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
   static constexpr size_t SMEM = (size_t)RING_BYTES + 256;
   static_assert(STAGES >= 2, "stage too large");
@@ -150,6 +157,7 @@ struct ConvTCfg {
   static_assert(SMEM <= 227 * 1024, "shared memory");
   static_assert(NACC <= 256 && NACC % 16 == 0 && NPAD % 16 == 0 || !X2, "X2: MMA N must be a multiple of 16, at most 256");
   static_assert(PW == 0 || (T == 4 && PY <= 256 && PX <= 256), "paired form: 4 taps per dimension, tensor-copy box <= 256");
+  static_assert(CW == 2 || (CW == 3 && PW > 0), "three consumer warpgroups: the paired form only");
 };
 
 // MODE 0: 8 parity classes (blockIdx.y), output at 2*j + parity (ConvTranspose3d stride 2); TZ = T = K/2 taps
@@ -175,7 +183,7 @@ struct ConvTCfg {
 //         halo of pitch PX = W + 2 starting at input x = -2.  Tap (ty, tx) is the same shared-memory array shifted by
 //         ((3 - ty) * PX + 3 - tx) * 16 bytes; reads past a row's right edge land on the next row's two leading columns,
 //         which are input x = -2, -1: zeros, the padding they need.  The A operand's 8-row core groups are 8 consecutive
-//         positions (SBO = 128 B).  CTA = one (b, z parity, z plane, run of MT * 128 positions of the (H+1) x PX plane); the
+//         positions (SBO = 128 B).  CTA = one (b, z parity, z plane, run of MT * M positions of the (H+1) x PX plane); the
 //         epilogue drops x = W + 1 (the pitch's spare column), y > H and outputs -1 and 2H / 2W.  Per output the MMAs that
 //         carry non-zero weights come in MODE 2's order (z tap, K chunk, y tap, x tap), and MODE 2's others add exact
 //         zeros, so the two modes give bit-identical results.
@@ -186,11 +194,14 @@ struct ConvTCfg {
 //     second register set with round-to-nearest fp32 adds and restarts the MMA accumulator from 0; the two sets take the
 //     register budget of twice the columns (launch_convt_impl narrows the tile as for X2).
 // PW: the input width of MODE 5 (its halo pitch is compile-time), 0 otherwise.
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0>
-__global__ void __launch_bounds__(CT_THREADS, 1)
+// CW: consumer warpgroups (ConvTCfg).  MODE 5 in the hi/lo split runs CW = 3: M-tiles of 192 positions, so every stage's
+// weights (80 KB) serve 192 positions instead of 128.  The accumulators of one M-tile (80 registers per thread) leave room
+// for a third warpgroup within the 128 registers per thread of a 512-thread CTA.
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0, int CW = 2>
+__global__ void __launch_bounds__(128 + 128 * CW, 1)
 convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1) {
   constexpr bool F16 = OP == 1 || OP == 2, X2 = OP == 2, FLUSH = OP == 3;
-  using Cfg = ConvTCfg<T, NPAD, MT, X2, PW>;
+  using Cfg = ConvTCfg<T, NPAD, MT, X2, PW, CW>;
   constexpr int NACC = Cfg::NACC;
   static_assert(!FLUSH || 2 * MT * NACC <= CT_ACC_COLS, "two-level accumulators exceed the register budget");
   constexpr bool PAR = MODE == 0, MERGE = MODE == 2, MERGE8 = MODE == 3, C1 = MODE == 4, PAIR = MODE == 5;
@@ -202,7 +213,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   uint8_t *stages = smem;
   uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)Cfg::RING_BYTES);
   uint64_t *empty = full + Cfg::STAGES;
-  float *acc_img = reinterpret_cast<float *>(smem);   // after the main loop: [128 rows][ACC_LD]
+  float *acc_img = reinterpret_cast<float *>(smem);   // after the main loop: [M rows][ACC_LD]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int par = blockIdx.y;  // parity class: bit 2 = z, bit 1 = y, bit 0 = x
@@ -216,11 +227,12 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   const int y0 = yt * CT_BY, x0 = xt * Cfg::W;
   // MODE 5: the CTA's first position q0, the plane row yq0 it lies in and its offset in that row; halo row r holds input row
   // yq0 - 2 + r, so position q under tap (ty, tx) reads halo element q - yq0 * PX + (3 - ty) * PX + 3 - tx
-  const int q0 = xt * 128 * MT, yq0 = q0 / Cfg::PX, qoff = q0 - yq0 * Cfg::PX;
+  const int q0 = xt * Cfg::M * MT, yq0 = q0 / Cfg::PX, qoff = q0 - yq0 * Cfg::PX;
   const int nchunk = (p.cg0 + p.cg1) / CT_KCG;
 
   // (z tap, K chunk) enumeration shared by the producer and the MMA issuer: qq = tz * nchunk + kc, skipped when the z tap
-  // plane of that K chunk lies outside the input (it contributes nothing).  Each qq is YS stages, stage ys holding the
+  // plane of that K chunk lies outside the input (it contributes nothing), and with s4d_zskip when its weights are all zero
+  // (an MMA whose products are all zero leaves the accumulator's value as it is).  Each qq is YS stages, stage ys holding the
   // tap rows [ys * ROWS, min(T, ys * ROWS + ROWS)): an unrolled loop, so every stage's MMA sequence has a compile-time
   // shape (a runtime bound on the tap rows makes ptxas serialize every wgmma).  The per-dimension base offset of a chunk
   // is uniform (parity class / plain convolution) or a function of the chunk's source sub-volume (strided conv).
@@ -237,6 +249,10 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       by = MERGE ? T / 2 : p.base[py];
       bx = MERGE ? T / 2 : p.base[px];
     }
+    if (MERGE && p.s4d_zskip) {
+      const int kz = 7 - 4 * tz + (kc & 3) - 2 * pz;
+      if (kz < 0 || kz >= 8) return false;
+    }
     const int zi = zj + bz - tz;
     return zi >= 0 && zi < p.D;
   };
@@ -245,7 +261,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
   if (tid == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], 1);                    // the producer's expect_tx arrival (halo + weight bytes)
-      mbar_init(&empty[s], CT_CONSUMER_WARPS);   // every consumer warp
+      mbar_init(&empty[s], 4 * CW);              // every consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -328,10 +344,10 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
 #pragma unroll
             for (int mt = 0; mt < MT; ++mt) {
               // rows of this M-tile under tap (ty,tx): halo row (T-1-ty) + y, column (T-1-tx) + 8*mt + x; this warpgroup's
-              // 64 rows are y = 8 wg .. 8 wg + 7.  MODE 5: positions q0 + 128 mt + 64 wg + [0, 64), consecutive in the
+              // 64 rows are y = 8 wg .. 8 wg + 7.  MODE 5: positions q0 + M mt + 64 wg + [0, 64), consecutive in the
               // flattened halo, so an 8-row core group is 8 consecutive 16-byte positions
               constexpr uint32_t SBO = PAIR ? 128 : Cfg::PX * 16;
-              const uint32_t a0 = PAIR ? sa + (qoff + 128 * mt + 64 * wg + (T - 1 - ty) * Cfg::PX + (T - 1 - tx)) * 16
+              const uint32_t a0 = PAIR ? sa + (qoff + Cfg::M * mt + 64 * wg + (T - 1 - ty) * Cfg::PX + (T - 1 - tx)) * 16
                                        : sa + (((T - 1 - ty + 8 * wg) * Cfg::PX) + (T - 1 - tx) + 8 * mt) * 16;
               const uint64_t adesc = gmma_desc(a0, Cfg::A_CG_STRIDE, SBO);
               if constexpr (X2) {
@@ -375,7 +391,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     wgmma_wait<0>();
     if (held >= 0) release(held);
     // every stage has been consumed, so no copy can still land in the ring: it becomes the accumulator image
-    asm volatile("bar.sync 1, 256;" ::: "memory");   // ... by BOTH consumer warpgroups: the other one may still be reading it
+    asm volatile("bar.sync 1, %0;" ::"n"(128 * CW) : "memory");   // ... by EVERY consumer warpgroup: another may still read it
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
       if constexpr (FLUSH) store_acc_tile<NPAD, X2>(tot[mt], acc_img + (size_t)(64 * wg) * Cfg::ACC_LD + mt * NPAD, Cfg::ACC_LD);
@@ -383,9 +399,10 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
     }
   }
   __syncthreads();
-  if (warp < 4) {
+  if (tid < Cfg::M) {
     // ===================== epilogue: accumulator image -> act(acc*scale+shift) -> blocked global store ===============
-    const int m = warp * 32 + lane;  // accumulator row
+    // one accumulator row per thread: the 4 producer warps, joined by the first 2 consumer warps when CW = 3
+    const int m = tid;
     const float *arow = acc_img + (size_t)m * Cfg::ACC_LD;
     const int yy = m >> 3, xx = m & 7;
     constexpr bool UP = PAR || MERGE || MERGE8 || C1 || PAIR;
@@ -426,7 +443,7 @@ convt3d_s2_kernel(const ConvTParams p, const __grid_constant__ CUtensorMap tmap0
       const int oz = 2 * zj + pz;
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt) {
-        const int q = q0 + 128 * mt + m, y = q / Cfg::PX, x = q - y * Cfg::PX;
+        const int q = q0 + Cfg::M * mt + m, y = q / Cfg::PX, x = q - y * Cfg::PX;
         if (y > p.H || x > p.W) continue;     // past the plane, or the pitch's spare column x = W + 1
 #pragma unroll
         for (int qy = 0; qy < 2; ++qy) {
@@ -608,10 +625,10 @@ static bool make_halo_tmap(CUtensorMap *m, const void *base, long long planes, i
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0>
+template <int TZ, int T, int NPAD, int MT, int MODE, int OP, int PW = 0, int CW = 2>
 static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
-  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2, PW>;
-  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP, PW>;
+  using Cfg = ConvTCfg<T, NPAD, MT, OP == 2, PW, CW>;
+  auto kern = convt3d_s2_kernel<TZ, T, NPAD, MT, MODE, OP, PW, CW>;
   static bool configured[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -626,7 +643,7 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
   ConvTParams q = p;
   if constexpr (PW > 0) {
     if (p.W != PW) return fail_arg(GENRE_B200_EINVAL, "convt3d: the paired kernel for W=%d got W=%d", PW, p.W);
-    q.xtiles = ((p.H + 1) * Cfg::PX + 128 * MT - 1) / (128 * MT);   // runs of MT * 128 positions per (H+1) x PX plane
+    q.xtiles = ((p.H + 1) * Cfg::PX + Cfg::M * MT - 1) / (Cfg::M * MT);   // runs of MT * M positions per (H+1) x PX plane
   } else {
     q.xtiles = p.W / Cfg::W;
     if (q.xtiles < 1 || q.xtiles * Cfg::W != p.W) return fail_arg(GENRE_B200_EINVAL, "convt3d: W=%d is not a multiple of the %d-wide tile", p.W, Cfg::W);
@@ -643,7 +660,7 @@ static int launch_convt_variant(const ConvTParams &p, cudaStream_t st) {
   if (p.cg1 > 0 && !make_halo_tmap(&tm1, p.src1, planes, p.cg1, p.H, p.W, Cfg::PX, Cfg::PY))
     return fail_arg(GENRE_B200_EINVAL, "convt3d: cuTensorMapEncodeTiled failed for the second operand");
   dim3 grid((unsigned)(p.B * p.D * (PW ? 1 : p.H / CT_BY) * q.xtiles), MODE == 0 ? 8 : MODE == 2 || MODE == 5 ? 2 : 1);
-  kern<<<grid, CT_THREADS, Cfg::SMEM, st>>>(q, tm0, tm1);
+  kern<<<grid, 128 + 128 * CW, Cfg::SMEM, st>>>(q, tm0, tm1);
   return check_launch("convt3d_s2 kernel");
 }
 
@@ -686,11 +703,11 @@ template <int TZ, int T, int NPAD, int MT>
 static int launch_convt_merged(const ConvTParams &p, int op, cudaStream_t st) {
   return launch_convt_op<TZ, T, NPAD, MT, 2>(p, op, st);
 }
-// MODE 5, the fp16 operand modes: three M-tiles per CTA in fp16 (240 accumulator columns), one in the hi/lo split (X2
-// narrows it), N = 80
+// MODE 5, the fp16 operand modes, N = 80: three M-tiles of 128 positions per CTA in fp16 (240 accumulator columns); in the
+// hi/lo split (160 columns) one M-tile of 192 positions on three consumer warpgroups
 template <int PW>
 static int launch_convt_paired(const ConvTParams &p, int op, cudaStream_t st) {
-  return op == 2 ? launch_convt_impl<4, 4, 80, 3, 5, 2, PW>(p, st) : launch_convt_impl<4, 4, 80, 3, 5, 1, PW>(p, st);
+  return op == 2 ? launch_convt_variant<4, 4, 80, 1, 5, 2, PW, 3>(p, st) : launch_convt_impl<4, 4, 80, 3, 5, 1, PW>(p, st);
 }
 // the operand destinations dst0, layout0, cpad0, dst1, layout1, cpad1 of an entry point
 struct OperandOut {
@@ -852,8 +869,12 @@ extern "C" int genre_b200_conv3d_k8s2_s4d_forward(const void *src, int cg, int64
   GB_REQUIRE(B * D * (H / CT_BY) * (W / 16) < (1ll << 31), GENRE_B200_EINVAL, "conv3d_k8s2_s4d: grid too large");
   p.base[0] = p.base[1] = 1;  // input cell = j + 1 - t
   // npad 80: the z class moves to blockIdx.y (MODE 2 with 3 z taps per class; wpack [2 qz][3][chunk][9][2][10][8][g]):
-  // twice the MMAs of the 8-class form, but half the accumulator columns and weight bytes per stage
-  if (npad == 80) return launch_convt_merged<3, 3, 80, 2>(p, f16, as_stream(stream));
+  // twice the MMAs of the 8-class form, but half the accumulator columns and weight bytes per stage.  In the fp16 operand
+  // modes (groups of 8 channels: K chunk = (c, rz)) the z class's all-zero (z tap, K chunk) stages are skipped
+  if (npad == 80) {
+    p.s4d_zskip = f16 == 1 || f16 == 2;
+    return launch_convt_merged<3, 3, 80, 2>(p, f16, as_stream(stream));
+  }
   return launch_conv_merged8<3, 160, 2>(p, f16, as_stream(stream));
 }
 

@@ -43,6 +43,9 @@ kappa per kernel family and mode (units of 2^-24 A, see kappa_* below):
                                        z taps x K chunks (8 channels of the tripled lo | hi | hi K range) x YS, with YS
                                        taken at its upper bound T (every tap row a stage of its own)
 
+Sigmoid outputs (VoxelGenerator's last layer) are held to sigmoid_bound: the logits' rule carried over at 1/4 (sigmoid
+is 1/4-Lipschitz) plus the epilogue's own exp, add and division.
+
 Probes.  Activations and weights in [0.25, 4], each an fp16 value plus a same-signed residual of 0.25-0.45 fp16 ulp: every
 lo' is positive, so a dropped lo part, cross term or cross accumulator moves EVERY output by 2^-13 .. 2^-10 of its A, i.e.
 2^11 .. 2^14 units, where random-sign data averages it out.  fp16 and TF32 have the same 10-bit mantissa, so the same
@@ -116,6 +119,17 @@ def steps_s4d(cin):
 def steps_flat(cin_total, transposed):
     k = cin_total if transposed else 8 * cin_total
     return (-(-k // 16)) * 8
+
+
+def steps_s2d(cin):
+    """Conv3d(cin -> n, k4 s2 p1) as 3 taps over the 2x space-to-depth input (conv3d_taps_forward, the critic's first
+    layer): 3 z taps x the 8 cin channels in chunks of 16 (zero-padded) x 3 x 3 taps"""
+    return 3 * (-(-8 * cin // 16)) * 9
+
+
+def steps_c1_tc(cin_total):
+    """MODE 4 (the 1-channel ConvTranspose3d on the tensor cores): 3 z taps x chunks x the 3 x 3 union (y, x) taps"""
+    return 3 * (-(-cin_total // 16)) * 9
 
 
 def stages_x3(tz, cin_k, t):
@@ -199,6 +213,27 @@ def rule_ratio(got, ref, A, Fl, kappa):
     if Fl is None or not bool((Fl > 0).any()):
         return err_ratio(got, ref, A)
     return err_ratio(got, ref, A + C_FLOOR * Fl / (kappa * U))
+
+
+def sigmoid_bound(y, L):
+    """bound on |got - sigmoid(y)| for got = fp32(1 / fp32(1 + __expf(-v))) of logits v within L of the fp64 logits y.
+    sigmoid is 1/4-Lipschitz: 1/4 L.  With e = exp(-v), d sigmoid / d e = -sigmoid (1 - sigmoid) / e, so a relative error
+    r of e moves the result by sigmoid (1 - sigmoid) r.  __expf is within 2 + floor(1.173 |v|) ulp (CUDA Programming
+    Guide; an ulp is at most 2^-23 of the value): 2^-23 sigmoid (1 - sigmoid) (2 + 1.173 |v|), written with 3 and 1.2 to
+    cover |v| - |y| and the second-order terms.  The rounding of 1 + e and the IEEE division (the library is built without
+    fast math) are 2^-24 of the result each: 2^-23 sigmoid.  Below fp32's normal range the result is 0 or subnormal
+    (exp(-v) overflows to inf from v < -88.7, where sigmoid < 2^-126): an absolute 2^-126.  torch's fp32 sigmoid (the
+    f16x2 path) is within the same."""
+    s = torch.sigmoid(y)
+    return 0.25 * L + 2.0 ** -23 * s * (1 - s) * (3 + 1.2 * y.abs()) + 2.0 ** -23 * s + 2.0 ** -126
+
+
+def sigmoid_ratio(got, y, A, Fl, kappa):
+    """rule_ratio's scale for a sigmoid of the layer's logits y (fp64): <= kappa iff |got - sigmoid(y)| <=
+    sigmoid_bound(y, kappa 2^-24 A + c F)"""
+    L = kappa * U * A + (0.0 if Fl is None else C_FLOOR * Fl)
+    d = (got.double() - torch.sigmoid(y)).abs()
+    return kappa * (d / sigmoid_bound(y, L)).max().item()
 
 
 # ---- operand emulation ---------------------------------------------------------------------------------------------
@@ -299,6 +334,43 @@ def skinny_chunk_drop_ref(x, conv, bn, slope, chunk, transposed):
     flat = x.view(b, -1)
     flat[:, chunk * L:(chunk + 1) * L] = 0
     return layer_ref64([x], conv, bn, slope)
+
+
+def x_tile_ref(srcs, conv, bn, slope, tile):
+    """every tile of `tile` output columns computed from the input columns of its own window only (a CTA whose halo lost
+    its x margin): the window is the tile's columns scaled by the input / output width ratio, the rest read as zeros"""
+    ref = layer_ref64(srcs, conv, bn, slope)
+    wo, wi = ref.shape[-1], srcs[0].shape[-1]
+    out = torch.empty_like(ref)
+    for x0 in range(0, wo, tile):
+        a, b = x0 * wi // wo, (x0 + tile) * wi // wo
+        cut = [s.detach().clone() for s in srcs]
+        for s in cut:
+            s[..., :a] = 0
+            s[..., b:] = 0
+        out[..., x0:x0 + tile] = layer_ref64(cut, conv, bn, slope)[..., x0:x0 + tile]
+    return out
+
+
+def dup_n_tile(w, dim=0, n=64):
+    """output channels [n, 2n) of a weight tensor (dim 0 for Conv3d, 1 for ConvTranspose3d) replaced by [0, n)"""
+    w = w.detach().clone()
+    w.narrow(dim, n, n).copy_(w.narrow(dim, 0, n))
+    return w
+
+
+def n_tile_ref(srcs, conv, bn, slope, n=64):
+    """the second N tile of `n` columns reading the first tile's weights"""
+    dim = 1 if isinstance(conv, torch.nn.ConvTranspose3d) else 0
+    return layer_ref64(srcs, conv, bn, slope, w=dup_n_tile(conv.weight, dim, n))
+
+
+def odd_x_dropped_ref(srcs, conv, bn, slope):
+    """the odd input columns lost (a space-to-depth operand whose x parity bit is dropped)"""
+    cut = [s.detach().clone() for s in srcs]
+    for s in cut:
+        s[..., 1::2] = 0
+    return layer_ref64(cut, conv, bn, slope)
 
 
 def col2im_seam_ref(srcs, conv, band=1, rows=2):

@@ -105,9 +105,10 @@ class Layer:
     """one layer of a net run on its own: run(srcs) through the nets' module path, its conv / bn / slope, the source
     shapes, the entry point it must take, its kernel family and the per-mode kappa"""
 
-    def __init__(self, kind, run, conv, bn, slope, shapes, entry, family, kappa, x3_stages=None, straddle=False):
+    def __init__(self, kind, run, conv, bn, slope, shapes, entry, family, kappa, x3_stages=None, straddle=False, controls=None):
         self.kind, self.run, self.conv, self.bn, self.slope, self.shapes = kind, run, conv, bn, slope, shapes
         self.entry, self.family, self.kappa, self.x3_stages, self.straddle = entry, family, kappa, x3_stages, straddle
+        self.controls = controls      # (srcs, mode) -> [(name, fp64 result)]: the layer's own negative controls
 
 
 def _tc(steps):
@@ -208,6 +209,8 @@ def _controls(L, srcs, mode, rnd):
         out.append(("last K chunk dropped", R.skinny_chunk_drop_ref(x, conv, bn, slope, last_chunk, transposed)))
     if L.family == "col2im":
         out.append(("band seam contribution dropped", R.col2im_seam_ref(srcs, conv)))
+    if L.controls is not None:
+        out += L.controls(srcs, mode)
     return out
 
 
@@ -230,7 +233,7 @@ def _check(tag, L, mode, monkeypatch):
         assert ops_conv._mode() == mode
         for data in ("random", "probe"):
             if data == "random":
-                srcs = [R.scaled_random(s, R.batch_scales(B), g, DEV) for s in L.shapes]
+                srcs = [R.scaled_random(s, R.batch_scales(s[0]), g, DEV) for s in L.shapes]
                 ctx = contextlib.nullcontext()
             else:
                 srcs = [R.probe(s, g, DEV) for s in L.shapes]
@@ -273,7 +276,10 @@ def test_voxel_decoder_layer_b16_vs_fp64(index, mode, monkeypatch):
 
 
 # ---- whole nets ------------------------------------------------------------------------------------------------------
-def _three_ways(net, x, monkeypatch):
+def _three_ways(net, x, monkeypatch, factor=None, scale=None):
+    """the net on this package, on torch fp32 and on an fp64 copy.  factor: the package / torch fp32 error bound (FACTOR);
+    scale: per-sample magnitudes the 1e-4 bound is relative to (default max|ref64|, overall and per sample)"""
+    factor = FACTOR if factor is None else factor
     with torch.no_grad():
         with _calls(monkeypatch) as n:
             y = net(x)
@@ -287,14 +293,18 @@ def _three_ways(net, x, monkeypatch):
         del net64
     ep = (y.double() - y64).abs()
     et = (y32.double() - y64).abs()
-    mx = y64.abs().max().item()
-    rel, rel32 = ep.max().item() / mx, et.max().item() / mx
-    per = [(ep[b].max() / y64[b].abs().max().clamp_min(1e-300)).item() for b in range(x.shape[0])]
+    if scale is None:
+        mx = y64.abs().max().item()
+        rel, rel32 = ep.max().item() / mx, et.max().item() / mx
+        per = [(ep[b].max() / y64[b].abs().max().clamp_min(1e-300)).item() for b in range(x.shape[0])]
+    else:
+        per = [(ep[b].max() / scale[b]).item() for b in range(x.shape[0])]
+        rel, rel32 = max(per), max((et[b].max() / scale[b]).item() for b in range(x.shape[0]))
     ratio = ep.max().item() / max(et.max().item(), 1e-300)
     print("[fp64] whole %s B=%d: package max rel %.3g (worst sample %.3g), torch fp32 %.3g, package / torch fp32 = %.3g "
-          "(factor %g); entry points %s" % (type(net).__name__, x.shape[0], rel, max(per), rel32, ratio, FACTOR, sorted(n.items())))
+          "(factor %g); entry points %s" % (type(net).__name__, x.shape[0], rel, max(per), rel32, ratio, factor, sorted(n.items())))
     assert rel <= 1e-4 and max(per) <= 1e-4, (rel, per)
-    assert ep.max().item() <= FACTOR * et.max().item(), ratio
+    assert ep.max().item() <= factor * et.max().item(), ratio
     return n
 
 

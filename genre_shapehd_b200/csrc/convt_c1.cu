@@ -16,8 +16,8 @@ constexpr int C1_TX = 16, C1_TY = 8, C1_TZ = 2;       // threads; each handles 4
 constexpr int C1_CELLS = 4;
 
 __global__ void __launch_bounds__(C1_TX *C1_TY *C1_TZ)
-convt_c1_kernel(const float4 *__restrict__ src0, int cg0, const float4 *__restrict__ src1, int cg1, int D, int H, int W,
-                const float *__restrict__ weight /* [Cin][64] */, float bias, int act_sigmoid,
+convt_c1_kernel(const float4 *__restrict__ src0, int cg0, const float4 *__restrict__ src1, int cg1, int BD, int D, int H,
+                int W, const float *__restrict__ weight /* [Cin][64] */, float bias, int act_sigmoid,
                 float *__restrict__ out /* [B][2D][2H][2W] */) {
   extern __shared__ float4 s_w[];  // [cg][64 taps] float4 over the 4 channels of the group
   const int ncg = cg0 + cg1;
@@ -31,7 +31,7 @@ convt_c1_kernel(const float4 *__restrict__ src0, int cg0, const float4 *__restri
   const int y = blockIdx.y * C1_TY + threadIdx.y;
   const int zb = blockIdx.z * C1_TZ + threadIdx.z;  // b * D + z
   const int b = zb / D, z = zb - b * D;
-  if (x0 >= W || y >= H || b < 0) return;
+  if (x0 >= W || y >= H || zb >= BD) return;  // the last z block is partial when B * D is odd
 
   float acc[C1_CELLS][8];
 #pragma unroll
@@ -131,6 +131,7 @@ extern "C" int genre_b200_convt_c1_forward(const float *src0, int cg0, const flo
             (unsigned)((B * D + C1_TZ - 1) / C1_TZ));
   GB_REQUIRE(grid.z <= 65535 && grid.y <= 65535, GENRE_B200_EINVAL, "convt_c1: grid too large");
   convt_c1_kernel<<<grid, block, (size_t)(cg0 + cg1) * 64 * sizeof(float4), as_stream(stream)>>>(
-      (const float4 *)src0, cg0, (const float4 *)src1, cg1, (int)D, (int)H, (int)W, weight, bias, act_sigmoid, out);
+      (const float4 *)src0, cg0, (const float4 *)src1, cg1, (int)(B * D), (int)D, (int)H, (int)W, weight, bias, act_sigmoid,
+      out);
   return check_launch("convt_c1 kernel");
 }

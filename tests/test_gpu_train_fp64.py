@@ -357,6 +357,27 @@ def test_convt_c1_gradients_through_autograd_vs_fp64(case):
     _check_c1("c1 %s %s" % (case, shape), x.detach(), m.weight.detach(), gx, gw, gy, n_slabs)
 
 
+@pytest.mark.parametrize("B,D", [(3, 1), (1, 5)])
+def test_convt_c1_forward_stays_inside_its_tensors_when_b_times_d_is_odd(B, D):
+    """The forward's CTAs cover 2 of the B * D input planes each, so for odd B * D the last CTA's second plane does not
+    exist.  Its threads used to read one sample past the input and write one (2H, 2W) plane pair past the output (the
+    h8_d1_w12 and slabs_2sm_plus_1 shapes above).  Here both tensors carry a spare sample, so such accesses stay inside
+    the allocations: the output's spare sample must keep its NaN sentinel, and the output must be the convolution."""
+    C, H, W = 24, 8, 12
+    cg, per_in, per_out = C // 4, D * C * H * W, 8 * D * H * W
+    torch.manual_seed(B + D)
+    src = torch.randn((B + 1) * per_in, device=DEV)                      # blocked [B*D][cg][H][W][4] + a spare sample
+    w = torch.randn(C, 1, 4, 4, 4, device=DEV)
+    out = torch.full(((B + 1) * per_out,), float("nan"), device=DEV)
+    _lib.call("genre_b200_convt_c1_forward", src.data_ptr(), cg, None, 0, B, D, H, W, w.data_ptr(), 0.25, 0,
+              out.data_ptr(), _lib.stream_ptr(out))
+    torch.cuda.synchronize()
+    assert torch.isnan(out[B * per_out:]).all(), "the forward wrote past its output"
+    x = src[:B * per_in].view(B, D, cg, H, W, 4).permute(0, 2, 5, 1, 3, 4).reshape(B, C, D, H, W)
+    ref = F.conv_transpose3d(x.double(), w.double(), stride=2, padding=1) + 0.25
+    assert (out[:B * per_out].view(ref.shape).double() - ref).abs().max().item() < 1e-4
+
+
 @pytest.mark.parametrize("kind,cin,shape", [("wgrad", 37, (2, 3, 16, 20)), ("wgrad", 52, (2, 3, 16, 20)), ("wgrad", 64, (1, 4, 8, 24)),
                                             ("dgrad", 64, (2, 3, 16, 20)), ("dgrad", 192, (1, 2, 8, 12))])
 def test_convt_c1_gradients_through_the_abi_vs_fp64(kind, cin, shape):

@@ -1,0 +1,333 @@
+// render_cam.cu — camera-view renderer of voxel occupancy grids and the differentiable ray-consistency loss, forward +
+// backward.
+//
+// The camera is cam_bp's (cam_bp.cu cam_unproject): at o = (-cam_dist, 0, 0), looking along +x, focal length fl in
+// pixels, so pixel (h, w) casts the ray o + t u with u = (fl, -imw, -imh) / |(fl, imw, imh)|, imh = h - (H-1)/2,
+// imw = w - (W-1)/2, and t is cam_bp's ray depth.  Samples t_k = cam_dist - sqrt(3)/2 + k sqrt(3)/(Z-1) cover the unit
+// cube for every ray.  Voxel (i, j, l) of vox[n] sits at cam_bp's voxel centre ((i+0.5)/R - 0.5, ...), so the trilinear
+// coordinate of a point g is f = (g + 0.5) R - 0.5 (zero padding).  The stop-probability model is render_spherical's:
+//     p_k = clamp(raw_k, 1e-5, 1 - 1e-5),   T_k = prod_{j<k} (1 - p_j),   s_k = p_k T_k,
+// and a ray's value is an expected cost  V = sum_k s_k c_k + T_Z c_esc:
+//     render           c_k = t_k, c_esc = bg (depth);  silhou = 1 - T_Z
+//     ray consistency  obs > 0: c_k = |t_k - obs|, c_esc = miss;   obs <= 0: c_k = miss, c_esc = 0
+// d V / d p_k = T_k c_k - (sum_{j>k} s_j c_j + T_Z c_esc) / (1 - p_k), zero where the clamp is active, scattered through
+// the tap weights.  The backward of the renderer is the same walk with the cost g_depth t_k + g_silhou, escape g_depth bg
+// (d silhou / d p_k is the expected cost of c_k = 1, c_esc = 0).
+//
+// Layout (as render_sph.cu): one warp per ray, lanes take 32 consecutive samples, the transmittance crosses lanes with a
+// shuffle product-scan and crosses 32-sample chunks through a register carry; only [N,H,W] maps are written.  The
+// backward walks each ray twice: forward, keeping each chunk's carry in shared memory (one float per chunk), then
+// backward over the chunks, recomputing the samples, so the suffix sum is a running sum of the chunks already walked and
+// T_k is the forward's value bit for bit.
+//
+// Sample coordinates (the arithmetic is part of the op's definition; tests/render_cam_ref.py restates it): in fp64, each
+// operation rounded to nearest in this order (explicit intrinsics: never contracted),
+//     nrm = sqrt((fl*fl + imw*imw) + imh*imh);  u = (fl / nrm, -imw / nrm, -imh / nrm)
+//     t   = (cam_dist - sqrt(3)/2) + k * (sqrt(3) / (Z - 1))          (k * 0 for Z = 1)
+//     g   = (t*ux - cam_dist, t*uy, t*uz);   f = (g + 0.5) * R - 0.5
+// then f and t are each rounded once to fp32.  fl and cam_dist are the fp32 inputs widened exactly.  Everything after is
+// fp32.
+#include "render.cuh"
+
+namespace gb {
+
+constexpr int RC_THREADS = 256;  // 8 rays per CTA
+constexpr int RC_WARPS = RC_THREADS / 32;
+constexpr int RC_MAX_Z = 4096;
+constexpr int RC_MAX_CHUNKS = RC_MAX_Z / 32;
+constexpr int RC_MAX_RES = 1024;
+constexpr int RC_MAX_HW = 16384;
+constexpr double RC_SQRT3 = 1.7320508075688772;       // the double nearest sqrt(3)
+constexpr double RC_HALF_SQRT3 = 0.8660254037844386;  // RC_SQRT3 / 2 (exact)
+
+enum { RC_RENDER = 0, RC_CONSISTENCY = 1 };
+
+struct CamRay {
+  double ux, uy, uz, cd, t0, dt;
+};
+
+__device__ __forceinline__ CamRay cam_ray(float fl, float cam_dist, int h, int w, int H, int W, int Z) {
+  const double f = (double)fl;
+  const double imh = (double)h - 0.5 * (double)(H - 1), imw = (double)w - 0.5 * (double)(W - 1);  // exact
+  const double nrm = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(f, f), __dmul_rn(imw, imw)), __dmul_rn(imh, imh)));
+  CamRay r;
+  r.ux = __ddiv_rn(f, nrm);
+  r.uy = __ddiv_rn(-imw, nrm);
+  r.uz = __ddiv_rn(-imh, nrm);
+  r.cd = (double)cam_dist;
+  r.t0 = __dadd_rn(r.cd, -RC_HALF_SQRT3);
+  r.dt = Z > 1 ? __ddiv_rn(RC_SQRT3, (double)(Z - 1)) : 0.0;
+  return r;
+}
+
+// sample k of the ray: taps at its fp32 voxel coordinate, and its fp32 ray depth
+__device__ __forceinline__ float cam_sample(const CamRay &r, int k, int R, Taps &taps) {
+  const double Rd = (double)R;
+  const double t = __dadd_rn(r.t0, __dmul_rn((double)k, r.dt));
+  const double gx = __dadd_rn(__dmul_rn(t, r.ux), -r.cd), gy = __dmul_rn(t, r.uy), gz = __dmul_rn(t, r.uz);
+  const float fx = (float)__dadd_rn(__dmul_rn(__dadd_rn(gx, 0.5), Rd), -0.5);
+  const float fy = (float)__dadd_rn(__dmul_rn(__dadd_rn(gy, 0.5), Rd), -0.5);
+  const float fz = (float)__dadd_rn(__dmul_rn(__dadd_rn(gz, 0.5), Rd), -0.5);
+  make_taps_at(fx, fy, fz, R, taps);
+  return (float)t;
+}
+
+// cost c_k = a t_k + b, escape e: the renderer's depth (a = 1, b = 0, e = bg) and its backward's weighted sum of the
+// depth and silhouette gradients
+struct LinearCost {
+  float a, b, e;
+  __device__ __forceinline__ float at(float t) const { return fmaf(a, t, b); }
+  __device__ __forceinline__ float esc() const { return e; }
+};
+
+// differentiable ray consistency against an observed ray depth (<= 0: background)
+struct RayCost {
+  float obs, miss;
+  __device__ __forceinline__ float at(float t) const { return obs > 0.0f ? fabsf(t - obs) : miss; }
+  __device__ __forceinline__ float esc() const { return obs > 0.0f ? miss : 0.0f; }
+};
+
+// The forward walk: returns (sum_k s_k c_k, T_Z) to every lane.  With chunk_T, chunk c's carry (T before its first
+// sample) is stored there and *last_chunk is the last chunk walked; the walk stops once T underflows to 0 (every later
+// term, and every later gradient, is exactly 0).
+template <class Cost>
+__device__ __forceinline__ void cam_walk(const float *__restrict__ vol, int R, const CamRay &ray, int Z, const Cost &cost,
+                                         float &sum, float &trans, float *chunk_T, int *last_chunk) {
+  const int lane = threadIdx.x & 31;
+  float carry = 1.0f, acc = 0.0f;
+  for (int c = 0; c * 32 < Z; ++c) {
+    const int k = c * 32 + lane;
+    float p = 0.0f, ck = 0.0f;  // lanes past the end behave like p = 0 (factor 1, no contribution)
+    if (k < Z) {
+      Taps t;
+      ck = cost.at(cam_sample(ray, k, R, t));
+      p = fminf(fmaxf(sample_trilinear<false>(vol, t, R, VoxPre{}), RS_PMIN), RS_PMAX);
+    }
+    if (chunk_T) {
+      if (lane == 0) chunk_T[c] = carry;
+      *last_chunk = c;
+    }
+    float total;
+    const float before = carry * warp_excl_prod32(1.0f - p, total);
+    if (k < Z) acc = fmaf(p * before, ck, acc);
+    carry *= total;
+    if (carry == 0.0f) break;  // warp-uniform
+  }
+  sum = warp_sum(acc);
+  trans = carry;
+}
+
+struct CamArgs {
+  const float *vox;
+  int R, H, W, Z;
+  long long n_rays;
+  const float *fl, *cd;
+  long long fN, dN;
+  float bg;                  // render: escape depth
+  const float *obs;          // consistency: observed ray depth [N,H,W], strides (oN, oH, oW)
+  long long oN, oH, oW;
+  float miss;
+  const float *g0, *g1;      // backward: grad_depth, grad_silhou (render) or grad_loss (consistency), [N,H,W] dense
+  float *out0, *out1;        // forward: depth, silhou (render) or loss (consistency), [N,H,W] dense
+  float *grad_vox;           // backward: [N,R,R,R] dense, accumulated
+};
+
+struct RayIndex {
+  long long n;
+  int h, w;
+};
+
+__device__ __forceinline__ RayIndex ray_index(const CamArgs &a, long long ray) {
+  const long long hw = (long long)a.H * a.W;
+  RayIndex ri;
+  ri.n = ray / hw;
+  const int pix = (int)(ray - ri.n * hw);
+  ri.h = pix / a.W;
+  ri.w = pix - ri.h * a.W;
+  return ri;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(RC_THREADS) render_camera_forward_kernel(const CamArgs a) {
+  const long long ray = (long long)blockIdx.x * RC_WARPS + (threadIdx.x >> 5);
+  if (ray >= a.n_rays) return;
+  const RayIndex ri = ray_index(a, ray);
+  const float *vol = a.vox + (size_t)ri.n * a.R * a.R * a.R;
+  const CamRay r = cam_ray(a.fl[ri.n * a.fN], a.cd[ri.n * a.dN], ri.h, ri.w, a.H, a.W, a.Z);
+  float sum, T;
+  if (MODE == RC_RENDER) {
+    const LinearCost cost{1.0f, 0.0f, a.bg};
+    cam_walk(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
+    if ((threadIdx.x & 31) == 0) {
+      a.out0[ray] = fmaf(T, cost.esc(), sum);
+      a.out1[ray] = 1.0f - T;
+    }
+  } else {
+    const RayCost cost{a.obs[ri.n * a.oN + ri.h * a.oH + ri.w * a.oW], a.miss};
+    cam_walk(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
+    if ((threadIdx.x & 31) == 0) a.out0[ray] = fmaf(T, cost.esc(), sum);
+  }
+}
+
+// the two walks of one ray; `scale` multiplies every gradient (the consistency loss's upstream gradient)
+template <class Cost>
+__device__ __forceinline__ void cam_backward_ray(const float *__restrict__ vol, float *__restrict__ gvol, int R,
+                                                 const CamRay &ray, int Z, const Cost &cost, float scale, float *chunk_T) {
+  const int lane = threadIdx.x & 31;
+  float sum, T_Z;
+  int last = 0;
+  cam_walk(vol, R, ray, Z, cost, sum, T_Z, chunk_T, &last);
+  __syncwarp();
+  float suffix = T_Z * cost.esc();  // sum over the chunks already walked of s_j c_j, plus the escape term
+  for (int c = last; c >= 0; --c) {
+    const int k = c * 32 + lane;
+    const bool live = k < Z;
+    float raw = 0.0f, p = 0.0f, ck = 0.0f;
+    Taps t;
+    if (live) {
+      ck = cost.at(cam_sample(ray, k, R, t));
+      raw = sample_trilinear<false>(vol, t, R, VoxPre{});
+      p = fminf(fmaxf(raw, RS_PMIN), RS_PMAX);
+    }
+    float total;
+    const float Tk = chunk_T[c] * warp_excl_prod32(1.0f - p, total);  // the forward's T_k, bit for bit
+    float chunk_sum;
+    const float Ak = suffix + warp_excl_suffix_sum32(live ? p * Tk * ck : 0.0f, chunk_sum);
+    suffix += chunk_sum;
+    if (live && raw >= RS_PMIN && raw <= RS_PMAX) {  // NaN and clamped samples pass no gradient
+      const float dp = scale * (Tk * ck - Ak / (1.0f - p));
+      if (dp != 0.0f) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (t.valid & (1u << i)) atomicAdd(gvol + t.base + tap_offset(i, R), dp * t.w[i]);
+      }
+    }
+  }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(RC_THREADS) render_camera_backward_kernel(const CamArgs a) {
+  __shared__ float s_T[RC_WARPS][RC_MAX_CHUNKS];
+  const int warp = threadIdx.x >> 5;
+  const long long ray = (long long)blockIdx.x * RC_WARPS + warp;
+  if (ray >= a.n_rays) return;
+  const RayIndex ri = ray_index(a, ray);
+  const size_t vol_off = (size_t)ri.n * a.R * a.R * a.R;
+  const float g0 = a.g0[ray], g1 = MODE == RC_RENDER ? a.g1[ray] : 0.0f;
+  if (g0 == 0.0f && g1 == 0.0f) return;  // warp-uniform
+  const CamRay r = cam_ray(a.fl[ri.n * a.fN], a.cd[ri.n * a.dN], ri.h, ri.w, a.H, a.W, a.Z);
+  if (MODE == RC_RENDER)
+    cam_backward_ray(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z, LinearCost{g0, g1, g0 * a.bg}, 1.0f, s_T[warp]);
+  else
+    cam_backward_ray(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z,
+                     RayCost{a.obs[ri.n * a.oN + ri.h * a.oH + ri.w * a.oW], a.miss}, g0, s_T[warp]);
+}
+
+static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+static int rc_check(const char *what, const float *vox, int64_t N, int res, int64_t H, int64_t W, int Z, const float *fl,
+                    const float *cd, CamArgs &a) {
+  GB_REQUIRE(vox && fl && cd, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(res >= 2 && res <= RC_MAX_RES, GENRE_B200_EINVAL, "%s: resolution %d unsupported (2..%d)", what, res,
+             RC_MAX_RES);
+  GB_REQUIRE(H >= 1 && W >= 1 && H <= RC_MAX_HW && W <= RC_MAX_HW, GENRE_B200_EINVAL,
+             "%s: image size %lld x %lld unsupported (1..%d per side)", what, (long long)H, (long long)W, RC_MAX_HW);
+  GB_REQUIRE(Z >= 1 && Z <= RC_MAX_Z, GENRE_B200_EINVAL, "%s: z_res %d unsupported (1..%d)", what, Z, RC_MAX_Z);
+  GB_REQUIRE(N >= 1 && (N * H * W + RC_WARPS - 1) / RC_WARPS < (1ll << 31), GENRE_B200_EINVAL,
+             "%s: batch %lld unsupported (1 .. 2^34 / (H W) rays)", what, (long long)N);
+  GB_REQUIRE(aligned4(vox) && aligned4(fl) && aligned4(cd), GENRE_B200_EALIGN, "%s: vox, fl and camdist must be 4-byte aligned",
+             what);
+  a = CamArgs{};
+  a.vox = vox;
+  a.R = res;
+  a.H = (int)H;
+  a.W = (int)W;
+  a.Z = Z;
+  a.n_rays = (long long)N * H * W;
+  a.fl = fl;
+  a.cd = cd;
+  return 0;
+}
+
+static unsigned rc_grid(const CamArgs &a) { return (unsigned)((a.n_rays + RC_WARPS - 1) / RC_WARPS); }
+
+}  // namespace gb
+
+using namespace gb;
+
+extern "C" int genre_b200_render_camera_forward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                                const float *fl, int64_t fN, const float *camdist, int64_t dN, float bg,
+                                                float *depth, float *silhou, void *stream) {
+  CamArgs a;
+  if (int rc = rc_check("render_camera", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  GB_REQUIRE(depth && silhou, GENRE_B200_EINVAL, "render_camera: null output");
+  GB_REQUIRE(aligned4(depth) && aligned4(silhou), GENRE_B200_EALIGN, "render_camera: outputs must be 4-byte aligned");
+  a.fN = fN;
+  a.dN = dN;
+  a.bg = bg;
+  a.out0 = depth;
+  a.out1 = silhou;
+  render_camera_forward_kernel<RC_RENDER><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("render_camera forward kernel");
+}
+
+extern "C" int genre_b200_render_camera_backward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                                 const float *fl, int64_t fN, const float *camdist, int64_t dN, float bg,
+                                                 const float *grad_depth, const float *grad_silhou, float *grad_vox,
+                                                 void *stream) {
+  CamArgs a;
+  if (int rc = rc_check("render_camera backward", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  GB_REQUIRE(grad_depth && grad_silhou && grad_vox, GENRE_B200_EINVAL, "render_camera backward: null pointer");
+  GB_REQUIRE(aligned4(grad_depth) && aligned4(grad_silhou) && aligned4(grad_vox), GENRE_B200_EALIGN,
+             "render_camera backward: gradients must be 4-byte aligned");
+  a.fN = fN;
+  a.dN = dN;
+  a.bg = bg;
+  a.g0 = grad_depth;
+  a.g1 = grad_silhou;
+  a.grad_vox = grad_vox;
+  render_camera_backward_kernel<RC_RENDER><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("render_camera backward kernel");
+}
+
+extern "C" int genre_b200_ray_consistency_forward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                                  const float *fl, int64_t fN, const float *camdist, int64_t dN,
+                                                  const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
+                                                  float *loss, void *stream) {
+  CamArgs a;
+  if (int rc = rc_check("ray_consistency", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  GB_REQUIRE(obs && loss, GENRE_B200_EINVAL, "ray_consistency: null pointer");
+  GB_REQUIRE(aligned4(obs) && aligned4(loss), GENRE_B200_EALIGN, "ray_consistency: obs and loss must be 4-byte aligned");
+  a.fN = fN;
+  a.dN = dN;
+  a.obs = obs;
+  a.oN = oN;
+  a.oH = oH;
+  a.oW = oW;
+  a.miss = miss_cost;
+  a.out0 = loss;
+  render_camera_forward_kernel<RC_CONSISTENCY><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("ray_consistency forward kernel");
+}
+
+extern "C" int genre_b200_ray_consistency_backward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                                   const float *fl, int64_t fN, const float *camdist, int64_t dN,
+                                                   const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
+                                                   const float *grad_loss, float *grad_vox, void *stream) {
+  CamArgs a;
+  if (int rc = rc_check("ray_consistency backward", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  GB_REQUIRE(obs && grad_loss && grad_vox, GENRE_B200_EINVAL, "ray_consistency backward: null pointer");
+  GB_REQUIRE(aligned4(obs) && aligned4(grad_loss) && aligned4(grad_vox), GENRE_B200_EALIGN,
+             "ray_consistency backward: obs and gradients must be 4-byte aligned");
+  a.fN = fN;
+  a.dN = dN;
+  a.obs = obs;
+  a.oN = oN;
+  a.oH = oH;
+  a.oW = oW;
+  a.miss = miss_cost;
+  a.g0 = grad_loss;
+  a.grad_vox = grad_vox;
+  render_camera_backward_kernel<RC_CONSISTENCY><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("ray_consistency backward kernel");
+}

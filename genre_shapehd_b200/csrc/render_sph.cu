@@ -14,76 +14,20 @@
 // is written.  Sample positions are formed in fp64 from the fp64 direction table exactly like the
 // numpy code, then rounded to fp32, so they equal the reference's registered `grid` buffer.
 #include <cstdlib>
-#include "common.cuh"
+#include "render.cuh"
 
 namespace gb {
 
 constexpr int RS_THREADS = 256;  // 8 rays per CTA
 
-struct Taps {
-  int base;        // linear index of corner (x0, y0, z0); may be out of range, see masks
-  float w[8];      // weights in order (x,y,z) = 000, 001, 010, 011, 100, 101, 110, 111
-  unsigned valid;  // bit i set if tap i is inside the volume
-};
-
+// grid-space position (align_corners=True semantics) -> taps
 __device__ __forceinline__ void make_taps(float gx, float gy, float gz, int R, Taps &t) {
   const float Rm1 = (float)(R - 1);
   // grid_sampler unnormalise, align_corners=True: ((coord + 1) / 2) * (size - 1)
   const float fx = __fmul_rn(__fmul_rn(__fadd_rn(gx, 1.0f), 0.5f), Rm1);
   const float fy = __fmul_rn(__fmul_rn(__fadd_rn(gy, 1.0f), 0.5f), Rm1);
   const float fz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.0f), 0.5f), Rm1);
-  const float x0f = floorf(fx), y0f = floorf(fy), z0f = floorf(fz);
-  // clamp before the int conversion so far-away samples (|coord| up to 2) stay well defined
-  const int x0 = (int)fminf(fmaxf(x0f, -2.0f), (float)R), y0 = (int)fminf(fmaxf(y0f, -2.0f), (float)R),
-            z0 = (int)fminf(fmaxf(z0f, -2.0f), (float)R);
-  const float wx1 = fx - x0f, wx0 = (x0f + 1.0f) - fx;
-  const float wy1 = fy - y0f, wy0 = (y0f + 1.0f) - fy;
-  const float wz1 = fz - z0f, wz0 = (z0f + 1.0f) - fz;
-  t.base = (x0 * R + y0) * R + z0;
-  t.w[0] = wx0 * wy0 * wz0; t.w[1] = wx0 * wy0 * wz1; t.w[2] = wx0 * wy1 * wz0; t.w[3] = wx0 * wy1 * wz1;
-  t.w[4] = wx1 * wy0 * wz0; t.w[5] = wx1 * wy0 * wz1; t.w[6] = wx1 * wy1 * wz0; t.w[7] = wx1 * wy1 * wz1;
-  const unsigned Rm = (unsigned)(R - 1);
-  if (((unsigned)x0 < Rm) & ((unsigned)y0 < Rm) & ((unsigned)z0 < Rm)) {  // all 8 taps inside: the common case
-    t.valid = 0xFFu;
-    return;
-  }
-  const bool vx0 = (unsigned)x0 < (unsigned)R, vx1 = (unsigned)(x0 + 1) < (unsigned)R;
-  const bool vy0 = (unsigned)y0 < (unsigned)R, vy1 = (unsigned)(y0 + 1) < (unsigned)R;
-  const bool vz0 = (unsigned)z0 < (unsigned)R, vz1 = (unsigned)(z0 + 1) < (unsigned)R;
-  t.valid = (unsigned)(vx0 & vy0 & vz0) | ((unsigned)(vx0 & vy0 & vz1) << 1) | ((unsigned)(vx0 & vy1 & vz0) << 2) |
-            ((unsigned)(vx0 & vy1 & vz1) << 3) | ((unsigned)(vx1 & vy0 & vz0) << 4) |
-            ((unsigned)(vx1 & vy0 & vz1) << 5) | ((unsigned)(vx1 & vy1 & vz0) << 6) |
-            ((unsigned)(vx1 & vy1 & vz1) << 7);
-}
-
-__device__ __forceinline__ int tap_offset(int i, int R) {
-  return ((i >> 2) & 1) * R * R + ((i >> 1) & 1) * R + (i & 1);
-}
-
-// Optional transform of every voxel value as it is fetched: v -> clamp(v * scale, lo, hi).  GenRe renders
-// clamp(proj * 50, 1e-5, 1 - 1e-5) (depth_pred_with_sph_inpaint.py:124): applying the two elementwise ops here (same
-// fp32 operations, same order) removes two dense passes over the volume.  Out-of-volume taps stay 0 (zero padding).
-struct VoxPre {
-  float scale, lo, hi;
-};
-template <bool PRE>
-__device__ __forceinline__ float fetch_vox(const float *__restrict__ p, const VoxPre &pre) {
-  const float v = __ldg(p);
-  return PRE ? fminf(fmaxf(__fmul_rn(v, pre.scale), pre.lo), pre.hi) : v;
-}
-
-template <bool PRE>
-__device__ __forceinline__ float sample_trilinear(const float *__restrict__ vol, const Taps &t, int R, const VoxPre &pre) {
-  float acc = 0.0f;
-  if (t.valid == 0xFFu) {  // interior: 4 pairs of z-adjacent taps
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc = fmaf(fetch_vox<PRE>(vol + t.base + tap_offset(i, R), pre), t.w[i], acc);
-  } else if (t.valid) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      if (t.valid & (1u << i)) acc = fmaf(fetch_vox<PRE>(vol + t.base + tap_offset(i, R), pre), t.w[i], acc);
-  }
-  return acc;
+  make_taps_at(fx, fy, fz, R, t);
 }
 
 // sample position k on the ray with fp64 direction (dx,dy,dz): (float)(dir*2*(1-alpha_k)), alpha = np.linspace(0,1,Z)
@@ -95,28 +39,6 @@ __device__ __forceinline__ void ray_point(double dx2, double dy2, double dz2, in
   gy = (float)(dy2 * f);
   gz = (float)(dz2 * f);
 }
-
-__device__ __forceinline__ float warp_excl_prod32(float v, float &total) {
-  float incl = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const float u = __shfl_up_sync(0xffffffffu, incl, d);
-    if ((threadIdx.x & 31) >= d) incl *= u;
-  }
-  total = __shfl_sync(0xffffffffu, incl, 31);
-  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-  if ((threadIdx.x & 31) == 0) excl = 1.0f;
-  return excl;
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-constexpr float RS_PMIN = 1e-5f;
-constexpr float RS_PMAX = (float)(1.0 - 1e-5);
 
 // forward pass over one ray; returns (sum_k s_k w_k, prod_k (1 - p_k)) to every lane
 template <bool PRE>
@@ -516,17 +438,9 @@ render_spherical_backward_kernel(const float *__restrict__ vox, int R, const dou
     const float p = live ? fminf(fmaxf(raw[c], RS_PMIN), RS_PMAX) : 0.0f;
     const float wk = live ? __ldg(depth_weight + k) : 0.0f;
     const float ws = wk * p * Tk[c];
-    // exclusive suffix sum over lanes
-    float incl = ws;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const float u = __shfl_down_sync(0xffffffffu, incl, d);
-      if (lane + d < 32) incl += u;
-    }
-    float excl = __shfl_down_sync(0xffffffffu, incl, 1);
-    if (lane == 31) excl = 0.0f;
-    const float Ak = suffix + excl;
-    suffix += __shfl_sync(0xffffffffu, incl, 0);
+    float chunk_sum;
+    const float Ak = suffix + warp_excl_suffix_sum32(ws, chunk_sum);
+    suffix += chunk_sum;
     if (live && raw[c] >= RS_PMIN && raw[c] <= RS_PMAX) {
       const float dp = g * (Tk[c] * wk - (Ak + t_all) / (1.0f - p));
       if (dp != 0.0f) {

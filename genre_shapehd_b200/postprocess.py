@@ -21,6 +21,8 @@ points drawn from their surfaces (the metric of the reference's nndistance op), 
 Pix3D ship their shapes as meshes) to grids: conservative voxelisation on the device, and the same metrics against
 ground-truth meshes.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -896,3 +898,125 @@ def pack_meshes(meshes, device):
         raise ValueError("pack_meshes: %d faces, fewer than 2^31 expected" % fo[-1])
     return (torch.from_numpy(np.concatenate(vs)).to(device), torch.from_numpy(np.concatenate(fs)).to(device),
             torch.from_numpy(vo).to(device), torch.from_numpy(fo).to(device))
+
+
+# ---- the input camera's view of a grid: rendered depth and silhouette, and the ray-consistency loss ---------------------
+# Camera_back_projection_layer's defaults: GenRe's 256^2 depth maps are back-projected with these
+CAM_FL = 418.3
+CAM_DIST = 2.2
+
+
+def default_z_res(res):
+    """samples per ray at grid resolution ``res``: ceil(2 sqrt(3) res) + 1, spacing at most half a voxel over the sqrt(3)
+    of ray the unit cube can hold"""
+    return int(math.ceil(2.0 * math.sqrt(3.0) * res)) + 1
+
+
+def _cam_param(x, n, name, dev):
+    """a float, [N] or [N,1] -> (fp32 tensor, element stride over the batch)"""
+    if not isinstance(x, torch.Tensor):
+        return torch.full((1,), float(x), dtype=torch.float32, device=dev), 0
+    _lib.require_cuda(x)
+    _lib.require_f32(x)
+    if x.dim() == 2 and x.shape[1] == 1:
+        x = x[:, 0]
+    if x.dim() != 1 or x.shape[0] not in (1, n):
+        raise ValueError("%s: a float, [N] or [N,1] expected with N = %d, got %s" % (name, n, tuple(x.shape)))
+    return x, (x.stride(0) if x.shape[0] == n else 0)
+
+
+def _cam_args(vox, fl, cam_dist, z_res, name):
+    """the leading arguments of the camera renderer's entry points, and the tensors they point into"""
+    v = _volumes(vox, name)
+    n, r = v.shape[0], v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]):
+        raise ValueError("%s expects cubic volumes, got %s" % (name, tuple(vox.shape)))
+    z = default_z_res(r) if z_res is None else int(z_res)
+    f, fs = _cam_param(fl, n, name + " fl", v.device)
+    d, ds = _cam_param(cam_dist, n, name + " cam_dist", v.device)
+    return v, (f, d), (n, r, z, f.data_ptr(), fs, d.data_ptr(), ds)
+
+
+class _RenderCamera(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, vox, v, keep, head, H, W, bg):
+        n = head[0]
+        depth = torch.empty((n, 1, H, W), dtype=torch.float32, device=v.device)
+        silhou = torch.empty_like(depth)
+        args = (v.data_ptr(), n, head[1], H, W) + head[2:]
+        _lib.call("genre_b200_render_camera_forward", *args, bg, depth.data_ptr(), silhou.data_ptr(), _lib.stream_ptr(v))
+        ctx.save_for_backward(v, *keep)
+        ctx.args, ctx.bg, ctx.vox_shape = args, bg, vox.shape
+        return depth, silhou
+
+    @staticmethod
+    def backward(ctx, grad_depth, grad_silhou):
+        v = ctx.saved_tensors[0]
+        shape = (v.shape[0],) + tuple(ctx.args[3:5])
+        gd = torch.zeros(shape, device=v.device) if grad_depth is None else grad_depth.reshape(shape).contiguous()
+        gs = torch.zeros(shape, device=v.device) if grad_silhou is None else grad_silhou.reshape(shape).contiguous()
+        grad = torch.zeros_like(v)
+        _lib.call("genre_b200_render_camera_backward", *ctx.args, ctx.bg, gd.data_ptr(), gs.data_ptr(), grad.data_ptr(),
+                  _lib.stream_ptr(v))
+        return grad.view(ctx.vox_shape), None, None, None, None, None, None
+
+
+def render_depth(vox, fl=CAM_FL, cam_dist=CAM_DIST, size=(256, 256), z_res=None, bg=0.0):
+    """Render occupancy grids into the input camera, differentiably in ``vox``.
+
+    vox [N,1,R,R,R] (or [N,R,R,R]) fp32 occupancy probabilities on CUDA (pass ``torch.sigmoid(logits)``), in cam_bp's frame:
+    voxel (i, j, l) at ((i+0.5)/R - 0.5, (j+0.5)/R - 0.5, (l+0.5)/R - 0.5), the camera at (-cam_dist, 0, 0) looking along +x
+    with focal length ``fl`` pixels (a float, [N] or [N,1]; defaults of ``Camera_back_projection_layer``).  Pixel (h, w) of
+    the ``size`` = (H, W) map casts the ray on which cam_bp places that pixel's points, sampled ``z_res`` times (default
+    ``default_z_res(R)``) over the unit cube; the stop probabilities are ``render_spherical``'s, clamp(v, 1e-5, 1 - 1e-5).
+    Returns (depth, silhou), each [N,1,H,W]: the expected ray depth (``bg`` where the ray escapes) and 1 - the escape
+    probability.  ``depth`` is a ray depth like cam_bp's input, not a z-depth.
+
+    Frames: GenRe's ``Net.forward`` ``pred_voxel`` (and ``fused.genre_forward_fused``'s) is already in this frame (the
+    refiner is trained on transpose(0,2,1) + flip(2) of the ground truth, genre_full_model.py:90-92); MarrNet-2's ``voxel``
+    ground truth needs that same transform, and ``forward_with_trimesh``'s output the inverse of genre_full_model.py:231."""
+    v, keep, head = _cam_args(vox, fl, cam_dist, z_res, "render_depth")
+    H, W = (int(size), int(size)) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    return _RenderCamera.apply(vox, v, keep, head, H, W, float(bg))
+
+
+class _RayConsistency(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, vox, v, keep, head, obs, miss_cost):
+        n, (H, W) = head[0], obs.shape[-2:]
+        loss = torch.empty((n, 1, H, W), dtype=torch.float32, device=v.device)
+        args = (v.data_ptr(), n, head[1], H, W) + head[2:] + (obs.data_ptr(), obs.stride(0), obs.stride(-2),
+                                                              obs.stride(-1), miss_cost)
+        _lib.call("genre_b200_ray_consistency_forward", *args, loss.data_ptr(), _lib.stream_ptr(v))
+        ctx.save_for_backward(v, obs, *keep)
+        ctx.args, ctx.vox_shape = args, vox.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        v = ctx.saved_tensors[0]
+        g = grad_loss.reshape(v.shape[0], *ctx.args[3:5]).contiguous()
+        grad = torch.zeros_like(v)
+        _lib.call("genre_b200_ray_consistency_backward", *ctx.args, g.data_ptr(), grad.data_ptr(), _lib.stream_ptr(v))
+        return grad.view(ctx.vox_shape), None, None, None, None, None
+
+
+def ray_consistency_loss(vox, obs_depth, fl=CAM_FL, cam_dist=CAM_DIST, z_res=None, miss_cost=1.0, reduction="mean"):
+    """Differentiable ray consistency (Tulsiani et al., CVPR 2017) of occupancy grids with observed depth maps: the
+    reprojection loss that trains a 3D prediction against the 2.5D sketch it came from, without 3D labels.
+
+    vox, fl, cam_dist, z_res as ``render_depth``; obs_depth [N,1,H,W] or [N,H,W] fp32 ray depth in cam_bp's convention (any
+    strides; <= 0 marks background, as GenRe's ``get_abs_depth`` writes 0 there).  Per ray, the expected cost of where it
+    stops: on a foreground ray a stop at depth t costs |t - obs| and escaping costs ``miss_cost``; on a background ray every
+    stop costs ``miss_cost`` and escaping is free.  Returns the per-sample mean over rays [N] (``reduction='mean'``) or the
+    per-ray loss [N,1,H,W] (``'none'``).  Differentiable in ``vox`` only."""
+    v, keep, head = _cam_args(vox, fl, cam_dist, z_res, "ray_consistency_loss")
+    _lib.require_cuda(obs_depth)
+    _lib.require_f32(obs_depth)
+    obs = obs_depth[:, 0] if obs_depth.dim() == 4 and obs_depth.shape[1] == 1 else obs_depth
+    if obs.dim() != 3 or obs.shape[0] != head[0]:
+        raise ValueError("ray_consistency_loss: obs_depth [%d,1,H,W] expected, got %s" % (head[0], tuple(obs_depth.shape)))
+    if reduction not in ("mean", "none"):
+        raise ValueError("ray_consistency_loss: reduction 'mean' or 'none', got %r" % (reduction,))
+    loss = _RayConsistency.apply(vox, v, keep, head, obs, float(miss_cost))
+    return loss.mean((1, 2, 3)) if reduction == "mean" else loss

@@ -143,6 +143,59 @@ int genre_b200_render_spherical_backward(const float *vox, int64_t N, int res,
                                          const float *grad_out, float *grad_vox, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Camera-view renderer of voxel grids and the differentiable ray-consistency loss (no reference
+ * counterpart: the reference's util/util_reproj.py attempt is not called by any model).
+ *
+ * The camera is cam_bp's: at (-cam_dist, 0, 0) looking along +x, focal length fl in pixels.  Pixel
+ * (h, w) of an H x W map casts the ray o + t u, u = (fl, -imw, -imh) / |(fl, imw, imh)|,
+ * imh = h - (H-1)/2, imw = w - (W-1)/2, so the point genre_b200_cam_bp_forward places from pixel
+ * (h, w) at ray depth d lies on this ray at t = d.  Z samples t_k = cam_dist - sqrt(3)/2 +
+ * k sqrt(3)/(Z-1) (t_0 only for Z = 1) cover the unit cube for every ray.  Voxel (i, j, l) of vox[n]
+ * sits at cam_bp's voxel centre ((i+0.5)/R - 0.5, (j+0.5)/R - 0.5, (l+0.5)/R - 0.5): a point g is
+ * sampled trilinearly at voxel coordinate f = (g + 0.5) R - 0.5 with zero padding (not
+ * render_spherical's align_corners mapping: this op inverts cam_bp).  Then, as render_spherical,
+ *   p_k = clamp(raw_k, 1e-5, 1 - 1e-5),  T_k = prod_{j<k} (1 - p_j),  s_k = p_k T_k,
+ * and a ray's value is the expected cost  sum_k s_k c_k + T_Z c_esc.
+ *
+ * Arithmetic of the sample coordinate: fp64, every operation rounded to nearest, in the order
+ *   nrm = sqrt((fl*fl + imw*imw) + imh*imh);  u = (fl/nrm, -imw/nrm, -imh/nrm)
+ *   t = (cam_dist - sqrt(3)/2) + k * (sqrt(3)/(Z-1));  g = (t*ux - cam_dist, t*uy, t*uz)
+ *   f = (g + 0.5) * R - 0.5
+ * (fl, cam_dist widened exactly from fp32; sqrt(3) the nearest double), then f and t are each
+ * rounded once to fp32.  Everything after the coordinate is fp32.
+ *
+ *   vox  [N, R, R, R] dense (C = 1), 2 <= R <= 1024;  fl, camdist [N] with strides fN, dN (0: shared)
+ *   1 <= H, W <= 16384;  1 <= z_res <= 4096;  every pointer 4-byte aligned (else GENRE_B200_EALIGN)
+ *   outputs and upstream gradients [N, H, W] dense; grad_vox [N,R,R,R] dense, zeroed by the caller
+ *   (accumulated with fp32 atomics: not bitwise repeatable, and a contribution or sum below 2^-126
+ *   is flushed to zero).  The forwards are bitwise repeatable and
+ *   each ray's value does not depend on the batch.  No allocation, no synchronisation.
+ * The gradient w.r.t. p_k is T_k c_k - (sum_{j>k} s_j c_j + T_Z c_esc) / (1 - p_k), zero where the
+ * clamp is active (and at NaN samples, which render as p = 1e-5), scattered through the tap weights.
+ * ------------------------------------------------------------------------------------------- */
+/* depth = sum_k s_k t_k + T_Z bg,  silhou = 1 - T_Z */
+int genre_b200_render_camera_forward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                     const float *fl, int64_t fN, const float *camdist, int64_t dN, float bg,
+                                     float *depth, float *silhou, void *stream);
+int genre_b200_render_camera_backward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                      const float *fl, int64_t fN, const float *camdist, int64_t dN, float bg,
+                                      const float *grad_depth, const float *grad_silhou, float *grad_vox,
+                                      void *stream);
+/* Differentiable ray consistency (Tulsiani et al., CVPR 2017) against an observed ray-depth map
+ * obs [N, H, W] with any strides (oN, oH, oW): per ray the expected cost with
+ *   obs > 0 (foreground):  c_k = |t_k - obs|, c_esc = miss_cost
+ *   obs <= 0 (background): c_k = miss_cost,   c_esc = 0     (GenRe's get_abs_depth writes 0 there)
+ * loss [N, H, W]; the backward takes the per-ray upstream gradient grad_loss [N, H, W]. */
+int genre_b200_ray_consistency_forward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                       const float *fl, int64_t fN, const float *camdist, int64_t dN,
+                                       const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
+                                       float *loss, void *stream);
+int genre_b200_ray_consistency_backward(const float *vox, int64_t N, int res, int64_t H, int64_t W, int z_res,
+                                        const float *fl, int64_t fN, const float *camdist, int64_t dN,
+                                        const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
+                                        const float *grad_loss, float *grad_vox, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Chamfer nearest-neighbour distance.  Replaces nnd_forward_cuda / nnd_backward_cuda
  * (toolbox/nndistance/src/my_lib_cuda.h:1-4, nnd_cuda.cu:6-177; functions/nnd.py:8-63).
  *   xyz1 [B,N,3], xyz2 [B,M,3] dense;  dist1 [B,N], dist2 [B,M] squared distances;

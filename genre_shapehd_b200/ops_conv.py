@@ -1486,9 +1486,14 @@ def convt_c1_tc(inputs, m, sigmoid=False):
     return out
 
 
+# K steps (16 channels of the concatenated, group-padded sources) whose weights csrc/convt_c1_col2im.cu keeps resident in
+# shared memory next to a 2-stage ring: 40 in the hi/lo split (4 KB of weights per step), 85 with fp16 operands (2 KB)
+C2I_MAX_KSTEPS = {"f16x2": 40, "f16": 85}
+
+
 def _convt_c1_col2im_supported(inputs, m):
     x0 = inputs[0]
-    return ("convt_c1_col2im" in POLICY and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
+    return ("convt_c1_col2im" in POLICY and sum(-(-t.shape[1] // 8) * 8 for t in inputs) <= 16 * C2I_MAX_KSTEPS.get(_mode(), 0) and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
             and tuple(m.padding) == (1, 1, 1) and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1)
             and m.groups == 1 and m.out_channels == 1 and len(inputs) <= 2
             and all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 5 and t.shape[2:] == x0.shape[2:] for t in inputs)

@@ -39,6 +39,10 @@ kappa per kernel family and mode (units of 2^-24 A, see kappa_* below):
                                        K-chunk partials; NN: a 128-term fma chain + the chunk partials; + the epilogue
   convt_c1_col2im:                     representation + 3 per K step + 1 (hi + cross) + 7 col2im adds + the bias + one
                                        red.global.add at band seams
+  tf32 (single pass, fp32 operands):   2^15 + 16 of representation (2^-10 per operand, whether the tensor core rounds or
+                                       truncates to TF32, and 2^-20 for their product), no floor (delta = 0), no cross
+                                       term; a K step is 8 channels (2 groups of 4): twice the MMA steps of the fp16 counts
+  convt_c1 (FP32 stencil):             one fma chain of 8 Cin products per output (1 unit per fma) + the bias add
   fp32x3:                              test_gpu_train_fp64._kappa_x3 over the stages of one output + the epilogue; stages =
                                        z taps x K chunks (8 channels of the tripled lo | hi | hi K range) x YS, with YS
                                        taken at its upper bound T (every tap row a stage of its own)
@@ -64,11 +68,14 @@ import torch.nn.functional as F
 
 from train_ref import U, err_ratio, plain_torch, tf32_round  # noqa: F401  (re-exported for the tests)
 
-DELTA = {"f16x2": 2.0 ** -36, "f16": 2.0 ** -25, "fp32x3": 0.0}
+DELTA = {"f16x2": 2.0 ** -36, "f16": 2.0 ** -25, "fp32x3": 0.0, "tf32": 0.0}
 C_FLOOR = 2.0
-REPR = {"f16x2": 12, "f16": 2 ** 14 + 4}
+# tf32: fp32 bits go straight to wgmma .tf32, which keeps 10 mantissa bits whether it rounds or truncates the low 13:
+# 2^-10 relative per operand (2^14 units each, + 2^-10 x 2^-10 = 16 units for their product), fp32's exponent range
+# (no floor)
+REPR = {"f16x2": 12, "f16": 2 ** 14 + 4, "tf32": 2 ** 15 + 16}
 MMA_STEP = 3
-CROSS = {"f16x2": 1, "f16": 0}
+CROSS = {"f16x2": 1, "f16": 0, "tf32": 0}
 EPILOGUE = 17
 FP16_MIN_NORMAL = 2.0 ** -14
 
@@ -88,6 +95,12 @@ def kappa_skinny(transposed, K):
     if transposed:
         return 128 + math.ceil(K / 128) + EPILOGUE - 1
     return 4 + 5 + 8 + math.ceil(K / 1024) + EPILOGUE - 1
+
+
+def kappa_c1_stencil(cin_total):
+    """csrc/convt_c1.cu (the FP32-pipe 1-channel ConvTranspose3d): one fma chain of 8 taps x Cin products per output, each
+    fma rounding a partial sum bounded by A (1 unit), then the bias add"""
+    return 8 * cin_total + 1
 
 
 def kappa_x3(stages):
@@ -242,6 +255,12 @@ def f16_round(t):
     return t.detach().float().half().double()
 
 
+def tf32_trunc(t, bits=10):
+    """an fp32 value with its mantissa truncated to `bits` bits (tf32: 10, the low 13 dropped), as fp64"""
+    i = t.detach().float().contiguous().view(torch.int32)
+    return (i & ~((1 << (23 - bits)) - 1)).view(torch.float32).double()
+
+
 def split_f16x2(t):
     """(hi, lo') of csrc/common.cuh split_hi_lo8 in torch: hi = fp16(a), lo' = fp16((a - hi) * 2^11)"""
     a = t.detach().float()
@@ -273,7 +292,10 @@ def scaled_random(shape, scales, gen, device=None):
 
 
 def batch_scales(b):
-    """one all-zero sample, one at 2^-20 (below fp16's normal range: the split floor), the rest from 2^-6 to 2^4"""
+    """one all-zero sample, one at 2^-20 (below fp16's normal range: the split floor), the rest from 2^-6 to 2^4; a batch
+    of one: one sample at scale 1"""
+    if b == 1:
+        return [1.0]
     rest = [2.0 ** v for v in np.linspace(-6, 4, b - 2)]
     return [0.0, 2.0 ** -20] + rest
 
@@ -353,9 +375,11 @@ def x_tile_ref(srcs, conv, bn, slope, tile):
 
 
 def dup_n_tile(w, dim=0, n=64):
-    """output channels [n, 2n) of a weight tensor (dim 0 for Conv3d, 1 for ConvTranspose3d) replaced by [0, n)"""
+    """output channels [n, 2n) of a weight tensor (dim 0 for Conv3d, 1 for ConvTranspose3d) replaced by [0, n) (as many of
+    them as the tensor has past n)"""
     w = w.detach().clone()
-    w.narrow(dim, n, n).copy_(w.narrow(dim, 0, n))
+    m = min(n, w.shape[dim] - n)
+    w.narrow(dim, n, m).copy_(w.narrow(dim, 0, m))
     return w
 
 

@@ -89,6 +89,7 @@ EXACT_WHEN_TF32_OFF = os.environ.get("GENRE_B200_CONV_EXACT", "1") != "0"
 
 _FORCED_MODE = None   # set by _forced_mode(): gradient convolutions use TF32 operands (fp16 would flush small gradients)
 _OVERRIDE = None      # set by precision()
+_NO_BIAS = False      # set by _bias_free(): the epilogue's shift leaves the conv bias out (_affine)
 _EXACT = ("exact", "fp32x3", "f16x2")
 
 
@@ -105,6 +106,20 @@ class _forced_mode:
     def __exit__(self, *exc):
         global _FORCED_MODE
         _FORCED_MODE = self.old
+
+
+class _bias_free:
+    """internal: the convolutions issued inside compute conv(x, W) without the module's bias (the double backward's
+    grad-of-grad convolution: adding the bias and subtracting it in fp32 would leave up to half an ulp of |bias| in
+    outputs that are often many orders of magnitude smaller)"""
+
+    def __enter__(self):
+        global _NO_BIAS
+        self.old, _NO_BIAS = _NO_BIAS, True
+
+    def __exit__(self, *exc):
+        global _NO_BIAS
+        _NO_BIAS = self.old
 
 
 class precision:
@@ -916,15 +931,18 @@ def _versions(*tensors):
 
 
 def _affine(m, bn, npad, dev):
-    """(scale, shift) [npad] of the epilogue: bias, and eval-mode BatchNorm folded in; None if bn needs batch statistics.
-    Cached on the conv module until one of the source tensors is modified in place or replaced."""
+    """(scale, shift) [npad] of the epilogue: bias (left out inside _bias_free), and eval-mode BatchNorm folded in; None if
+    bn needs batch statistics.  Cached on the conv module per (npad, bias left out) until one of the source tensors is
+    modified in place or replaced."""
     cout = m.out_channels
     if bn is not None and (bn.training or not bn.track_running_stats):
         return None
-    ver = (_versions(m.bias, *((bn.running_mean, bn.running_var, bn.weight, bn.bias) if bn is not None else ())),
+    bias = None if _NO_BIAS else m.bias
+    ver = (_versions(bias, *((bn.running_mean, bn.running_var, bn.weight, bn.bias) if bn is not None else ())),
            bn.eps if bn is not None else None, str(dev))
     cache = m.__dict__.setdefault("_gb_affine", {})
-    hit = cache.get(npad)
+    key = (npad, _NO_BIAS)
+    hit = cache.get(key)
     if hit is not None and hit[0] == ver:
         return hit[1]
     scale = shift = None
@@ -932,13 +950,13 @@ def _affine(m, bn, npad, dev):
         if bn is not None:
             inv = torch.rsqrt(bn.running_var + bn.eps)
             scale = inv * (bn.weight if bn.weight is not None else 1.0)
-            bias = m.bias.detach() if m.bias is not None else torch.zeros_like(bn.running_mean)
-            shift = (bias - bn.running_mean) * scale + (bn.bias if bn.bias is not None else 0.0)
+            b = bias.detach() if bias is not None else torch.zeros_like(bn.running_mean)
+            shift = (b - bn.running_mean) * scale + (bn.bias if bn.bias is not None else 0.0)
         sc = torch.ones(npad, device=dev) if scale is None else torch.nn.functional.pad(scale.float(), (0, npad - cout), value=1.0)
         if shift is None:
-            shift = m.bias.detach() if m.bias is not None else torch.zeros(cout, device=dev)
+            shift = bias.detach() if bias is not None else torch.zeros(cout, device=dev)
         out = (sc.contiguous(), torch.nn.functional.pad(shift.float(), (0, npad - cout)).contiguous())
-    cache[npad] = (ver, out)
+    cache[key] = (ver, out)
     return out
 
 
@@ -1165,15 +1183,14 @@ class _ConvInputGrad(torch.autograd.Function):
         ggx = ggx.contiguous()
         g_gy = g_w = None
         if ctx.needs_input_grad[0]:
-            # no grad mode here: the custom forward kernel (bias is not part of it).  Grad-of-grads of a penalty are ~1e-4..1e-7:
-            # never fp16 operands (subnormal / flushed), TF32 at least (the exact modes stay exact)
-            with _forced_mode("tf32"):
+            # no grad mode here: the custom forward kernel, run without the bias (the derivative has no bias term, and adding
+            # it then subtracting it would leave its rounding in these tiny values).  Grad-of-grads of a penalty are
+            # ~1e-4..1e-7: never fp16 operands (subnormal / flushed), TF32 at least (the exact modes stay exact)
+            with _forced_mode("tf32"), _bias_free():
                 g_gy = conv3d(ggx, m)
             if g_gy is None:
                 with cudnn_precision():
                     g_gy = torch.nn.functional.conv3d(ggx, weight, None, m.stride, m.padding, m.dilation, m.groups)
-            elif m.bias is not None:
-                g_gy = g_gy - m.bias.detach().view(1, -1, 1, 1, 1)
         if ctx.needs_input_grad[1]:
             with cudnn_precision():
                 _, g_w, _ = torch.ops.aten.convolution_backward(gy, ggx, weight, None, *ctx.conf, [False, True, False])
@@ -1190,9 +1207,9 @@ def dgrad_convt_k8s2(gy, m):
     """Input gradient of ConvTranspose3d(Cin -> Cout, k8, s2, p3) (Unet_3D.dec5, networks.py:166): out[2i-3+k] += x[i] W[ci,co,k]
     =>  dx[ci, i] = sum_{co,k} gy[co, 2i - 3 + k] W[ci, co, k] = Conv3d(Cout -> Cin, k8, s2, p3) of gy with the SAME weight
     tensor read as [out = Cin, in = Cout, 8, 8, 8]: the 5-tap form over the 2x space-to-depth of gy (kernel MODE 1, N = 96)."""
-    cin_t, cout_t = m.in_channels, m.out_channels
+    cin_t = m.in_channels
     b, _, d, h, w = gy.shape
-    if not (gy.is_cuda and gy.dtype == torch.float32 and cin_t <= 96 and (cout_t * 8) % 8 == 0 and d % 2 == 0 and h % 32 == 0
+    if not (gy.is_cuda and gy.dtype == torch.float32 and cin_t <= 96 and d % 2 == 0 and h % 32 == 0
             and (w // 2) in (16, 32, 64)):
         return None
     with torch.no_grad(), _forced_mode("tf32"):

@@ -7,9 +7,9 @@ calls, the kernel family and kappa per operand mode (tests/infer_ref.py's terms)
 launch: the arguments ops_conv passes (npad, tile width, op) and the C++ dispatch of csrc/convt3d.cu (launch_convt_impl's
 MT narrowing, op 3 falling back to one-level accumulation above N = 128, MODE 5's (PW, CW)), csrc/convflat.cu (one or two
 M-tiles per CTA, narrowed to the register budget) and csrc/convt_c1_col2im.cu.  abi_instances() enumerates every
-instance those dispatchers can reach through the C ABI; ABI_ONLY lists the ones no case reaches, each with why and
-which test runs it.  tests/test_conv_domain_cpu.py checks the ledger against the built library, and
-tests/test_gpu_conv_domain_fp64.py runs every case against fp64.
+instance those dispatchers can reach through the C ABI; ABI_ONLY lists the ones neither this table nor the gradient
+table (tests/conv_grad_domain.py) reaches, each with why and which test runs it.  tests/test_conv_domain_cpu.py checks the
+ledger against the built library, and tests/test_gpu_conv_domain_fp64.py runs every case against fp64.
 
 MMA steps per output (kappa): fp16 operands take K steps of 16 channels (one m64nNk16 wgmma), the fp32 operand modes
 (tf32, the 3xTF32 split) steps of 8 channels (CT_KCG = 2 groups of 4, m64nNk8).  A halo kernel's output sums
@@ -395,7 +395,6 @@ def table_instances():
 
 # Instances the C ABI reaches that no case of the table does: (kernel, args) -> (why no route of ops_conv takes it in the
 # table's modes, the tests that do run it)
-_TRAIN = "test_gpu_train_fp64 (dgrad_convt_k8s2 against fp64)"
 _NONE = "none: reachable only through the C ABI"
 _PAIRED = "test_gpu_convt_paired / test_gpu_k8_stream (paired = 0, bit-equal to the paired walk)"
 _SPLITZ = "test_gpu_conv_k8_tiles / test_gpu_k8_stream (S4D_SPLIT_Z = True)"
@@ -417,8 +416,6 @@ ABI_ONLY = {
     (HALO, (4, 5, 80, 1, 2, 2, 0, 2)): ("merged MODE 2 in the fp16 hi/lo split: ops_conv pairs the classes at W in {16, 32}, "
                                         "the only widths _convt_supported accepts", _PAIRED),
     (HALO, (4, 5, 80, 2, 2, 1, 0, 2)): ("merged MODE 2 with fp16 operands: as above", _PAIRED),
-    (HALO, (5, 5, 96, 1, 1, 3, 0, 2)): ("dec5's input gradient in the exact modes (3xTF32): a backward kernel", _TRAIN),
-    (HALO, (5, 5, 96, 2, 1, 0, 0, 2)): ("dec5's input gradient with TF32 allowed: a backward kernel", _TRAIN),
     (HALO, (5, 5, 96, 1, 1, 2, 0, 2)): (_DGRAD16, _NONE),
     (HALO, (5, 5, 96, 2, 1, 1, 0, 2)): (_DGRAD16, _NONE),
 }

@@ -2,8 +2,9 @@
 
 Ledger: the convt3d_s2_kernel, convflat_kernel and convt_c1_col2im_kernel instances in the built library (cuobjdump
 -symbols; where the library is absent, the three sources are compiled here, convt3d.cu taking about 2 minutes) are
-exactly the instances conv_domain.abi_instances() restates from the C++ dispatch, and exactly those the case table
-reaches plus the listed ABI-only ones.  A kernel instance added without a case fails here.
+exactly the instances conv_domain.abi_instances() restates from the C++ dispatch, and exactly those the forward and
+gradient case tables (conv_domain, conv_grad_domain) reach plus the listed ABI-only ones.  A kernel instance added
+without a case fails here.  The gradient table's cases are checked for their effective modes, entry points and kappa.
 
 tf32 rule (infer_ref: REPR 2^15 + 16, no floor, a K step of 8 channels): an fp64 emulation of the convolution on
 operands truncated to TF32's 10 mantissa bits passes it, so does one rounded to nearest; operands truncated to 9 bits
@@ -18,6 +19,7 @@ import torch
 import torch.nn.functional as F
 
 import conv_domain as D
+import conv_grad_domain as G
 import infer_ref as R
 from genre_shapehd_b200.networks import networks as nets
 
@@ -74,7 +76,9 @@ def test_dispatch_restatement_reaches_exactly_the_built_instances(built_instance
 
 
 def test_table_and_abi_only_list_cover_every_instance_exactly(built_instances):
-    table = set(D.table_instances())
+    grad = set(G.table_instances())
+    assert (D.HALO, (5, 5, 96, 2, 1, 0, 0, 2)) in grad and (D.HALO, (5, 5, 96, 1, 1, 3, 0, 2)) in grad
+    table = set(D.table_instances()) | grad
     abi_only = set(D.ABI_ONLY)
     assert not table & abi_only, sorted(table & abi_only)
     missing = built_instances - table - abi_only
@@ -118,6 +122,39 @@ def test_instance_of_narrows_the_tile_as_the_launcher_does():
     # the flat kernel: two M-tiles once the grid holds 120 CTAs, one at npad 80 in the hi/lo split
     f = D.case("flat convt B5 8^3 c16->80 (two M tiles)")
     assert D.instance_of(f, "f16")[1] == (80, 2, 1) and D.instance_of(f, "f16x2")[1] == (80, 1, 2)
+
+
+@pytest.mark.parametrize("setting", list(G.SETTINGS))
+def test_gradient_settings_give_their_forward_and_effective_modes(setting):
+    from genre_shapehd_b200 import ops_conv
+    precision, allow, fwd, eff = G.SETTINGS[setting]
+    old = ops_conv.PRECISION, ops_conv.EXACT_IMPL, torch.backends.cudnn.allow_tf32
+    try:
+        ops_conv.PRECISION, ops_conv.EXACT_IMPL, torch.backends.cudnn.allow_tf32 = precision, "f16x2", allow
+        assert ops_conv._mode() == fwd
+        with ops_conv._forced_mode("tf32"):
+            assert ops_conv._mode() == eff
+    finally:
+        ops_conv.PRECISION, ops_conv.EXACT_IMPL, torch.backends.cudnn.allow_tf32 = old
+
+
+def test_gradient_table_routes_and_kappa():
+    for c in G.CASES:
+        if c.entry is None:
+            assert not any(c.runs_custom(s[2]) for s in G.SETTINGS.values()), c
+            continue
+        for mode in G.EFFECTIVE:
+            kernel, inst = c.instance(mode)
+            assert inst is not None and inst[5] == D.OP[mode], (c, mode, inst)      # op 3 keeps its second accumulator
+            assert 0 < c.kappa(mode) < 2 ** 17, (c, mode)
+        assert c.kappa("fp32x3") < c.kappa("tf32"), c
+    # the input gradients of ConvTranspose3d k8 are the N = 96 instances, whatever the width
+    for c in G.CASES:
+        if c.kind == "dgrad_convt" and c.entry is not None:
+            assert c.instance("tf32")[1] == (5, 5, 96, 2, 1, 0, 0, 2) and c.instance("fp32x3")[1] == (5, 5, 96, 1, 1, 3, 0, 2)
+    # in the fp16 forward modes ConvTranspose3d needs Cin % 16: 8 -> 2 runs custom only with fp32 forward operands
+    c = G.case("convt 8->2 B1 D3 48x16 (K 16, three row tiles)")
+    assert [s for s, v in G.SETTINGS.items() if c.runs_custom(v[2])] == ["tf32", "fp32x3"]
 
 
 # ---- the tf32 rule ------------------------------------------------------------------------------------------------------

@@ -84,6 +84,20 @@ def _profiled(run, seen):
     return wrapped
 
 
+PROFILE_RETRIES = 3
+
+
+def _profile_again(c, L, mode, seen):
+    """the profiler's CUDA activity has come back without any kernel for both data sets of a case (the numbers were
+    right): run the case again, profiled, until a run records its kernels"""
+    g = torch.Generator(device=DEV).manual_seed(len(c.name))
+    with ops_conv.precision("exact" if mode == "f16x2" else mode), torch.no_grad():
+        for _ in range(PROFILE_RETRIES):
+            if seen:
+                return
+            L.run([R.probe(s, g, DEV) for s in c.shapes])
+
+
 def _extra_controls(c, conv, bn, slope):
     def controls(srcs, mode):
         out = []
@@ -155,6 +169,7 @@ def test_conv_domain_case_vs_fp64(name, mode, monkeypatch):
     _check(c.name, L, mode, monkeypatch)
     want = D.instance_of(c, mode)
     if want is not None:
+        _profile_again(c, L, mode, seen)
         print("[fp64] %s %s kernels %s, expected %s" % (c.name, mode, seen, want))
         assert seen and set(seen) == {want}, (seen, want)
     if seq is not None:

@@ -7,6 +7,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import conv_grad_domain as G
+import infer_ref as IR
 import train_ref as R
 
 
@@ -202,3 +204,24 @@ def test_grid_parameters():
     assert R.bn_nsplit(20, 64 ** 3, 132) == 27 and R.bn_nsplit(4, 64 ** 3, 132) == 64 and R.bn_nsplit(320, 64, 132) == 1
     assert R.c1_slabs(4, 64, 64) == 2048 and R.k8s2_slabs(4, 128, 128) == 2048
     assert R.wgrad_grid(2 * 132 + 1, 132) == 2 * 132
+
+
+@pytest.mark.parametrize("name", [c.name for c in G.CASES if c.kind == "double"])
+def test_bias_round_trip_control_fails_the_fp32x3_rule_of_every_double_backward_route(name):
+    """The double backward's grad-of-grad convolution conv3d(v, W) at the GPU cases' shapes and layers (PyTorch's default
+    bias), v at infer_ref.batch_scales (an all-zero sample, one at 2^-20): fp32(fp32(ref + b) - b), the bias added by the
+    epilogue and subtracted again, exceeds the route's fp32x3 kappa, while the correctly rounded fp32 result is within
+    one unit and the all-zero sample's round trip is exact"""
+    c = G.case(name)
+    m = G.module(c)
+    v = IR.scaled_random(c.x, IR.batch_scales(c.x[0]), torch.Generator().manual_seed(sum(c.x)))
+    w = m.weight.detach().double()
+    ref = IR.conv64(v.double(), w, m)
+    A = IR.conv64(v.double().abs(), w.abs(), m)
+    kappa = c.kappa("fp32x3")
+    ctl = R.bias_round_trip(ref, m.bias)
+    assert R.err_ratio(ref.float(), ref, A) <= 1.0
+    assert R.err_ratio(ctl[:1], ref[:1], A[:1]) == 0.0                 # the zero sample: (0 + b) - b = 0 exactly
+    r = R.err_ratio(ctl[1:2], ref[1:2], A[1:2])
+    print("%s: bias round trip at 2^-20 err/(2^-24 A) = %.4g, fp32x3 kappa %.4g" % (name, r, kappa))
+    assert r > kappa, (r, kappa)

@@ -227,6 +227,14 @@ def drop_lane(t, dim=1, lane=3):
     return t
 
 
+def bias_round_trip(ref, bias):
+    """fp32(fp32(ref + b) - b) per output channel: a bias-free convolution computed by an epilogue that adds the bias,
+    with the bias subtracted again in fp32.  The sum keeps half an ulp of |b|, which dwarfs tiny outputs: the negative
+    control of the double backward's grad-of-grad convolution"""
+    b = bias.detach().view(1, -1, 1, 1, 1)
+    return (ref.double() + b.double()).float() - b.float()
+
+
 def drop_c1_slab(x, slab):
     """zero the input positions of one slab (b, z, 8 rows) of the 1-channel ConvTranspose3d gradients: every term of that
     slab's contribution to dW carries one of them"""

@@ -265,8 +265,6 @@ class Deconv3d_skip(nn.Module):
         if y is not None:
             return y
         ops_conv._fp32_only(x, skip_in)
-        if isinstance(x, ops_conv.BlockedActivation):
-            x = x.ncdhw()
         if ops_conv.BN_TRAIN and x.is_cuda and isinstance(self.net, nn.Sequential) and self.net[1].training:
             c = self.net[0](cat((x, skip_in), dim=1))
             z = ops_conv.bn_act_train(c, self.net[1], self.net[2])

@@ -4,7 +4,7 @@
 library's kernels, or ``None`` when no kernel covers the layer (shape / dtype / device / autograd) — the caller then
 runs the layer the way the reference does (torch.nn -> cuDNN; in the fp32-accurate mode through ``exact_fallback``).
 
-Kernels and what they cover (routing conditions are the ``*_supported`` predicates below, all of them tested both ways):
+Kernels and what they cover (_conv_route / _convt_route pick one per call from the ``*_supported`` predicates below):
   csrc/convt3d.cu          wgmma implicit GEMM on halo tiles: ConvTranspose3d k 4 / 8, s 2 (planes 16 or 32 wide), Conv3d
                            k 4 s 2 via parity sub-volumes, Conv3d k 8 s 2 via space-to-depth, the 1-channel ConvTranspose3d
                            with 27 union taps; forward under autograd too, tensor-core input gradients for the k 8 layers
@@ -149,14 +149,6 @@ def _mode():
             return "fp32x3"
         return base if base == "f16x2" else EXACT_IMPL
     return _FORCED_MODE or base
-
-
-def cudnn_precision():
-    """cuDNN flags for GRADIENT convolutions this module hands to cuDNN: the caller's global setting (PyTorch's default allows
-    TF32).  The north_star's 1e-4 bound is on the forward outputs; gradients follow PyTorch's switch, as they do upstream:
-    `torch.backends.cudnn.allow_tf32 = False` makes them fp32."""
-    import contextlib
-    return contextlib.nullcontext()
 
 
 def exact_fallback(x, m, transposed, output_size=None):
@@ -365,7 +357,7 @@ PLAIN, PARITY = 1, 2     # operand layouts of csrc/convt3d.cu: blocked [B*D][par
 class OperandActivation:
     """The output of a layer that exists only as the fp16 operand(s) of the layers consuming it: `operands[layout]` =
     (tensor, cpad) for PLAIN (a following ConvTranspose3d) and / or PARITY (a following Conv3d k4 s2).  Quacks like the
-    NCDHW fp32 tensor for the routing predicates but holds no fp32 values: the hi/lo split loses ~2 bits, so fp32 cannot be
+    NCDHW fp32 tensor for the entry points' source checks but holds no fp32 values: the hi/lo split loses ~2 bits, so fp32 cannot be
     rebuilt from it, and a layer that would need fp32 refuses it (operand()).  Producers write one only when
     conv_operand_layout / deconv_operand_layout said that every consumer reads it directly."""
     is_cuda, dtype, requires_grad = True, torch.float32, False
@@ -393,36 +385,28 @@ def _fp32_only(*xs):
             x.operand(None)     # raises
 
 
-def _operand_outputs_ok(m, bn):
-    """can a layer with module m [and BatchNorm bn] read its input straight from the producer's operand output?  The fp16
-    modes only (the fp32x3 / tf32 operands are fp32 values), no autograd, no batch statistics"""
-    return (_mode() in ("f16x2", "f16") and _no_autograd(m.weight, m.bias) and not _needs_grad(m.weight, m.bias)
-            and (bn is None or (not bn.training and bn.track_running_stats)))
-
-
 def conv_operand_layout(x_shape, m, bn=None):
     """(layout, cpad) in which conv3d(x, m, bn) reads an input of x_shape as the kernel operand in the current mode, or None
-    when it needs the fp32 activation.  Same predicates, in the same order, as conv3d's routing."""
-    x = OperandActivation(x_shape)
-    if (not _operand_outputs_ok(m, bn) or _skinny_conv_supported(x, m) or _flat_conv_supported(x, m)
-            or not _conv_k4s2_supported(x, m)):
+    when it needs the fp32 activation: the fp16 modes (the fp32x3 / tf32 operands are fp32 values) on the k4 s2 route."""
+    route = _conv_route(m, (tuple(x_shape), "operand"), bn, False, _needs_grad(m.weight, m.bias))
+    if _mode() not in ("f16x2", "f16") or route != "conv_k4s2":
         return None
     return PARITY, _k4s2_cpad(x_shape[1])
 
 
 def deconv_operand_layout(x_shape, skip_shape, conv, bn=None):
     """(layout, cpad) in which deconv_skip reads each of its two inputs (shapes x_shape, skip_shape) as the kernel operand
-    in the current mode, or None when it needs the fp32 activations.  Same predicates, in the same order, as deconv_skip's
-    routing; the two inputs have the same channel count in Unet_3D, so one layout serves both."""
-    x, s = OperandActivation(x_shape), OperandActivation(skip_shape)
-    if x_shape[1] != skip_shape[1] or not _operand_outputs_ok(conv, bn):
+    in the current mode, or None when it needs the fp32 activations: the fp16 modes on the col2im or the halo route.  The two
+    inputs have the same channel count in Unet_3D, so one layout serves both."""
+    if x_shape[1] != skip_shape[1] or _mode() not in ("f16x2", "f16"):
         return None
-    if bn is None and conv.out_channels == 1:
-        cpad = -(-x_shape[1] // 8) * 8     # the padding _operand_of gives the fp32 blocked twin
-        return (PLAIN, cpad) if _convt_c1_col2im_supported((x, s), conv) and (2 * cpad) % 16 == 0 else None
-    if _flat_convt_supported((x, s), conv) or not _deconv_kernel_supported(x, s, conv):
-        return None
-    return PLAIN, x_shape[1]
+    srcs = [(tuple(x_shape), "operand"), (tuple(skip_shape), "operand")]
+    route = _convt_route(conv, srcs, bn, False, _needs_grad(conv.weight, conv.bias))
+    if route == "convt_c1_col2im":
+        return PLAIN, _operand_cpad(srcs[0])
+    if route in ("convt_k4", "convt_k8"):
+        return PLAIN, x_shape[1]
+    return None
 
 
 def _operand_request(operands, shape, device):
@@ -450,31 +434,8 @@ def _operand_destinations(operands, shape, device):
     return act, args + [None, 0, 0] * (2 - len(operands))
 
 
-class BlockedActivation:
-    """An activation that exists only in the fp32 blocked layout [B*D, C/4, H, W, 4].  Quacks like the NCDHW tensor for
-    the dispatch checks: the custom layers read its blocked tensor directly, and ncdhw() materialises it for a layer that
-    needs the plain layout."""
-    is_cuda, dtype, requires_grad = True, torch.float32, False
-
-    def __init__(self, y, batch, channels):
-        bd, cg, h, w, _ = y.shape
-        self._gb_blocked, self.batch, self.shape = y, batch, torch.Size((batch, channels, bd // batch, h, w))
-        self.device = y.device
-
-    def dim(self):
-        return 5
-
-    def size(self, i=None):
-        return self.shape if i is None else self.shape[i]
-
-    def ncdhw(self):
-        return from_blocked(self._gb_blocked, self.batch, self.shape[1])
-
-
 def _cached_blocked(x):
     """the blocked twin a custom layer attached to its NCDHW result, unless that result was since modified in place"""
-    if isinstance(x, BlockedActivation):
-        return x._gb_blocked
     hit = getattr(x, "_gb_blocked", None)
     if hit is None or hit[1] != x._version:
         return None
@@ -651,15 +612,12 @@ def _cached_pack(module, key, make):
     return hit[1]
 
 
-def _convt_supported(shape_bcdhw, module):
-    b, c, d, h, w = shape_bcdhw
-    k = module.kernel_size[0]
-    if ("convt_k8" if k == 8 else "convt_k4") not in POLICY:
-        return False
-    return (ENABLED and tuple(module.kernel_size) == (k, k, k) and k in (4, 8) and tuple(module.stride) == (2, 2, 2)
-            and tuple(module.padding) == (k // 2 - 1,) * 3 and tuple(module.output_padding) == (0, 0, 0)
-            and tuple(module.dilation) == (1, 1, 1) and module.groups == 1 and w in (16, 32) and h % 16 == 0
-            and c % (2 * _group()) == 0 and module.out_channels <= 64)
+def _convt_supported(shape, m):
+    """ConvTranspose3d k 4 / 8, s 2 on the halo kernel (convt3d_s2_blocked); shape: the (concatenated) source"""
+    b, c, d, h, w = shape
+    geo = _geometry(m)
+    return (ENABLED and geo in (_CONVT_K4S2, _CONVT_K8S2) and ("convt_k8" if geo == _CONVT_K8S2 else "convt_k4") in POLICY
+            and w in (16, 32) and h % 16 == 0 and c % (2 * _group()) == 0 and m.out_channels <= 64)
 
 
 def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0, operands=None):
@@ -702,12 +660,11 @@ def convt3d_s2_blocked(src0, src1, batch, module, bn=None, slope=1.0, operands=N
     return out if act is None else act
 
 
-def _no_autograd(*tensors):
-    """The kernels are forward-only: they run when no gradient is needed.  torch.backends.cudnn.allow_tf32 (PyTorch's own
-    switch, on by default, for the cuDNN path they replace) selects the operand mode, see _mode()."""
-    if not torch.backends.cudnn.allow_tf32 and not EXACT_WHEN_TF32_OFF:
-        return False
-    return not (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors))
+def _inference(grad):
+    """The kernels are forward-only: they run when no gradient is needed (grad = _needs_grad(...)).
+    torch.backends.cudnn.allow_tf32 (PyTorch's own switch, on by default, for the cuDNN path they replace) selects the operand
+    mode, see _mode()."""
+    return not grad and (torch.backends.cudnn.allow_tf32 or EXACT_WHEN_TF32_OFF)
 
 
 def space_to_depth_blocked(x, group=4, dtype=None, cpad=0):
@@ -809,20 +766,16 @@ def pack_conv_k4s2_s2d_weights(weight, cpad, npad, group=4):
     return _finish_pack(out, g)
 
 
-def _conv_k4s2_s2d_supported(x, m):
+def _conv_k4s2_s2d_supported(shape, m):
     """few input channels (the critic's 1 -> 64 first layer): the 8*Cin space-to-depth channels fit one K chunk"""
-    return ("conv_k4s2_s2d" in POLICY and ENABLED and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
-            and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2) and tuple(m.padding) == (1, 1, 1)
-            and tuple(m.dilation) == (1, 1, 1) and m.groups == 1 and m.padding_mode == "zeros" and x.shape[1] <= 2
-            and 32 < m.out_channels <= 64 and all(v % 2 == 0 for v in x.shape[2:]) and x.shape[4] // 2 in (16, 32, 64)
-            and (x.shape[3] // 2) % 16 == 0)
+    return ("conv_k4s2_s2d" in POLICY and ENABLED and _geometry(m) == _CONV_K4S2 and shape[1] <= 2
+            and 32 < m.out_channels <= 64 and all(v % 2 == 0 for v in shape[2:]) and shape[4] // 2 in (16, 32, 64)
+            and (shape[3] // 2) % 16 == 0)
 
 
 def _conv_k4s2_s2d(x, m, bn, slope):
     cout, npad, g = m.out_channels, 64, _group()
     aff = _affine(m, bn, npad, x.device)
-    if aff is None:
-        return None
     cpad = -(-x.shape[1] * 8 // (2 * g)) * 2 * g          # the 8*Cin channels rounded up to whole K chunks
     wpack = _pack(m, ("k4s2_s2d", cpad, npad, g), lambda w: pack_conv_k4s2_s2d_weights(w, cpad, npad, g), 1)
     if _x2_direct(x):
@@ -867,17 +820,58 @@ def pack_conv_k8s2_weights(weight, npad, group=4):
     return _finish_pack(out, g)
 
 
-def _packed_conv(module, npad):
+def _conv_k8s2_supported(shape, m):
+    return ("conv_k8s2" in POLICY and ENABLED and _geometry(m) == _CONV_K8S2 and m.out_channels <= 32 and shape[1] % 2 == 0
+            and shape[1] <= 8 and all(v % 2 == 0 for v in shape[2:]) and shape[4] // 2 in (16, 32, 64)
+            and (shape[3] // 2) % 16 == 0)
+
+
+def _conv_k8s2_s4d_form(shape, m):
+    """the k8 s2 layer as 3 taps over the 4x space-to-depth input (else the 5 taps over the 2x one)"""
+    return MERGE_PARITIES and m.out_channels <= 20 and all(v % 64 == 0 for v in shape[3:]) and shape[2] % 4 == 0
+
+
+def _conv_k8s2_s4d(x, m, bn, slope, operands=None):
+    # 4x space-to-depth: 3 taps over 64*Cin channels, the 8 output classes of the 2x finer grid merged along N
+    aff = _affine(m, bn, 20, x.device)
+    g, b, cout = _group(), x.shape[0], m.out_channels
+    split_z = S4D_SPLIT_Z or _x2() or _x3()   # f16x2 / fp32x3 double the accumulator columns: 8 classes x 20 x 2 = 320 > 256
+    wpack = _pack(m, ("k8s2_s4d", 20, g, split_z), lambda wt: pack_conv_k8s2_s4d_weights(wt, 20, g, split_z),
+                  2 if split_z else 1)
+    if _x2_direct(x):
+        xb = space_to_depth4_blocked(x, 16, torch.float16)
+    else:
+        xb = _finish_operand(space_to_depth4_blocked(x, _act_group(), torch.float16 if _f16() else None))
+    bd, cg, h, w, _ = xb.shape
+    cgo = (cout + 3) // 4
+    # operand outputs: output class q at coarse position j is enc2's parity sub-volume q at j
+    act, dst = _operand_request(operands, (b, cout, 2 * (bd // b), 2 * h, 2 * w), x.device)
+    out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=x.device, dtype=torch.float32) if act is None else None
+    _lib.call("genre_b200_conv3d_k8s2_s4d_forward", xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(),
+              80 if split_z else 160, _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
+              out.data_ptr() if out is not None else None, cgo, *dst, _lib.stream_ptr(x))
+    return from_blocked(out, b, cout) if act is None else act
+
+
+def _conv_k8s2_taps(x, m, bn, slope):
+    cout, npad = m.out_channels, 32
+    aff = _affine(m, bn, npad, x.device)
+    sc, sh = aff
+    dev = x.device
     g = _group()
-    return _pack(module, ("k8s2", npad, g), lambda w: pack_conv_k8s2_weights(w, npad, g), 1)
-
-
-def _conv_k8s2_supported(x, m):
-    return ("conv_k8s2" in POLICY and ENABLED and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and tuple(m.kernel_size) == (8, 8, 8)
-            and tuple(m.stride) == (2, 2, 2) and tuple(m.padding) == (3, 3, 3) and tuple(m.dilation) == (1, 1, 1)
-            and m.groups == 1 and m.out_channels <= 32 and x.shape[1] % 2 == 0 and x.shape[1] <= 8
-            and all(v % 2 == 0 for v in x.shape[2:]) and x.shape[4] // 2 in (16, 32, 64) and (x.shape[3] // 2) % 16 == 0
-            and m.padding_mode == "zeros")
+    wpack = _pack(m, ("k8s2", npad, g), lambda w: pack_conv_k8s2_weights(w, npad, g), 1)
+    if _x2_direct(x):
+        xb = space_to_depth_blocked(x, 16, torch.float16)
+    else:
+        xb = _finish_operand(space_to_depth_blocked(x, 8, torch.float16) if _f16() else space_to_depth_blocked(x))
+    b = x.shape[0]
+    bd, cg, h, w, _ = xb.shape
+    cgo = (cout + 3) // 4
+    out = torch.empty((bd, cgo, h, w, 4), device=dev, dtype=torch.float32)
+    _lib.call("genre_b200_conv3d_taps_forward", xb.data_ptr(), cg // _parts(), None, 0, b, bd // b, h, w,
+              wpack.data_ptr(), 5, 2, npad, _op_flag(), sc.data_ptr(), sh.data_ptr(),
+              1.0 if slope is None else float(slope), out.data_ptr(), cgo, _lib.stream_ptr(x))
+    return from_blocked(out, b, cout)
 
 
 def space_to_depth_sources(x, cpad, group, dtype):
@@ -919,11 +913,10 @@ def pack_conv_k4s2_weights(weight, cpad, npad, group):
     return _finish_pack(out, g)
 
 
-def _conv_k4s2_supported(x, m):
-    return ("conv_k4s2" in POLICY and ENABLED and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and tuple(m.kernel_size) == (4, 4, 4)
-            and tuple(m.stride) == (2, 2, 2) and tuple(m.padding) == (1, 1, 1) and tuple(m.dilation) == (1, 1, 1)
-            and m.groups == 1 and m.out_channels <= 128 and x.shape[1] >= K4S2_MIN_CIN and m.padding_mode == "zeros"
-            and all(v % 2 == 0 for v in x.shape[2:]) and x.shape[4] // 2 in (16, 32) and (x.shape[3] // 2) % 16 == 0)
+def _conv_k4s2_supported(shape, m):
+    return ("conv_k4s2" in POLICY and ENABLED and _geometry(m) == _CONV_K4S2 and m.out_channels <= 128
+            and shape[1] >= K4S2_MIN_CIN and all(v % 2 == 0 for v in shape[2:]) and shape[4] // 2 in (16, 32)
+            and (shape[3] // 2) % 16 == 0)
 
 
 def _versions(*tensors):
@@ -935,7 +928,7 @@ def _affine(m, bn, npad, dev):
     bn needs batch statistics.  Cached on the conv module per (npad, bias left out) until one of the source tensors is
     modified in place or replaced."""
     cout = m.out_channels
-    if bn is not None and (bn.training or not bn.track_running_stats):
+    if _batch_stats(bn):
         return None
     bias = None if _NO_BIAS else m.bias
     ver = (_versions(bias, *((bn.running_mean, bn.running_var, bn.weight, bn.bias) if bn is not None else ())),
@@ -970,8 +963,6 @@ def _conv_k4s2(x, m, bn, slope, operands=None):
     cout = m.out_channels
     npad = 32 * ((cout + 31) // 32)
     aff = _affine(m, bn, npad, x.device)
-    if aff is None:
-        return None
     g = _group()
     cpad = _k4s2_cpad(x.shape[1])
     wpack = _pack(m, ("k4s2", cpad, npad, g), lambda w: pack_conv_k4s2_weights(w, cpad, npad, g), 1)
@@ -1050,36 +1041,25 @@ def pack_flat_conv_weights(weight, npad, group=8):
 
 
 def _flat_common(m):
-    return ("flat" in POLICY and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
-            and tuple(m.padding) == (1, 1, 1) and tuple(m.dilation) == (1, 1, 1) and m.groups == 1
+    return ("flat" in POLICY and ENABLED and (_f16() or _x2())
             and m.out_channels >= 8)     # fewer output channels: the one-channel kernels (an N tile here is 64 columns)
 
 
-def _flat_source_ok(x):
-    return (torch.is_tensor(x) or isinstance(x, OperandActivation)) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and x.shape[1] % 8 == 0
-
-
 def _flat_convt_supported(sources, m):
-    return (isinstance(m, torch.nn.ConvTranspose3d) and _flat_common(m) and tuple(m.output_padding) == (0, 0, 0)
-            and all(_flat_source_ok(x) and x.shape[2:] == sources[0].shape[2:] and x.shape[0] == sources[0].shape[0] for x in sources)
-            and max(sources[0].shape[2:]) <= FLAT_MAX and sum(x.shape[1] for x in sources) == m.in_channels
-            and _no_autograd(*sources, m.weight, m.bias))
+    """do conv_transpose3d / deconv_skip run these activations on the flat kernel?"""
+    return _convt_route(m, [_source(x) for x in sources], grad=_needs_grad(*sources, m.weight, m.bias)) == "flat"
 
 
 def _flat_conv_supported(x, m):
-    return (isinstance(m, torch.nn.Conv3d) and _flat_common(m) and m.padding_mode == "zeros" and _flat_source_ok(x)
-            and x.shape[1] % 16 == 0 and x.shape[1] == m.in_channels and all(v % 2 == 0 for v in x.shape[2:])
-            and max(x.shape[2:]) <= 2 * FLAT_MAX and _no_autograd(x, m.weight, m.bias))
+    """does conv3d run the activation x on the flat kernel?"""
+    return _conv_route(m, _source(x), grad=_needs_grad(x, m.weight, m.bias)) == "flat"
 
 
 def _flat_run(sources, m, bn, slope, transposed):
-    _fp32_only(*sources)
     cout = m.out_channels
     npad = flat_npad(cout)
     dev = sources[0].device
     aff = _affine(m, bn, -(-cout // npad) * npad, dev)
-    if aff is None:
-        return None
     b = sources[0].shape[0]
     if transposed:
         d, h, w = sources[0].shape[2:]
@@ -1110,22 +1090,20 @@ def _flat_run(sources, m, bn, slope, transposed):
 
 
 # ---- the 1^3 end of the U-Net: weight-streaming FP32 products (csrc/skinny_gemm.cu) ------------------------------------------
-def _skinny_ok(x, m):
-    return ("skinny" in POLICY and ENABLED and torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
-            and m.groups == 1 and tuple(m.dilation) == (1, 1, 1) and tuple(m.padding) == (0, 0, 0) and m.weight.dtype == torch.float32
-            and not (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, m.weight, m.bias))))
+def _skinny_ok(m, transposed):
+    t, _, _, p, op, d, groups, mode = _geometry(m)
+    return ("skinny" in POLICY and ENABLED and t == transposed and p == op == (0, 0, 0) and d == (1, 1, 1) and groups == 1
+            and mode == "zeros" and m.weight.dtype == torch.float32)
 
 
 def _skinny_conv_supported(x, m):
-    """Conv3d whose kernel is its whole input: one output voxel per (sample, channel)"""
-    return (isinstance(m, torch.nn.Conv3d) and _skinny_ok(x, m) and m.padding_mode == "zeros" and tuple(x.shape[2:]) == tuple(m.kernel_size)
-            and x.shape[1] == m.in_channels and (x.shape[1] * x.shape[2] * x.shape[3] * x.shape[4]) % 4 == 0)
+    """does conv3d run the activation x on the skinny kernel?"""
+    return _conv_route(m, _source(x), grad=_needs_grad(x, m.weight, m.bias)) == "skinny"
 
 
 def _skinny_convt_supported(x, m):
-    """ConvTranspose3d of a 1^3 input: the output is the kernel weighted by the input channels"""
-    return (isinstance(m, torch.nn.ConvTranspose3d) and _skinny_ok(x, m) and tuple(x.shape[2:]) == (1, 1, 1) and x.shape[1] == m.in_channels
-            and tuple(m.output_padding) == (0, 0, 0) and (m.out_channels * m.kernel_size[0] * m.kernel_size[1] * m.kernel_size[2]) % 4 == 0)
+    """does conv_transpose3d run the activation x on the skinny kernel?"""
+    return _convt_route(m, [_source(x)], grad=_needs_grad(x, m.weight, m.bias)) == "skinny"
 
 
 def _aligned(t):
@@ -1136,8 +1114,6 @@ def _aligned(t):
 def _skinny_run(x, m, bn, slope, transposed):
     cout = m.out_channels
     aff = _affine(m, bn, cout, x.device)
-    if aff is None:
-        return None
     b = x.shape[0]
     x2 = _aligned(x.reshape(b, -1))
     w = _aligned(m.weight.detach())
@@ -1169,8 +1145,7 @@ class _ConvInputGrad(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gy, weight, x, m):
         conf = (list(m.stride), list(m.padding), list(m.dilation), False, [0, 0, 0], m.groups)
-        with cudnn_precision():
-            gx, _, _ = torch.ops.aten.convolution_backward(gy, x, weight, None, *conf, [True, False, False])
+        gx, _, _ = torch.ops.aten.convolution_backward(gy, x, weight, None, *conf, [True, False, False])
         ctx.save_for_backward(gy, weight)
         ctx.m, ctx.conf = m, conf
         return gx
@@ -1189,11 +1164,9 @@ class _ConvInputGrad(torch.autograd.Function):
             with _forced_mode("tf32"), _bias_free():
                 g_gy = conv3d(ggx, m)
             if g_gy is None:
-                with cudnn_precision():
-                    g_gy = torch.nn.functional.conv3d(ggx, weight, None, m.stride, m.padding, m.dilation, m.groups)
+                g_gy = torch.nn.functional.conv3d(ggx, weight, None, m.stride, m.padding, m.dilation, m.groups)
         if ctx.needs_input_grad[1]:
-            with cudnn_precision():
-                _, g_w, _ = torch.ops.aten.convolution_backward(gy, ggx, weight, None, *ctx.conf, [False, True, False])
+            _, g_w, _ = torch.ops.aten.convolution_backward(gy, ggx, weight, None, *ctx.conf, [False, True, False])
         return g_gy, g_w, None, None
 
 
@@ -1203,14 +1176,28 @@ class _ConvInputGrad(torch.autograd.Function):
 TC_BACKWARD = os.environ.get("GENRE_B200_CONV_TC_BACKWARD", "1") != "0"
 
 
+def _tc_dgrad_supported(gy_shape, m):
+    """the input gradient of a k8 s2 layer on the tensor cores, for an output gradient of gy_shape: dgrad_convt_k8s2 for a
+    ConvTranspose3d with Cin <= 96 (Unet_3D.dec5), dgrad_conv_k8s2 for a Conv3d with Cin <= 20 (Unet_3D.enc1)"""
+    b, _, d, h, w = gy_shape
+    geo = _geometry(m)
+    if geo == _CONVT_K8S2:
+        return m.in_channels <= 96 and d % 2 == 0 and h % 32 == 0 and (w // 2) in (16, 32, 64)
+    return geo == _CONV_K8S2 and m.in_channels <= 20 and h % 16 == 0 and (w == 16 or w % 32 == 0)
+
+
+def _k8_wgrad_supported(x_shape, m):
+    """Unet_3D.enc1's weight gradient on csrc/convt_c1_wgrad.cu (first-order backward only; cuDNN's: a 40 ms direct kernel)"""
+    return ("conv_k8s2_wgrad" in POLICY and _geometry(m) == _CONV_K8S2 and m.in_channels <= 2 and m.out_channels <= 20
+            and x_shape[3] % 16 == 0 and x_shape[4] <= 128 and x_shape[2] % 2 == 0 and x_shape[4] % 2 == 0)
+
+
 def dgrad_convt_k8s2(gy, m):
     """Input gradient of ConvTranspose3d(Cin -> Cout, k8, s2, p3) (Unet_3D.dec5, networks.py:166): out[2i-3+k] += x[i] W[ci,co,k]
     =>  dx[ci, i] = sum_{co,k} gy[co, 2i - 3 + k] W[ci, co, k] = Conv3d(Cout -> Cin, k8, s2, p3) of gy with the SAME weight
     tensor read as [out = Cin, in = Cout, 8, 8, 8]: the 5-tap form over the 2x space-to-depth of gy (kernel MODE 1, N = 96)."""
-    cin_t = m.in_channels
-    b, _, d, h, w = gy.shape
-    if not (gy.is_cuda and gy.dtype == torch.float32 and cin_t <= 96 and d % 2 == 0 and h % 32 == 0
-            and (w // 2) in (16, 32, 64)):
+    cin_t, b = m.in_channels, gy.shape[0]
+    if not (gy.is_cuda and gy.dtype == torch.float32 and _tc_dgrad_supported(gy.shape, m)):
         return None
     with torch.no_grad(), _forced_mode("tf32"):
         g = _group()
@@ -1235,9 +1222,8 @@ def dgrad_conv_k8s2(gy, m):
     """Input gradient of Conv3d(Cin -> Cout, k8, s2, p3) with Cin <= 20 (Unet_3D.enc1, networks.py:151) = ConvTranspose3d(Cout ->
     Cin, k8, s2, p3) of gy with the SAME weight tensor read as [in = Cout, out = Cin, 8, 8, 8]: the merged-parity kernel
     (MODE 2) over 32-wide x tiles.  Cout is zero-padded to a multiple of 8 (whole K chunks)."""
-    cin, cout = m.in_channels, m.out_channels
-    b, _, d, h, w = gy.shape
-    if not (gy.is_cuda and gy.dtype == torch.float32 and cin <= 20 and h % 16 == 0 and (w == 16 or w % 32 == 0)):
+    cin, cout, b = m.in_channels, m.out_channels, gy.shape[0]
+    if not (gy.is_cuda and gy.dtype == torch.float32 and _tc_dgrad_supported(gy.shape, m)):
         return None
     pad = (-cout) % 8
     with torch.no_grad(), _forced_mode("tf32"):
@@ -1287,11 +1273,7 @@ class _ConvForward(torch.autograd.Function):
         mask = [ctx.needs_input_grad[0], ctx.needs_input_grad[1], bias_sizes is not None and ctx.needs_input_grad[2]]
         gy = gy.contiguous()
         gw_custom = None
-        if (mask[1] and not transposed and not torch.is_grad_enabled() and "conv_k8s2_wgrad" in POLICY
-                and tuple(weight.shape[2:]) == (8, 8, 8) and stride == (2, 2, 2) and padding == (3, 3, 3)
-                and dilation == (1, 1, 1) and groups == 1 and weight.shape[1] <= 2 and weight.shape[0] <= 20
-                and x.shape[3] % 16 == 0 and x.shape[4] <= 128 and x.shape[2] % 2 == 0 and x.shape[4] % 2 == 0):
-            # Unet_3D.enc1: cuDNN's wgrad for this shape is a 40 ms grouped direct kernel (csrc/convt_c1_wgrad.cu)
+        if mask[1] and not torch.is_grad_enabled() and _k8_wgrad_supported(x.shape, ctx.module):
             xc = x.contiguous()
             nbytes = _lib.load().genre_b200_conv_k8s2_wgrad_workspace_bytes()
             ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
@@ -1301,19 +1283,16 @@ class _ConvForward(torch.autograd.Function):
             mask[1] = False
         gx = gw = gb = None
         gx_custom = None
-        if (TC_BACKWARD and mask[0] and not torch.is_grad_enabled() and ctx.module is not None
-                and tuple(weight.shape[2:]) == (8, 8, 8) and stride == (2, 2, 2) and padding == (3, 3, 3) and groups == 1
-                and dilation == (1, 1, 1) and out_pad == (0, 0, 0)):
+        if TC_BACKWARD and mask[0] and not torch.is_grad_enabled():
             gx_custom = (dgrad_convt_k8s2 if transposed else dgrad_conv_k8s2)(gy, ctx.module)
             if gx_custom is not None:
                 mask[0] = False
-        if mask[0] and torch.is_grad_enabled() and not transposed and ctx.module is not None:
+        if mask[0] and torch.is_grad_enabled() and not transposed:
             gx_custom = _ConvInputGrad.apply(gy, weight, x, ctx.module)   # double backward stays on the custom forward
             mask[0] = False
         if any(mask):
-            with cudnn_precision():
-                gx, gw, gb = torch.ops.aten.convolution_backward(gy, x, weight, bias_sizes, list(stride), list(padding),
-                                                                  list(dilation), transposed, list(out_pad), groups, mask)
+            gx, gw, gb = torch.ops.aten.convolution_backward(gy, x, weight, bias_sizes, list(stride), list(padding),
+                                                              list(dilation), transposed, list(out_pad), groups, mask)
         return (gx_custom if gx_custom is not None else gx), (gw_custom if gw_custom is not None else gw), gb, None
 
 
@@ -1355,95 +1334,21 @@ class _ConvTC1Train(torch.autograd.Function):
         return gx, gw, gb, None
 
 
-def _convt_c1_train_supported(x, m):
-    return (ENABLED and "convt_c1_train" in POLICY and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
-            and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2) and tuple(m.padding) == (1, 1, 1)
-            and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1) and m.groups == 1
-            and m.out_channels == 1 and x.shape[1] % 4 == 0 and x.shape[1] <= 48 and x.shape[3] % 8 == 0
-            and x.shape[4] % 4 == 0 and x.shape[4] <= 64)
+def _convt_c1_train_supported(shape, m):
+    return (ENABLED and "convt_c1_train" in POLICY and _geometry(m) == _CONVT_K4S2 and m.out_channels == 1
+            and shape[1] % 4 == 0 and shape[1] <= 48 and shape[3] % 8 == 0 and shape[4] % 4 == 0 and shape[4] <= 64)
 
 
 TRAIN_FORWARD = os.environ.get("GENRE_B200_CONV_TRAIN_FORWARD", "1") != "0"
 
 
-def _train_forward(x, m, supported):
-    """conv-only call under autograd: custom forward + cuDNN backward when the layer is covered, else None"""
-    if not (TRAIN_FORWARD and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and supported):
-        return None
+def _train_forward(x, m):
+    """conv-only call under autograd: custom forward + cuDNN backward"""
     return _ConvForward.apply(x, m.weight, m.bias, m)
 
 
-def conv3d(x, m, bn=None, slope=None, operands=None):
-    """Conv3d on the tensor-core kernel [+ folded eval BatchNorm3d + LeakyReLU]: k=8,s=2,p=3 on few input channels
-    (Unet_3D.enc1) via space-to-depth, or k=4,s=2,p=1 (discriminator, Unet_3D.enc2/enc3) via parity sub-volumes.
-    operands: [(layout, cpad)] of the consumers (conv_operand_layout / deconv_operand_layout): enc1 and the k4 s2 layers then
-    return the output as an OperandActivation."""
-    if not x.is_cuda:
-        return None
-    if isinstance(x, OperandActivation):
-        if _flat_conv_supported(x, m) or not (_no_autograd(x, m.weight, m.bias) and _conv_k4s2_supported(x, m)):
-            _fp32_only(x)
-        return _conv_k4s2(x, m, bn, slope, operands)
-    if _needs_grad(x, m.weight, m.bias):
-        if bn is not None or slope is not None:
-            return None     # fused epilogues are inference-only; the caller falls back to module-by-module
-        return _train_forward(x, m, _conv_k4s2_supported(x, m) or _conv_k8s2_supported(x, m) or _conv_k4s2_s2d_supported(x, m))
-    if not _no_autograd(x, m.weight, m.bias):
-        return None
-    if _skinny_conv_supported(x, m):
-        return _skinny_run(x, m, bn, slope, False)
-    if _flat_conv_supported(x, m):
-        return _flat_run((x,), m, bn, slope, False)
-    if _conv_k4s2_supported(x, m):
-        return _conv_k4s2(x, m, bn, slope, operands)
-    if _conv_k4s2_s2d_supported(x, m):
-        return _conv_k4s2_s2d(x, m, bn, slope)
-    if not _conv_k8s2_supported(x, m):
-        return None
-    if MERGE_PARITIES and m.out_channels <= 20 and all(v % 64 == 0 for v in x.shape[3:]) and x.shape[2] % 4 == 0:
-        # 4x space-to-depth: 3 taps over 64*Cin channels, the 8 output classes of the 2x finer grid merged along N
-        aff = _affine(m, bn, 20, x.device)
-        if aff is None:
-            return None
-        g, b, cout = _group(), x.shape[0], m.out_channels
-        split_z = S4D_SPLIT_Z or _x2() or _x3()   # f16x2 / fp32x3 double the accumulator columns: 8 classes x 20 x 2 = 320 > 256
-        wpack = _pack(m, ("k8s2_s4d", 20, g, split_z), lambda wt: pack_conv_k8s2_s4d_weights(wt, 20, g, split_z),
-                      2 if split_z else 1)
-        if _x2_direct(x):
-            xb = space_to_depth4_blocked(x, 16, torch.float16)
-        else:
-            xb = _finish_operand(space_to_depth4_blocked(x, _act_group(), torch.float16 if _f16() else None))
-        bd, cg, h, w, _ = xb.shape
-        cgo = (cout + 3) // 4
-        # operand outputs: output class q at coarse position j is enc2's parity sub-volume q at j
-        act, dst = _operand_request(operands, (b, cout, 2 * (bd // b), 2 * h, 2 * w), x.device)
-        out = torch.empty((bd * 2, cgo, 2 * h, 2 * w, 4), device=x.device, dtype=torch.float32) if act is None else None
-        _lib.call("genre_b200_conv3d_k8s2_s4d_forward", xb.data_ptr(), cg // _parts(), b, bd // b, h, w, wpack.data_ptr(),
-                  80 if split_z else 160, _op_flag(), aff[0].data_ptr(), aff[1].data_ptr(), 1.0 if slope is None else float(slope),
-                  out.data_ptr() if out is not None else None, cgo, *dst, _lib.stream_ptr(x))
-        return from_blocked(out, b, cout) if act is None else act
-    cout, npad = m.out_channels, 32
-    aff = _affine(m, bn, npad, x.device)
-    if aff is None:
-        return None
-    sc, sh = aff
-    dev = x.device
-    if _x2_direct(x):
-        xb = space_to_depth_blocked(x, 16, torch.float16)
-    else:
-        xb = _finish_operand(space_to_depth_blocked(x, 8, torch.float16) if _f16() else space_to_depth_blocked(x))
-    b = x.shape[0]
-    bd, cg, h, w, _ = xb.shape
-    cgo = (cout + 3) // 4
-    out = torch.empty((bd, cgo, h, w, 4), device=dev, dtype=torch.float32)
-    _lib.call("genre_b200_conv3d_taps_forward", xb.data_ptr(), cg // _parts(), None, 0, b, bd // b, h, w,
-              _packed_conv(m, npad).data_ptr(), 5, 2, npad, _op_flag(), sc.data_ptr(), sh.data_ptr(),
-              1.0 if slope is None else float(slope), out.data_ptr(), cgo, _lib.stream_ptr(x))
-    return from_blocked(out, b, cout)
-
-
 def _operand_of(x):
-    """blocked operand of the tensor-core kernels for activation x (NCDHW tensor, BlockedActivation or OperandActivation) in
+    """blocked operand of the tensor-core kernels for activation x (NCDHW tensor or OperandActivation) in
     the current PRECISION, reusing the fp32 blocked twin a previous custom layer left behind; (operand, padded channels) or None"""
     if isinstance(x, OperandActivation):
         return x.operand(PLAIN, -(-x.shape[1] // 8) * 8)
@@ -1467,26 +1372,29 @@ def _operand_of(x):
     return (to_blocked(x, 8, torch.float16), c) if c % 8 == 0 else None
 
 
+def _convt_c1_operands_ok(srcs, m, kstep):
+    """ConvTranspose3d(Cin -> 1, k4, s2, p1) over <= 2 sources of one extent whose _operand_of operands fill whole K steps"""
+    s0, cpads = srcs[0][0], [_operand_cpad(s) for s in srcs]
+    return (ENABLED and _geometry(m) == _CONVT_K4S2 and m.out_channels == 1 and len(srcs) <= 2
+            and all(s[2:] == s0[2:] for s, _ in srcs) and None not in cpads and sum(cpads) % kstep == 0)
+
+
+def _convt_c1_tc_supported(srcs, m):
+    """the 1-channel layer on the tensor cores (MODE 4) over the channel concatenation of the sources"""
+    s0 = srcs[0][0]
+    # fp32 wanted: the FP32-pipe stencil (csrc/convt_c1.cu) is exact and, measured, faster than the split-operand MMAs once
+    # the operand split of its two 336 MB sources is paid (Unet_3D.dec6: 1.33 vs 1.79 ms at B=16)
+    return ("convt_c1_tc" in POLICY and _mode() in ("f16", "tf32") and _convt_c1_operands_ok(srcs, m, 2 * _group())
+            and s0[4] in (16, 32, 64) and s0[3] % 16 == 0)
+
+
 def convt_c1_tc(inputs, m, sigmoid=False):
-    """ConvTranspose3d(Cin -> 1, k4, s2, p1) over the channel concatenation of `inputs` on the tensor cores (MODE 4);
-    NCDHW [B,1,2D,2H,2W] or None if not covered."""
+    """ConvTranspose3d(Cin -> 1, k4, s2, p1) over the channel concatenation of `inputs` on the tensor cores (MODE 4), on
+    the shapes _convt_c1_tc_supported accepts; NCDHW [B,1,2D,2H,2W]."""
     x0 = inputs[0]
-    if _x3() or _x2():
-        return None   # fp32 wanted: the FP32-pipe stencil (csrc/convt_c1.cu) is exact and, measured, faster than the split-operand
-                      # MMAs once the operand split of its two 336 MB sources is paid (Unet_3D.dec6: 1.33 vs 1.79 ms at B=16)
-    if not ("convt_c1_tc" in POLICY and ENABLED and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
-            and tuple(m.padding) == (1, 1, 1) and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1)
-            and m.groups == 1 and m.out_channels == 1 and len(inputs) <= 2
-            and all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 5 and t.shape[2:] == x0.shape[2:] for t in inputs)
-            and x0.shape[4] in (16, 32, 64) and x0.shape[3] % 16 == 0 and _no_autograd(*inputs, m.weight, m.bias)):
-        return None
     ops = [_operand_of(t) for t in inputs]
-    if any(o is None for o in ops):
-        return None
     g = _group()
     segments = tuple((t.shape[1], o[1]) for t, o in zip(inputs, ops))
-    if sum(pc for _, pc in segments) % (2 * g) != 0:
-        return None
     wpack = _pack(m, ("c1_tc", segments, g), lambda wt: pack_convt_c1_tc_weights(wt, segments, g), 1)
     b, _, d, h, w = x0.shape
     if m.bias is not None:
@@ -1508,27 +1416,19 @@ def convt_c1_tc(inputs, m, sigmoid=False):
 C2I_MAX_KSTEPS = {"f16x2": 40, "f16": 85}
 
 
-def _convt_c1_col2im_supported(inputs, m):
-    x0 = inputs[0]
-    return ("convt_c1_col2im" in POLICY and sum(-(-t.shape[1] // 8) * 8 for t in inputs) <= 16 * C2I_MAX_KSTEPS.get(_mode(), 0) and ENABLED and (_f16() or _x2()) and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2)
-            and tuple(m.padding) == (1, 1, 1) and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1)
-            and m.groups == 1 and m.out_channels == 1 and len(inputs) <= 2
-            and all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 5 and t.shape[2:] == x0.shape[2:] for t in inputs)
-            and x0.shape[4] == 64 and x0.shape[3] % 8 == 0 and x0.shape[0] <= 65535 and _no_autograd(*inputs, m.weight, m.bias))
+def _convt_c1_col2im_supported(srcs, m):
+    s0 = srcs[0][0]
+    return ("convt_c1_col2im" in POLICY and (_f16() or _x2()) and _convt_c1_operands_ok(srcs, m, 16)
+            and sum(-(-s[1] // 8) * 8 for s, _ in srcs) <= 16 * C2I_MAX_KSTEPS.get(_mode(), 0)
+            and s0[4] == 64 and s0[3] % 8 == 0 and s0[0] <= 65535)
 
 
 def convt_c1_col2im(inputs, m):
     """ConvTranspose3d(Cin -> 1, k4, s2, p1) over the channel concatenation of `inputs` on 64-wide volumes: tap GEMM + col2im
-    (csrc/convt_c1_col2im.cu); NCDHW [B,1,2D,2H,128] or None if not covered."""
+    (csrc/convt_c1_col2im.cu), on the shapes _convt_c1_col2im_supported accepts; NCDHW [B,1,2D,2H,128]."""
     x0 = inputs[0]
-    if not _convt_c1_col2im_supported(inputs, m):
-        return None
     ops = [_operand_of(t) for t in inputs]
-    if any(o is None for o in ops):
-        return None
     segments = tuple((t.shape[1], o[1]) for t, o in zip(inputs, ops))
-    if sum(pc for _, pc in segments) % 16 != 0:
-        return None
     wpack = _pack(m, ("c1_col2im", segments, 8), lambda wt: pack_convt_c1_col2im_weights(wt, segments), 0)
     b, _, d, h, w = x0.shape
     if m.bias is not None:
@@ -1549,13 +1449,9 @@ def _has_blocked(x):
     return _cached_blocked(x) is not None
 
 
-def _convt_c1_supported(cin, shape_dhw, m, inputs=()):
-    if "convt_c1" not in POLICY:
-        return False
-    if "convt_c1_convert" not in POLICY and not all(_has_blocked(t) for t in inputs):
-        return False
-    return (ENABLED and tuple(m.kernel_size) == (4, 4, 4) and tuple(m.stride) == (2, 2, 2) and tuple(m.padding) == (1, 1, 1)
-            and tuple(m.output_padding) == (0, 0, 0) and tuple(m.dilation) == (1, 1, 1) and m.groups == 1
+def _convt_c1_supported(cin, shape_dhw, m, twins=True):
+    """the FP32-pipe stencil (csrc/convt_c1.cu); twins: every source carries its fp32 blocked twin (else "convt_c1_convert")"""
+    return ("convt_c1" in POLICY and ("convt_c1_convert" in POLICY or twins) and ENABLED and _geometry(m) == _CONVT_K4S2
             and m.out_channels == 1 and cin % 4 == 0 and cin <= C1_MAX_CIN and shape_dhw[2] % 4 == 0)
 
 
@@ -1578,34 +1474,171 @@ def convt_c1(src0, src1, batch, m):
     return out
 
 
+# ---- routing: the kernel each entry point runs, decided from the layer's geometry and its sources' shapes ---------------------
+def _geometry(m):
+    """(transposed, kernel, stride, padding, output_padding, dilation, groups, padding_mode) of a Conv3d / ConvTranspose3d"""
+    return (isinstance(m, torch.nn.ConvTranspose3d), tuple(m.kernel_size), tuple(m.stride), tuple(m.padding),
+            tuple(m.output_padding), tuple(m.dilation), m.groups, m.padding_mode)
+
+
+# the stride-2 geometries of the halo and flat kernels: k 4 padding 1, k 8 padding 3
+_CONV_K4S2, _CONV_K8S2, _CONVT_K4S2, _CONVT_K8S2 = (
+    (t, (k,) * 3, (2,) * 3, (k // 2 - 1,) * 3, (0,) * 3, (1,) * 3, 1, "zeros") for t in (False, True) for k in (4, 8))
+
+
+def _source(x):
+    """(shape, kind) of an activation, as routes read it: kind operand (OperandActivation), twin (blocked twin) or plain"""
+    if isinstance(x, OperandActivation):
+        return tuple(x.shape), "operand"
+    return tuple(x.shape), "twin" if _has_blocked(x) else "plain"
+
+
+def _fp32_source(x):
+    return x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
+
+
+def _operand_cpad(src):
+    """channels (padded to whole groups) of the operand _operand_of builds for a source (shape, kind), or None: it has none"""
+    (shape, kind), g = src, _group()
+    if kind == "plain" and shape[1] % _act_group():
+        return None
+    return -(-shape[1] // g) * g
+
+
+def _batch_stats(bn):
+    return bn is not None and (bn.training or not bn.track_running_stats)
+
+
+def _conv_route(m, src, bn=None, slope=False, grad=False):
+    """the kernel conv3d(x, m, bn, slope) runs for src = _source(x), grad = _needs_grad(x, m.weight, m.bias): a POLICY key,
+    "train_forward" (_ConvForward: custom forward, cuDNN backward) or None (not covered)"""
+    shape, kind = src
+    if grad:    # fused epilogues are inference-only; the caller falls back to module-by-module
+        covered = (_conv_k4s2_supported(shape, m) or _conv_k8s2_supported(shape, m) or _conv_k4s2_s2d_supported(shape, m))
+        return "train_forward" if TRAIN_FORWARD and bn is None and not slope and covered else None
+    if not _inference(grad) or _batch_stats(bn):
+        return None
+    if (kind != "operand" and _skinny_ok(m, False) and shape[2:] == tuple(m.kernel_size) and shape[1] == m.in_channels
+            and (shape[1] * shape[2] * shape[3] * shape[4]) % 4 == 0):     # the kernel covers the whole input
+        return "skinny"
+    if (_flat_common(m) and _geometry(m) == _CONV_K4S2 and shape[1] % 16 == 0 and shape[1] == m.in_channels
+            and all(v % 2 == 0 for v in shape[2:]) and max(shape[2:]) <= 2 * FLAT_MAX):
+        return "flat"
+    if _conv_k4s2_supported(shape, m):
+        return "conv_k4s2"
+    if _conv_k4s2_s2d_supported(shape, m):
+        return "conv_k4s2_s2d"
+    if _conv_k8s2_supported(shape, m):
+        return "conv_k8s2"
+    return None
+
+
+def _convt_route(m, srcs, bn=None, slope=False, grad=False, sigmoid=False):
+    """as _conv_route, for conv_transpose3d (srcs = [_source(x)], under autograd also "convt_c1_train"), deconv_skip
+    (srcs = [_source(x), _source(skip)]) and fused_block's ConvTranspose3d -> Sigmoid (sigmoid)"""
+    shapes = [s for s, _ in srcs]
+    s0 = shapes[0]
+    cat = (s0[0], sum(s[1] for s in shapes)) + s0[2:]
+    plain = bn is None and not slope and not sigmoid
+    if grad:
+        if len(srcs) > 1 or not (plain and TRAIN_FORWARD):
+            return None
+        if _convt_c1_train_supported(s0, m):
+            return "convt_c1_train"
+        return "train_forward" if m.out_channels > 1 and _convt_supported(s0, m) else None
+    if _batch_stats(bn):
+        return None
+    inference, same = _inference(grad), all(s[2:] == s0[2:] for s in shapes)
+    if sigmoid:     # VoxelGenerator's last stage: ConvT(-> 1 channel) -> Sigmoid, on the tensor cores or not at all
+        return "convt_c1_tc" if inference and bn is None and _convt_c1_tc_supported(srcs, m) else None
+    if inference and plain and m.out_channels == 1:
+        if _convt_c1_col2im_supported(srcs, m):
+            return "convt_c1_col2im"
+        if _convt_c1_tc_supported(srcs, m):
+            return "convt_c1_tc"
+        if (same and all(s[1] % 4 == 0 for s in shapes)
+                and _convt_c1_supported(cat[1], s0[2:], m, all(k == "twin" for _, k in srcs))):
+            return "convt_c1"
+    if all(k != "operand" for _, k in srcs) and same and s0[2:] == (1, 1, 1):     # output = kernel weighted by the input
+        if (_skinny_ok(m, True) and cat[1] == m.in_channels
+                and (m.out_channels * m.kernel_size[0] * m.kernel_size[1] * m.kernel_size[2]) % 4 == 0):
+            return "skinny"
+        if len(srcs) > 1:
+            return None     # a concatenation of 1^3 sources runs on the skinny kernel or not at all
+    if not inference:
+        return None
+    if (_flat_common(m) and _geometry(m) == _CONVT_K4S2 and max(s0[2:]) <= FLAT_MAX and cat[1] == m.in_channels
+            and all(s[1] % 8 == 0 and s[2:] == s0[2:] and s[0] == s0[0] for s in shapes)):
+        return "flat"
+    if same and all(s[1] % _group() == 0 for s in shapes) and _convt_supported(cat, m):
+        return "convt_k8" if m.kernel_size[0] == 8 else "convt_k4"
+    return None
+
+
+_OPERAND_READERS = ("conv_k4s2", "convt_c1_col2im", "convt_c1_tc", "convt_k4", "convt_k8")   # read an OperandActivation
+
+
+def conv3d(x, m, bn=None, slope=None, operands=None):
+    """Conv3d on the tensor-core kernel [+ folded eval BatchNorm3d + LeakyReLU]: k=8,s=2,p=3 on few input channels
+    (Unet_3D.enc1) via space-to-depth, or k=4,s=2,p=1 (discriminator, Unet_3D.enc2/enc3) via parity sub-volumes.
+    operands: [(layout, cpad)] of the consumers (conv_operand_layout / deconv_operand_layout): enc1 and the k4 s2 layers then
+    return the output as an OperandActivation."""
+    if not _fp32_source(x):
+        return None
+    route = _conv_route(m, _source(x), bn, slope is not None, _needs_grad(x, m.weight, m.bias))
+    if route not in _OPERAND_READERS:
+        _fp32_only(x)
+    if route == "train_forward":
+        return _train_forward(x, m)
+    if route == "skinny":
+        return _skinny_run(x, m, bn, slope, False)
+    if route == "flat":
+        return _flat_run((x,), m, bn, slope, False)
+    if route == "conv_k4s2":
+        return _conv_k4s2(x, m, bn, slope, operands)
+    if route == "conv_k4s2_s2d":
+        return _conv_k4s2_s2d(x, m, bn, slope)
+    if route == "conv_k8s2" and _conv_k8s2_s4d_form(x.shape, m):
+        return _conv_k8s2_s4d(x, m, bn, slope, operands)
+    return _conv_k8s2_taps(x, m, bn, slope) if route == "conv_k8s2" else None
+
+
+def _launch_convt(route, srcs, m, bn, slope, operands=None):
+    """run a ConvTranspose3d route of conv_transpose3d / deconv_skip over the channel concatenation of srcs"""
+    if route not in _OPERAND_READERS:
+        _fp32_only(*srcs)
+    if route == "convt_c1_col2im":
+        return convt_c1_col2im(srcs, m)
+    if route == "convt_c1_tc":
+        return convt_c1_tc(srcs, m)
+    if route == "skinny":
+        return _skinny_run(torch.cat(srcs, dim=1) if len(srcs) > 1 else srcs[0], m, bn, slope, True)
+    if route == "flat":
+        return _flat_run(srcs, m, bn, slope, True)
+    if route == "convt_c1":
+        return convt_c1(_blocked_f32(srcs[0]), _blocked_f32(srcs[1]) if len(srcs) > 1 else None, srcs[0].shape[0], m)
+    if route in ("convt_k4", "convt_k8"):
+        # the concatenation stays two K ranges (a K chunk of 2 channel groups may straddle them: the halo producer picks the
+        # source per channel group)
+        b = srcs[0].shape[0]
+        y = convt3d_s2_blocked(_to_operand(srcs[0]), _to_operand(srcs[1]) if len(srcs) > 1 else None, b, m, bn,
+                               1.0 if slope is None else slope, operands)
+        return y if y is None or isinstance(y, OperandActivation) else from_blocked(y, b, m.out_channels)
+    return None
+
+
 def conv_transpose3d(x, m, bn=None, slope=None):
     """ConvTranspose3d [-> eval-mode BatchNorm3d folded into the epilogue -> ReLU / LeakyReLU(slope)]; None if not covered
     (the caller then runs the plain modules)."""
     _fp32_only(x)
-    if x.is_cuda and not isinstance(x, BlockedActivation) and _needs_grad(x, m.weight, m.bias):
-        if bn is not None or slope is not None or x.dim() != 5:
-            return None
-        if TRAIN_FORWARD and _convt_c1_train_supported(x, m):
-            return _ConvTC1Train.apply(x, m.weight, m.bias, m)
-        return _train_forward(x, m, m.out_channels > 1 and _convt_supported(x.shape, m))
-    if bn is None and slope is None and m.out_channels == 1:
-        y = convt_c1_col2im((x,), m)
-        if y is None:
-            y = convt_c1_tc((x,), m)
-        if y is not None:
-            return y
-    if _skinny_convt_supported(x, m):
-        return _skinny_run(x, m, bn, slope, True)
-    if _flat_convt_supported((x,), m):
-        return _flat_run((x,), m, bn, slope, True)
-    if (bn is None and slope is None and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5
-            and _convt_c1_supported(x.shape[1], x.shape[2:], m, (x,)) and _no_autograd(x, m.weight, m.bias)):
-        return convt_c1(_blocked_f32(x), None, x.shape[0], m)
-    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and _convt_supported(x.shape, m)
-            and _no_autograd(x, m.weight, m.bias)):
+    if not _fp32_source(x):
         return None
-    y = convt3d_s2_blocked(_to_operand(x), None, x.shape[0], m, bn, 1.0 if slope is None else slope)
-    return None if y is None else from_blocked(y, x.shape[0], m.out_channels)
+    route = _convt_route(m, [_source(x)], bn, slope is not None, _needs_grad(x, m.weight, m.bias))
+    if route == "convt_c1_train":
+        return _ConvTC1Train.apply(x, m.weight, m.bias, m)
+    if route == "train_forward":
+        return _train_forward(x, m)
+    return _launch_convt(route, (x,), m, bn, slope)
 
 
 # ---- BatchNorm3d with batch statistics + activation, training mode (csrc/bn_train.cu) --------------------------------
@@ -1693,54 +1726,19 @@ def gemm_conv(x, m):
 def fused_block(x, conv, bn, act):
     """conv [-> BatchNorm3d] -> ReLU/LeakyReLU as ONE kernel launch when the conv has a custom kernel: the normalisation
     and activation passes over the activation (0.9 ms of VoxelGenerator's 64^3 stage at B=16) disappear into the epilogue."""
-    if isinstance(act, torch.nn.Sigmoid):   # VoxelGenerator's last stage: ConvT(-> 1 channel) -> Sigmoid
-        return convt_c1_tc((x,), conv, sigmoid=True) if bn is None and isinstance(conv, torch.nn.ConvTranspose3d) else None
+    if isinstance(act, torch.nn.Sigmoid):
+        route = _convt_route(conv, [_source(x)], bn, False, _needs_grad(x, conv.weight, conv.bias), sigmoid=True)
+        return convt_c1_tc((x,), conv, sigmoid=True) if _fp32_source(x) and route == "convt_c1_tc" else None
     slope = 0.0 if isinstance(act, torch.nn.ReLU) else float(act.negative_slope)
     if isinstance(conv, torch.nn.ConvTranspose3d):
         return conv_transpose3d(x, conv, bn, slope)
     return conv3d(x, conv, bn, slope)
 
 
-def _deconv_kernel_supported(x, skip, conv):
-    """deconv_skip's condition for the halo kernel (convt3d_s2_blocked)"""
-    return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and skip.shape[2:] == x.shape[2:]
-            and x.shape[1] % _group() == 0 and skip.shape[1] % _group() == 0
-            and _convt_supported((x.shape[0], x.shape[1] + skip.shape[1]) + tuple(x.shape[2:]), conv)
-            and _no_autograd(x, skip, conv.weight, conv.bias))
-
-
 def deconv_skip(x, skip, conv, bn=None, slope=None, operands=None):
     """cat(x, skip) -> ConvTranspose3d [-> eval-mode BatchNorm3d folded into the epilogue -> LeakyReLU(slope)] with the
     concatenation walked as two K ranges instead of being materialised.  None if not covered.  operands: as conv3d's."""
-    if bn is None and conv.out_channels == 1:
-        y = convt_c1_col2im((x, skip), conv)
-        if y is None:
-            y = convt_c1_tc((x, skip), conv)
-        if y is not None:
-            return y
-    if (bn is None and x.is_cuda and x.dtype == torch.float32 and x.dim() == 5 and skip.shape[2:] == x.shape[2:]
-            and x.shape[1] % 4 == 0 and skip.shape[1] % 4 == 0
-            and _convt_c1_supported(x.shape[1] + skip.shape[1], x.shape[2:], conv, (x, skip))
-            and _no_autograd(x, skip, conv.weight, conv.bias)):
-        return convt_c1(_blocked_f32(x), _blocked_f32(skip), x.shape[0], conv)
-    if isinstance(x, BlockedActivation):
-        x = x.ncdhw()
-    if (torch.is_tensor(skip) and skip.dim() == 5 and tuple(skip.shape[2:]) == (1, 1, 1) and torch.is_tensor(x) and x.dim() == 5
-            and tuple(x.shape[2:]) == (1, 1, 1)):
-        xc = torch.cat((x, skip), dim=1)
-        return _skinny_run(xc, conv, bn, slope, True) if _skinny_convt_supported(xc, conv) else None
-    if _flat_convt_supported((x, skip), conv):
-        return _flat_run((x, skip), conv, bn, slope, True)
-    if not _deconv_kernel_supported(x, skip, conv):
-        _fp32_only(x, skip)
+    if not (_fp32_source(x) and _fp32_source(skip)):
         return None
-    if bn is not None and (bn.training or not bn.track_running_stats):
-        _fp32_only(x, skip)
-        return None  # batch statistics need the un-normalised output first
-    # the concatenation stays two K ranges (a K chunk of 2 channel groups may straddle them: the halo producer picks the
-    # source per channel group)
-    a, bsrc = _to_operand(x), _to_operand(skip)
-    y = convt3d_s2_blocked(a, bsrc, x.shape[0], conv, bn, 1.0 if slope is None else slope, operands)
-    if isinstance(y, OperandActivation):
-        return y
-    return from_blocked(y, x.shape[0], conv.out_channels)
+    route = _convt_route(conv, [_source(x), _source(skip)], bn, slope is not None, _needs_grad(x, skip, conv.weight, conv.bias))
+    return _launch_convt(route, (x, skip), conv, bn, slope, operands)

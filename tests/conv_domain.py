@@ -17,6 +17,7 @@ z taps x ceil(K / step) x (y, x) taps of its configuration: T x T per parity cla
 (MODE 2), the 4 x 4 paired taps (MODE 5), 3 x 3 over space-to-depth (MODE 3 and the taps forms).
 """
 import infer_ref as R
+from genre_shapehd_b200.ops_conv import PARITY, PLAIN
 
 MODES_HALO = ("f16x2", "f16", "fp32x3", "tf32")
 MODES_FP16 = ("f16x2", "f16")
@@ -256,6 +257,53 @@ CASE_IDS = [c.name for c in CASES]
 
 def case(name):
     return next(c for c in CASES if c.name == name)
+
+
+# ---- route boundaries: the nearest shapes each predicate rejects -------------------------------------------------------
+BOUNDARIES = [   # (name, transposed, cin, cout, k, s, p, input shape, modes)
+    ("convt_k4 W = 48", True, 16, 8, 4, 2, 1, (1, 16, 1, 16, 48), MODES_FP16),
+    ("convt_k4 H = 24", True, 16, 8, 4, 2, 1, (1, 16, 1, 24, 16), MODES_FP16),
+    ("convt_k4 Cout 65", True, 16, 65, 4, 2, 1, (1, 16, 1, 16, 16), MODES_FP16),
+    ("convt_k8 Cout 65", True, 16, 65, 8, 2, 3, (1, 16, 1, 16, 16), MODES_FP16),
+    ("k4s2 Cin 7", False, 7, 32, 4, 2, 1, (1, 7, 2, 32, 32), MODES_FP16),
+    ("k4s2 Cout 129", False, 16, 129, 4, 2, 1, (1, 16, 2, 32, 32), MODES_FP16),
+    ("k4s2 W' = 64", False, 16, 32, 4, 2, 1, (1, 16, 2, 32, 128), MODES_FP16),
+    ("k8s2 Cin 10", False, 10, 8, 8, 2, 3, (1, 10, 2, 32, 32), MODES_FP16),
+    ("k8s2 Cout 33", False, 2, 33, 8, 2, 3, (1, 2, 2, 32, 32), MODES_FP16),
+    ("k4s2 s2d Cout 65", False, 1, 65, 4, 2, 1, (1, 1, 2, 32, 32), MODES_FP16),
+    ("k4s2 s2d Cin 3", False, 3, 64, 4, 2, 1, (1, 3, 2, 32, 32), MODES_FP16),
+    ("flat convt extent 9", True, 16, 8, 4, 2, 1, (1, 16, 2, 2, 9), MODES_FP16),
+    ("flat conv extent 18", False, 16, 8, 4, 2, 1, (1, 16, 2, 2, 18), MODES_FP16),
+    ("flat conv Cin 8", False, 8, 8, 4, 2, 1, (1, 8, 4, 4, 4), MODES_FP16),
+    ("flat convt Cout 7", True, 16, 7, 4, 2, 1, (1, 16, 4, 4, 4), MODES_FP16),
+    ("col2im Cin 656 (41 K steps)", True, 656, 1, 4, 2, 1, (1, 656, 1, 8, 64), ("f16x2",)),
+    ("col2im Cin 1376 (86 K steps)", True, 1376, 1, 4, 2, 1, (1, 1376, 1, 8, 64), ("f16",)),
+    ("c1_tc W = 128 Cin 56", True, 56, 1, 4, 2, 1, (1, 56, 1, 16, 128), MODES_FP16),
+    ("col2im H = 12 Cin 56", True, 56, 1, 4, 2, 1, (1, 56, 1, 12, 64), MODES_FP16),
+    ("convt_c1 Cin 52", True, 52, 1, 4, 2, 1, (1, 52, 1, 8, 20), MODES_FP16),
+    ("convt_c1 Cin 6", True, 6, 1, 4, 2, 1, (1, 6, 1, 8, 20), MODES_FP16),
+    ("convt_c1 W = 18", True, 8, 1, 4, 2, 1, (1, 8, 1, 8, 18), MODES_FP16),
+    ("skinny K % 4", False, 3, 4, 1, 1, 0, (1, 3, 1, 1, 1), MODES_FP16),
+    ("skinny kernel < input", False, 8, 4, 4, 1, 0, (1, 8, 5, 5, 5), MODES_FP16),
+]
+
+# ---- operand outputs off the nets' shapes ------------------------------------------------------------------------------
+# (name, producer, module arguments, source shapes, requested operands): two shapes per producer at odd B and depths
+# Unet_3D does not use; D odd where the layout allows it (a Conv3d k4 s2 output; the parity layout needs even extents)
+OPERAND_CASES = [
+    ("s4d B3 D4 64x64 c2->12", "block", (2, 12, 8, 2, 3), [(3, 2, 4, 64, 64)], [(PARITY, 16), (PLAIN, 16)]),
+    ("s4d B5 D8 64x128 c4->20", "block", (4, 20, 8, 2, 3), [(5, 4, 8, 64, 128)], [(PLAIN, 24), (PARITY, 32)]),
+    ("k4s2 B3 D6 32x64 c20->40 (output D 3)", "block", (20, 40, 4, 2, 1), [(3, 20, 6, 32, 64)], [(PLAIN, 40)]),
+    ("k4s2 B5 D4 32x32 c24->36", "block", (24, 36, 4, 2, 1), [(5, 24, 4, 32, 32)], [(PARITY, 48), (PLAIN, 40)]),
+    ("convt_k4 B3 D3 16x16 skip 16+16->24", "skip", (32, 24, 4, 2, 1), [(3, 16, 3, 16, 16)] * 2,
+     [(PLAIN, 24), (PARITY, 32)]),
+    ("convt_k4 B5 D1 32x32 skip 16+16->33", "skip", (32, 33, 4, 2, 1), [(5, 16, 1, 32, 32)] * 2,
+     [(PARITY, 48), (PLAIN, 40)]),
+    ("convt_k8 paired B3 D3 16x32 skip 8+8->20", "skip", (16, 20, 8, 2, 3), [(3, 8, 3, 16, 32)] * 2,
+     [(PLAIN, 24), (PARITY, 32)]),
+    ("convt_k8 paired B5 D1 32x16 skip 8+8->7", "skip", (16, 7, 8, 2, 3), [(5, 8, 1, 32, 16)] * 2,
+     [(PLAIN, 8), (PARITY, 16)]),
+]
 
 
 # ---- the C++ dispatch, restated -----------------------------------------------------------------------------------------

@@ -234,7 +234,7 @@ def test_fused_sequential_is_a_plain_sequential_on_cpu_and_keeps_state_dict_keys
     assert torch.equal(y, z)
 
 
-def test_blocked_twin_cache_semantics_on_cpu():
+def test_blocked_twin_is_reused_until_an_inplace_update_on_cpu():
     x = torch.randn(2, 8, 3, 4, 4)
     y = ops_conv.from_blocked(ops_conv.to_blocked(x, 4), 2, 8)
     assert torch.equal(y, x) and ops_conv._has_blocked(y)
@@ -242,9 +242,6 @@ def test_blocked_twin_cache_semantics_on_cpu():
     y.add_(1.0)                                              # in-place update: the twin is stale and must be ignored
     assert not ops_conv._has_blocked(y)
     assert torch.equal(ops_conv.from_blocked(ops_conv._blocked_f32(y), 2, 8), y)
-    act = ops_conv.BlockedActivation(ops_conv.to_blocked(x, 4), 2, 8)
-    assert tuple(act.shape) == (2, 8, 3, 4, 4) and act.dim() == 5 and act.size(1) == 8 and not act.requires_grad
-    assert torch.equal(act.ncdhw(), x)
 
 
 def test_operand_mode_selection():

@@ -74,7 +74,7 @@ def test_helpers_and_import_surface():
 def test_forward_matches_reference_on_gpu(name, mode):
     """CUDA path against the reference digests (recorded on CPU fp32).
     exact (the DEFAULT mode, under PyTorch's default allow_tf32 = True): the custom kernels run their fp32-accurate operand-split
-          scheme and the layers without a custom kernel are pinned to cuDNN fp32 (ops_conv.cudnn_precision): whole-net outputs
+          scheme and the layers without a custom kernel run ops_conv.exact_fallback's 3xTF32 split on cuDNN: whole-net outputs
           within 1e-4 (north_star) with the fp16 hi/lo split,
           3e-4 with the older 3xTF32 scheme (its accumulator truncation error grows with 3x the MMA steps);
     f16   (opt-in): single-pass fp16 operands, with the tolerance a 10-bit mantissa allows through a 12-layer network."""

@@ -42,6 +42,14 @@ _SIGNATURES = {
                                            _f32, _ptr, _ptr],
     "genre_b200_ray_consistency_backward": [_ptr, _i64, _int, _i64, _i64, _int, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i64, _i64,
                                             _f32, _ptr, _ptr, _ptr],
+    "genre_b200_render_views_forward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr,
+                                        _i64, _i64, _f32, _ptr, _ptr, _ptr],
+    "genre_b200_render_views_backward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr,
+                                         _i64, _i64, _f32, _ptr, _ptr, _ptr, _ptr],
+    "genre_b200_ray_consistency_views_forward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64,
+                                                 _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _f32, _ptr, _ptr],
+    "genre_b200_ray_consistency_views_backward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64,
+                                                  _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _f32, _ptr, _ptr, _ptr],
     "genre_b200_nnd_forward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_nnd_backward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_convt3d_s2_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr, _ptr,
@@ -123,7 +131,9 @@ _LAUNCHES = {
     "genre_b200_sph_bp_forward": 2, "genre_b200_sph_bp_backward": 1, "genre_b200_calc_prob_forward": 1,
     "genre_b200_calc_prob_backward": 1, "genre_b200_render_spherical_forward": 1,
     "genre_b200_render_spherical_backward": 1, "genre_b200_render_camera_forward": 1, "genre_b200_render_camera_backward": 1,
-    "genre_b200_ray_consistency_forward": 1, "genre_b200_ray_consistency_backward": 1, "genre_b200_nnd_forward": 1, "genre_b200_nnd_backward": 1,
+    "genre_b200_ray_consistency_forward": 1, "genre_b200_ray_consistency_backward": 1,
+    "genre_b200_render_views_forward": 1, "genre_b200_render_views_backward": 1,
+    "genre_b200_ray_consistency_views_forward": 1, "genre_b200_ray_consistency_views_backward": 1, "genre_b200_nnd_forward": 1, "genre_b200_nnd_backward": 1,
     "genre_b200_cam_bp_stage_project": 1, "genre_b200_voxelize_stage_splat": 1,
     "genre_b200_convt3d_s2_forward": 1, "genre_b200_conv3d_taps_forward": 1,
     "genre_b200_convt_c1_forward": 1, "genre_b200_conv3d_k4s2_forward": 1,

@@ -27,6 +27,18 @@
 //     g   = (t*ux - cam_dist, t*uy, t*uz);   f = (g + 0.5) * R - 0.5
 // then f and t are each rounded once to fp32.  fl and cam_dist are the fp32 inputs widened exactly.  Everything after is
 // fp32.
+//
+// Posed views (the *_views entry points): rays over [N, V, H, W], all V views of grid n reading vox[n] (the backward's
+// atomics sum the views' gradients into it).  View (n, v) has a rotation rot (3x3 row-major, its columns the camera's
+// axes in the grid frame), an eye e and fl; pixel (h, w) keeps the camera-frame u above, and the ray is, in the same
+// fp64 arithmetic,
+//     u'_i = (rot[i][0]*ux + rot[i][1]*uy) + rot[i][2]*uz;   d = sqrt((ex*ex + ey*ey) + ez*ez)
+//     t    = (d - sqrt(3)/2) + k * (sqrt(3) / (Z - 1));      g = (t*u'x + ex, t*u'y + ey, t*u'z + ez)
+// With rot = I and e = (-cam_dist, 0, 0) every value equals the fixed camera's bit for bit (products by 1 are exact,
+// products by 0 add a signed zero, and the square root of a widened fp32 square is exact).  The fixed camera is the
+// POSED = false instantiation of the same templates, with exactly the arithmetic above it.
+#include <initializer_list>
+
 #include "render.cuh"
 
 namespace gb {
@@ -43,10 +55,13 @@ constexpr double RC_HALF_SQRT3 = 0.8660254037844386;  // RC_SQRT3 / 2 (exact)
 enum { RC_RENDER = 0, RC_CONSISTENCY = 1 };
 
 struct CamRay {
-  double ux, uy, uz, cd, t0, dt;
+  double ux, uy, uz;  // direction (grid frame)
+  double ex, ey, ez;  // eye (the fixed camera uses ex = -cam_dist only)
+  double t0, dt;      // first sample's depth, spacing
 };
 
-__device__ __forceinline__ CamRay cam_ray(float fl, float cam_dist, int h, int w, int H, int W, int Z) {
+// pixel (h, w)'s camera-frame direction and the sample spacing
+__device__ __forceinline__ CamRay cam_dir(float fl, int h, int w, int H, int W, int Z) {
   const double f = (double)fl;
   const double imh = (double)h - 0.5 * (double)(H - 1), imw = (double)w - 0.5 * (double)(W - 1);  // exact
   const double nrm = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(f, f), __dmul_rn(imw, imw)), __dmul_rn(imh, imh)));
@@ -54,17 +69,46 @@ __device__ __forceinline__ CamRay cam_ray(float fl, float cam_dist, int h, int w
   r.ux = __ddiv_rn(f, nrm);
   r.uy = __ddiv_rn(-imw, nrm);
   r.uz = __ddiv_rn(-imh, nrm);
-  r.cd = (double)cam_dist;
-  r.t0 = __dadd_rn(r.cd, -RC_HALF_SQRT3);
   r.dt = Z > 1 ? __ddiv_rn(RC_SQRT3, (double)(Z - 1)) : 0.0;
   return r;
 }
 
+// the fixed camera at (-cam_dist, 0, 0) looking along +x
+__device__ __forceinline__ CamRay cam_ray(float fl, float cam_dist, int h, int w, int H, int W, int Z) {
+  CamRay r = cam_dir(fl, h, w, H, W, Z);
+  r.ex = -(double)cam_dist;
+  r.t0 = __dadd_rn((double)cam_dist, -RC_HALF_SQRT3);
+  return r;
+}
+
+// a posed view: rot [9] row-major, eye [3]
+__device__ __forceinline__ CamRay cam_ray_posed(float fl, const float *__restrict__ rot, const float *__restrict__ eye,
+                                                int h, int w, int H, int W, int Z) {
+  const CamRay c = cam_dir(fl, h, w, H, W, Z);
+  double m[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) m[i] = (double)__ldg(rot + i);
+  CamRay r;
+  r.ux = __dadd_rn(__dadd_rn(__dmul_rn(m[0], c.ux), __dmul_rn(m[1], c.uy)), __dmul_rn(m[2], c.uz));
+  r.uy = __dadd_rn(__dadd_rn(__dmul_rn(m[3], c.ux), __dmul_rn(m[4], c.uy)), __dmul_rn(m[5], c.uz));
+  r.uz = __dadd_rn(__dadd_rn(__dmul_rn(m[6], c.ux), __dmul_rn(m[7], c.uy)), __dmul_rn(m[8], c.uz));
+  r.ex = (double)__ldg(eye);
+  r.ey = (double)__ldg(eye + 1);
+  r.ez = (double)__ldg(eye + 2);
+  const double d = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(r.ex, r.ex), __dmul_rn(r.ey, r.ey)), __dmul_rn(r.ez, r.ez)));
+  r.t0 = __dadd_rn(d, -RC_HALF_SQRT3);
+  r.dt = c.dt;
+  return r;
+}
+
 // sample k of the ray: taps at its fp32 voxel coordinate, and its fp32 ray depth
+template <bool POSED>
 __device__ __forceinline__ float cam_sample(const CamRay &r, int k, int R, Taps &taps) {
   const double Rd = (double)R;
   const double t = __dadd_rn(r.t0, __dmul_rn((double)k, r.dt));
-  const double gx = __dadd_rn(__dmul_rn(t, r.ux), -r.cd), gy = __dmul_rn(t, r.uy), gz = __dmul_rn(t, r.uz);
+  const double gx = __dadd_rn(__dmul_rn(t, r.ux), r.ex);
+  const double gy = POSED ? __dadd_rn(__dmul_rn(t, r.uy), r.ey) : __dmul_rn(t, r.uy);
+  const double gz = POSED ? __dadd_rn(__dmul_rn(t, r.uz), r.ez) : __dmul_rn(t, r.uz);
   const float fx = (float)__dadd_rn(__dmul_rn(__dadd_rn(gx, 0.5), Rd), -0.5);
   const float fy = (float)__dadd_rn(__dmul_rn(__dadd_rn(gy, 0.5), Rd), -0.5);
   const float fz = (float)__dadd_rn(__dmul_rn(__dadd_rn(gz, 0.5), Rd), -0.5);
@@ -90,7 +134,7 @@ struct RayCost {
 // The forward walk: returns (sum_k s_k c_k, T_Z) to every lane.  With chunk_T, chunk c's carry (T before its first
 // sample) is stored there and *last_chunk is the last chunk walked; the walk stops once T underflows to 0 (every later
 // term, and every later gradient, is exactly 0).
-template <class Cost>
+template <bool POSED, class Cost>
 __device__ __forceinline__ void cam_walk(const float *__restrict__ vol, int R, const CamRay &ray, int Z, const Cost &cost,
                                          float &sum, float &trans, float *chunk_T, int *last_chunk) {
   const int lane = threadIdx.x & 31;
@@ -100,7 +144,7 @@ __device__ __forceinline__ void cam_walk(const float *__restrict__ vol, int R, c
     float p = 0.0f, ck = 0.0f;  // lanes past the end behave like p = 0 (factor 1, no contribution)
     if (k < Z) {
       Taps t;
-      ck = cost.at(cam_sample(ray, k, R, t));
+      ck = cost.at(cam_sample<POSED>(ray, k, R, t));
       p = fminf(fmaxf(sample_trilinear<false>(vol, t, R, VoxPre{}), RS_PMIN), RS_PMAX);
     }
     if (chunk_T) {
@@ -123,60 +167,83 @@ struct CamArgs {
   long long n_rays;
   const float *fl, *cd;
   long long fN, dN;
+  long long V;               // posed: views per grid (rays over [N,V,H,W])
+  const float *rot, *eye;    // posed: 9 and 3 contiguous floats per view, strides (rN, rV), (eN, eV); fl strides (fN, fV)
+  long long fV, rN, rV, eN, eV;
   float bg;                  // render: escape depth
-  const float *obs;          // consistency: observed ray depth [N,H,W], strides (oN, oH, oW)
-  long long oN, oH, oW;
+  const float *obs;          // consistency: observed ray depth [N,(V,)H,W], strides (oN, (oV,) oH, oW)
+  long long oN, oV, oH, oW;
   float miss;
-  const float *g0, *g1;      // backward: grad_depth, grad_silhou (render) or grad_loss (consistency), [N,H,W] dense
-  float *out0, *out1;        // forward: depth, silhou (render) or loss (consistency), [N,H,W] dense
+  const float *g0, *g1;      // backward: grad_depth, grad_silhou (render) or grad_loss (consistency), [N,(V,)H,W] dense
+  float *out0, *out1;        // forward: depth, silhou (render) or loss (consistency), [N,(V,)H,W] dense
   float *grad_vox;           // backward: [N,R,R,R] dense, accumulated
 };
 
 struct RayIndex {
-  long long n;
+  long long n, v;
   int h, w;
 };
 
+template <bool POSED>
 __device__ __forceinline__ RayIndex ray_index(const CamArgs &a, long long ray) {
   const long long hw = (long long)a.H * a.W;
   RayIndex ri;
-  ri.n = ray / hw;
-  const int pix = (int)(ray - ri.n * hw);
+  const long long nv = ray / hw;
+  const int pix = (int)(ray - nv * hw);
+  if (POSED) {
+    ri.n = nv / a.V;
+    ri.v = nv - ri.n * a.V;
+  } else {
+    ri.n = nv;
+    ri.v = 0;
+  }
   ri.h = pix / a.W;
   ri.w = pix - ri.h * a.W;
   return ri;
 }
 
-template <int MODE>
+template <bool POSED>
+__device__ __forceinline__ CamRay ray_of(const CamArgs &a, const RayIndex &ri) {
+  if (!POSED) return cam_ray(a.fl[ri.n * a.fN], a.cd[ri.n * a.dN], ri.h, ri.w, a.H, a.W, a.Z);
+  return cam_ray_posed(a.fl[ri.n * a.fN + ri.v * a.fV], a.rot + ri.n * a.rN + ri.v * a.rV, a.eye + ri.n * a.eN + ri.v * a.eV,
+                       ri.h, ri.w, a.H, a.W, a.Z);
+}
+
+template <bool POSED>
+__device__ __forceinline__ float obs_of(const CamArgs &a, const RayIndex &ri) {
+  return a.obs[ri.n * a.oN + (POSED ? ri.v * a.oV : 0) + ri.h * a.oH + ri.w * a.oW];
+}
+
+template <int MODE, bool POSED>
 __global__ void __launch_bounds__(RC_THREADS) render_camera_forward_kernel(const CamArgs a) {
   const long long ray = (long long)blockIdx.x * RC_WARPS + (threadIdx.x >> 5);
   if (ray >= a.n_rays) return;
-  const RayIndex ri = ray_index(a, ray);
+  const RayIndex ri = ray_index<POSED>(a, ray);
   const float *vol = a.vox + (size_t)ri.n * a.R * a.R * a.R;
-  const CamRay r = cam_ray(a.fl[ri.n * a.fN], a.cd[ri.n * a.dN], ri.h, ri.w, a.H, a.W, a.Z);
+  const CamRay r = ray_of<POSED>(a, ri);
   float sum, T;
   if (MODE == RC_RENDER) {
     const LinearCost cost{1.0f, 0.0f, a.bg};
-    cam_walk(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
+    cam_walk<POSED>(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
     if ((threadIdx.x & 31) == 0) {
       a.out0[ray] = fmaf(T, cost.esc(), sum);
       a.out1[ray] = 1.0f - T;
     }
   } else {
-    const RayCost cost{a.obs[ri.n * a.oN + ri.h * a.oH + ri.w * a.oW], a.miss};
-    cam_walk(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
+    const RayCost cost{obs_of<POSED>(a, ri), a.miss};
+    cam_walk<POSED>(vol, a.R, r, a.Z, cost, sum, T, nullptr, nullptr);
     if ((threadIdx.x & 31) == 0) a.out0[ray] = fmaf(T, cost.esc(), sum);
   }
 }
 
 // the two walks of one ray; `scale` multiplies every gradient (the consistency loss's upstream gradient)
-template <class Cost>
+template <bool POSED, class Cost>
 __device__ __forceinline__ void cam_backward_ray(const float *__restrict__ vol, float *__restrict__ gvol, int R,
                                                  const CamRay &ray, int Z, const Cost &cost, float scale, float *chunk_T) {
   const int lane = threadIdx.x & 31;
   float sum, T_Z;
   int last = 0;
-  cam_walk(vol, R, ray, Z, cost, sum, T_Z, chunk_T, &last);
+  cam_walk<POSED>(vol, R, ray, Z, cost, sum, T_Z, chunk_T, &last);
   __syncwarp();
   float suffix = T_Z * cost.esc();  // sum over the chunks already walked of s_j c_j, plus the escape term
   for (int c = last; c >= 0; --c) {
@@ -185,7 +252,7 @@ __device__ __forceinline__ void cam_backward_ray(const float *__restrict__ vol, 
     float raw = 0.0f, p = 0.0f, ck = 0.0f;
     Taps t;
     if (live) {
-      ck = cost.at(cam_sample(ray, k, R, t));
+      ck = cost.at(cam_sample<POSED>(ray, k, R, t));
       raw = sample_trilinear<false>(vol, t, R, VoxPre{});
       p = fminf(fmaxf(raw, RS_PMIN), RS_PMAX);
     }
@@ -205,47 +272,73 @@ __device__ __forceinline__ void cam_backward_ray(const float *__restrict__ vol, 
   }
 }
 
-template <int MODE>
+template <int MODE, bool POSED>
 __global__ void __launch_bounds__(RC_THREADS) render_camera_backward_kernel(const CamArgs a) {
   __shared__ float s_T[RC_WARPS][RC_MAX_CHUNKS];
   const int warp = threadIdx.x >> 5;
   const long long ray = (long long)blockIdx.x * RC_WARPS + warp;
   if (ray >= a.n_rays) return;
-  const RayIndex ri = ray_index(a, ray);
-  const size_t vol_off = (size_t)ri.n * a.R * a.R * a.R;
+  const RayIndex ri = ray_index<POSED>(a, ray);
+  const size_t vol_off = (size_t)ri.n * a.R * a.R * a.R;  // every view of grid n scatters into grad_vox[n]
   const float g0 = a.g0[ray], g1 = MODE == RC_RENDER ? a.g1[ray] : 0.0f;
   if (g0 == 0.0f && g1 == 0.0f) return;  // warp-uniform
-  const CamRay r = cam_ray(a.fl[ri.n * a.fN], a.cd[ri.n * a.dN], ri.h, ri.w, a.H, a.W, a.Z);
+  const CamRay r = ray_of<POSED>(a, ri);
   if (MODE == RC_RENDER)
-    cam_backward_ray(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z, LinearCost{g0, g1, g0 * a.bg}, 1.0f, s_T[warp]);
+    cam_backward_ray<POSED>(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z, LinearCost{g0, g1, g0 * a.bg}, 1.0f,
+                            s_T[warp]);
   else
-    cam_backward_ray(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z,
-                     RayCost{a.obs[ri.n * a.oN + ri.h * a.oH + ri.w * a.oW], a.miss}, g0, s_T[warp]);
+    cam_backward_ray<POSED>(a.vox + vol_off, a.grad_vox + vol_off, a.R, r, a.Z, RayCost{obs_of<POSED>(a, ri), a.miss}, g0,
+                            s_T[warp]);
 }
 
 static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
-static int rc_check(const char *what, const float *vox, int64_t N, int res, int64_t H, int64_t W, int Z, const float *fl,
-                    const float *cd, CamArgs &a) {
-  GB_REQUIRE(vox && fl && cd, GENRE_B200_EINVAL, "%s: null pointer", what);
+constexpr long long RC_MAX_RAYS = 1ll << 34;
+
+// the checks every entry point shares: rays over [N, V, H, W] (V = 1: the fixed camera), and the camera's pointers cams
+// (fl and camdist, or fl, rot and eye; named in cam_names)
+static int rc_check(const char *what, const float *vox, int64_t N, int64_t V, int res, int64_t H, int64_t W, int Z,
+                    std::initializer_list<const float *> cams, const char *cam_names, CamArgs &a) {
+  bool cams_set = true, cams_aligned = true;
+  for (const float *p : cams) {
+    cams_set = cams_set && p;
+    cams_aligned = cams_aligned && aligned4(p);
+  }
+  GB_REQUIRE(vox && cams_set, GENRE_B200_EINVAL, "%s: null pointer", what);
   GB_REQUIRE(res >= 2 && res <= RC_MAX_RES, GENRE_B200_EINVAL, "%s: resolution %d unsupported (2..%d)", what, res,
              RC_MAX_RES);
   GB_REQUIRE(H >= 1 && W >= 1 && H <= RC_MAX_HW && W <= RC_MAX_HW, GENRE_B200_EINVAL,
              "%s: image size %lld x %lld unsupported (1..%d per side)", what, (long long)H, (long long)W, RC_MAX_HW);
   GB_REQUIRE(Z >= 1 && Z <= RC_MAX_Z, GENRE_B200_EINVAL, "%s: z_res %d unsupported (1..%d)", what, Z, RC_MAX_Z);
-  GB_REQUIRE(N >= 1 && (N * H * W + RC_WARPS - 1) / RC_WARPS < (1ll << 31), GENRE_B200_EINVAL,
-             "%s: batch %lld unsupported (1 .. 2^34 / (H W) rays)", what, (long long)N);
-  GB_REQUIRE(aligned4(vox) && aligned4(fl) && aligned4(cd), GENRE_B200_EALIGN, "%s: vox, fl and camdist must be 4-byte aligned",
-             what);
+  GB_REQUIRE(V >= 1 && V <= RC_MAX_RAYS, GENRE_B200_EINVAL, "%s: %lld views unsupported (1 .. 2^34)", what, (long long)V);
+  GB_REQUIRE(N >= 1 && N <= RC_MAX_RAYS / V && (N * V * H * W + RC_WARPS - 1) / RC_WARPS < (1ll << 31), GENRE_B200_EINVAL,
+             "%s: batch %lld unsupported (1 .. 2^34 / (%sH W) rays)", what, (long long)N, V == 1 ? "" : "V ");
+  GB_REQUIRE(aligned4(vox) && cams_aligned, GENRE_B200_EALIGN, "%s: vox, %s must be 4-byte aligned", what, cam_names);
   a = CamArgs{};
   a.vox = vox;
   a.R = res;
   a.H = (int)H;
   a.W = (int)W;
   a.Z = Z;
-  a.n_rays = (long long)N * H * W;
+  a.V = V;
+  a.n_rays = (long long)N * V * H * W;
+  return 0;
+}
+
+// the posed views' checks and camera arguments
+static int rv_check(const char *what, const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int Z,
+                    const float *fl, int64_t fN, int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye,
+                    int64_t eN, int64_t eV, CamArgs &a) {
+  if (int rc = rc_check(what, vox, N, V, res, H, W, Z, {fl, rot, eye}, "fl, rot and eye", a)) return rc;
   a.fl = fl;
-  a.cd = cd;
+  a.fN = fN;
+  a.fV = fV;
+  a.rot = rot;
+  a.rN = rN;
+  a.rV = rV;
+  a.eye = eye;
+  a.eN = eN;
+  a.eV = eV;
   return 0;
 }
 
@@ -259,15 +352,17 @@ extern "C" int genre_b200_render_camera_forward(const float *vox, int64_t N, int
                                                 const float *fl, int64_t fN, const float *camdist, int64_t dN, float bg,
                                                 float *depth, float *silhou, void *stream) {
   CamArgs a;
-  if (int rc = rc_check("render_camera", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  if (int rc = rc_check("render_camera", vox, N, 1, res, H, W, z_res, {fl, camdist}, "fl and camdist", a)) return rc;
   GB_REQUIRE(depth && silhou, GENRE_B200_EINVAL, "render_camera: null output");
   GB_REQUIRE(aligned4(depth) && aligned4(silhou), GENRE_B200_EALIGN, "render_camera: outputs must be 4-byte aligned");
+  a.fl = fl;
+  a.cd = camdist;
   a.fN = fN;
   a.dN = dN;
   a.bg = bg;
   a.out0 = depth;
   a.out1 = silhou;
-  render_camera_forward_kernel<RC_RENDER><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  render_camera_forward_kernel<RC_RENDER, false><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
   return check_launch("render_camera forward kernel");
 }
 
@@ -276,17 +371,19 @@ extern "C" int genre_b200_render_camera_backward(const float *vox, int64_t N, in
                                                  const float *grad_depth, const float *grad_silhou, float *grad_vox,
                                                  void *stream) {
   CamArgs a;
-  if (int rc = rc_check("render_camera backward", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  if (int rc = rc_check("render_camera backward", vox, N, 1, res, H, W, z_res, {fl, camdist}, "fl and camdist", a)) return rc;
   GB_REQUIRE(grad_depth && grad_silhou && grad_vox, GENRE_B200_EINVAL, "render_camera backward: null pointer");
   GB_REQUIRE(aligned4(grad_depth) && aligned4(grad_silhou) && aligned4(grad_vox), GENRE_B200_EALIGN,
              "render_camera backward: gradients must be 4-byte aligned");
+  a.fl = fl;
+  a.cd = camdist;
   a.fN = fN;
   a.dN = dN;
   a.bg = bg;
   a.g0 = grad_depth;
   a.g1 = grad_silhou;
   a.grad_vox = grad_vox;
-  render_camera_backward_kernel<RC_RENDER><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  render_camera_backward_kernel<RC_RENDER, false><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
   return check_launch("render_camera backward kernel");
 }
 
@@ -295,9 +392,11 @@ extern "C" int genre_b200_ray_consistency_forward(const float *vox, int64_t N, i
                                                   const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
                                                   float *loss, void *stream) {
   CamArgs a;
-  if (int rc = rc_check("ray_consistency", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  if (int rc = rc_check("ray_consistency", vox, N, 1, res, H, W, z_res, {fl, camdist}, "fl and camdist", a)) return rc;
   GB_REQUIRE(obs && loss, GENRE_B200_EINVAL, "ray_consistency: null pointer");
   GB_REQUIRE(aligned4(obs) && aligned4(loss), GENRE_B200_EALIGN, "ray_consistency: obs and loss must be 4-byte aligned");
+  a.fl = fl;
+  a.cd = camdist;
   a.fN = fN;
   a.dN = dN;
   a.obs = obs;
@@ -306,7 +405,7 @@ extern "C" int genre_b200_ray_consistency_forward(const float *vox, int64_t N, i
   a.oW = oW;
   a.miss = miss_cost;
   a.out0 = loss;
-  render_camera_forward_kernel<RC_CONSISTENCY><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  render_camera_forward_kernel<RC_CONSISTENCY, false><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
   return check_launch("ray_consistency forward kernel");
 }
 
@@ -315,10 +414,12 @@ extern "C" int genre_b200_ray_consistency_backward(const float *vox, int64_t N, 
                                                    const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
                                                    const float *grad_loss, float *grad_vox, void *stream) {
   CamArgs a;
-  if (int rc = rc_check("ray_consistency backward", vox, N, res, H, W, z_res, fl, camdist, a)) return rc;
+  if (int rc = rc_check("ray_consistency backward", vox, N, 1, res, H, W, z_res, {fl, camdist}, "fl and camdist", a)) return rc;
   GB_REQUIRE(obs && grad_loss && grad_vox, GENRE_B200_EINVAL, "ray_consistency backward: null pointer");
   GB_REQUIRE(aligned4(obs) && aligned4(grad_loss) && aligned4(grad_vox), GENRE_B200_EALIGN,
              "ray_consistency backward: obs and gradients must be 4-byte aligned");
+  a.fl = fl;
+  a.cd = camdist;
   a.fN = fN;
   a.dN = dN;
   a.obs = obs;
@@ -328,6 +429,88 @@ extern "C" int genre_b200_ray_consistency_backward(const float *vox, int64_t N, 
   a.miss = miss_cost;
   a.g0 = grad_loss;
   a.grad_vox = grad_vox;
-  render_camera_backward_kernel<RC_CONSISTENCY><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  render_camera_backward_kernel<RC_CONSISTENCY, false><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
   return check_launch("ray_consistency backward kernel");
+}
+
+extern "C" int genre_b200_render_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                               int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                               int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, float bg,
+                                               float *depth, float *silhou, void *stream) {
+  CamArgs a;
+  if (int rc = rv_check("render_views", vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, a)) return rc;
+  GB_REQUIRE(depth && silhou, GENRE_B200_EINVAL, "render_views: null output");
+  GB_REQUIRE(aligned4(depth) && aligned4(silhou), GENRE_B200_EALIGN, "render_views: outputs must be 4-byte aligned");
+  a.bg = bg;
+  a.out0 = depth;
+  a.out1 = silhou;
+  render_camera_forward_kernel<RC_RENDER, true><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("render_views forward kernel");
+}
+
+extern "C" int genre_b200_render_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                                int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                                int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, float bg,
+                                                const float *grad_depth, const float *grad_silhou, float *grad_vox,
+                                                void *stream) {
+  CamArgs a;
+  if (int rc = rv_check("render_views backward", vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, a))
+    return rc;
+  GB_REQUIRE(grad_depth && grad_silhou && grad_vox, GENRE_B200_EINVAL, "render_views backward: null pointer");
+  GB_REQUIRE(aligned4(grad_depth) && aligned4(grad_silhou) && aligned4(grad_vox), GENRE_B200_EALIGN,
+             "render_views backward: gradients must be 4-byte aligned");
+  a.bg = bg;
+  a.g0 = grad_depth;
+  a.g1 = grad_silhou;
+  a.grad_vox = grad_vox;
+  render_camera_backward_kernel<RC_RENDER, true><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("render_views backward kernel");
+}
+
+extern "C" int genre_b200_ray_consistency_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                        int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                        const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                        int64_t eN, int64_t eV, const float *obs, int64_t oN, int64_t oV,
+                                                        int64_t oH, int64_t oW, float miss_cost, float *loss,
+                                                        void *stream) {
+  CamArgs a;
+  if (int rc = rv_check("ray_consistency_views", vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, a))
+    return rc;
+  GB_REQUIRE(obs && loss, GENRE_B200_EINVAL, "ray_consistency_views: null pointer");
+  GB_REQUIRE(aligned4(obs) && aligned4(loss), GENRE_B200_EALIGN,
+             "ray_consistency_views: obs and loss must be 4-byte aligned");
+  a.obs = obs;
+  a.oN = oN;
+  a.oV = oV;
+  a.oH = oH;
+  a.oW = oW;
+  a.miss = miss_cost;
+  a.out0 = loss;
+  render_camera_forward_kernel<RC_CONSISTENCY, true><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("ray_consistency_views forward kernel");
+}
+
+extern "C" int genre_b200_ray_consistency_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                         int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                         const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                         int64_t eN, int64_t eV, const float *obs, int64_t oN, int64_t oV,
+                                                         int64_t oH, int64_t oW, float miss_cost, const float *grad_loss,
+                                                         float *grad_vox, void *stream) {
+  CamArgs a;
+  if (int rc = rv_check("ray_consistency_views backward", vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN,
+                        eV, a))
+    return rc;
+  GB_REQUIRE(obs && grad_loss && grad_vox, GENRE_B200_EINVAL, "ray_consistency_views backward: null pointer");
+  GB_REQUIRE(aligned4(obs) && aligned4(grad_loss) && aligned4(grad_vox), GENRE_B200_EALIGN,
+             "ray_consistency_views backward: obs and gradients must be 4-byte aligned");
+  a.obs = obs;
+  a.oN = oN;
+  a.oV = oV;
+  a.oH = oH;
+  a.oW = oW;
+  a.miss = miss_cost;
+  a.g0 = grad_loss;
+  a.grad_vox = grad_vox;
+  render_camera_backward_kernel<RC_CONSISTENCY, true><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
+  return check_launch("ray_consistency_views backward kernel");
 }

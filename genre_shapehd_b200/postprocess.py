@@ -938,25 +938,24 @@ def _cam_args(vox, fl, cam_dist, z_res, name):
 
 
 class _RenderCamera(torch.autograd.Function):
+    """the fixed camera's (``genre_b200_render_camera_*``) or the posed views' (``genre_b200_render_views_*``) renderer;
+    ``args`` are the entry points' leading arguments, ``shape`` their dense [N,(V,)H,W] output shape"""
     @staticmethod
-    def forward(ctx, vox, v, keep, head, H, W, bg):
-        n = head[0]
-        depth = torch.empty((n, 1, H, W), dtype=torch.float32, device=v.device)
+    def forward(ctx, vox, v, keep, args, shape, bg, entry):
+        depth = torch.empty(shape, dtype=torch.float32, device=v.device)
         silhou = torch.empty_like(depth)
-        args = (v.data_ptr(), n, head[1], H, W) + head[2:]
-        _lib.call("genre_b200_render_camera_forward", *args, bg, depth.data_ptr(), silhou.data_ptr(), _lib.stream_ptr(v))
+        _lib.call(entry + "_forward", *args, bg, depth.data_ptr(), silhou.data_ptr(), _lib.stream_ptr(v))
         ctx.save_for_backward(v, *keep)
-        ctx.args, ctx.bg, ctx.vox_shape = args, bg, vox.shape
+        ctx.args, ctx.shape, ctx.bg, ctx.entry, ctx.vox_shape = args, shape, bg, entry, vox.shape
         return depth, silhou
 
     @staticmethod
     def backward(ctx, grad_depth, grad_silhou):
         v = ctx.saved_tensors[0]
-        shape = (v.shape[0],) + tuple(ctx.args[3:5])
-        gd = torch.zeros(shape, device=v.device) if grad_depth is None else grad_depth.reshape(shape).contiguous()
-        gs = torch.zeros(shape, device=v.device) if grad_silhou is None else grad_silhou.reshape(shape).contiguous()
+        gd = torch.zeros(ctx.shape, device=v.device) if grad_depth is None else grad_depth.reshape(ctx.shape).contiguous()
+        gs = torch.zeros(ctx.shape, device=v.device) if grad_silhou is None else grad_silhou.reshape(ctx.shape).contiguous()
         grad = torch.zeros_like(v)
-        _lib.call("genre_b200_render_camera_backward", *ctx.args, ctx.bg, gd.data_ptr(), gs.data_ptr(), grad.data_ptr(),
+        _lib.call(ctx.entry + "_backward", *ctx.args, ctx.bg, gd.data_ptr(), gs.data_ptr(), grad.data_ptr(),
                   _lib.stream_ptr(v))
         return grad.view(ctx.vox_shape), None, None, None, None, None, None
 
@@ -976,28 +975,32 @@ def render_depth(vox, fl=CAM_FL, cam_dist=CAM_DIST, size=(256, 256), z_res=None,
     refiner is trained on transpose(0,2,1) + flip(2) of the ground truth, genre_full_model.py:90-92); MarrNet-2's ``voxel``
     ground truth needs that same transform, and ``forward_with_trimesh``'s output the inverse of genre_full_model.py:231."""
     v, keep, head = _cam_args(vox, fl, cam_dist, z_res, "render_depth")
-    H, W = (int(size), int(size)) if isinstance(size, int) else (int(size[0]), int(size[1]))
-    return _RenderCamera.apply(vox, v, keep, head, H, W, float(bg))
+    H, W = _image_size(size)
+    return _RenderCamera.apply(vox, v, keep, (v.data_ptr(), head[0], head[1], H, W) + head[2:], (head[0], 1, H, W),
+                               float(bg), "genre_b200_render_camera")
+
+
+def _image_size(size):
+    return (int(size), int(size)) if isinstance(size, int) else (int(size[0]), int(size[1]))
 
 
 class _RayConsistency(torch.autograd.Function):
+    """the fixed camera's (``genre_b200_ray_consistency_*``) or the posed views' (``genre_b200_ray_consistency_views_*``)
+    loss; ``args`` end with the observation's pointer, strides and the miss cost"""
     @staticmethod
-    def forward(ctx, vox, v, keep, head, obs, miss_cost):
-        n, (H, W) = head[0], obs.shape[-2:]
-        loss = torch.empty((n, 1, H, W), dtype=torch.float32, device=v.device)
-        args = (v.data_ptr(), n, head[1], H, W) + head[2:] + (obs.data_ptr(), obs.stride(0), obs.stride(-2),
-                                                              obs.stride(-1), miss_cost)
-        _lib.call("genre_b200_ray_consistency_forward", *args, loss.data_ptr(), _lib.stream_ptr(v))
-        ctx.save_for_backward(v, obs, *keep)
-        ctx.args, ctx.vox_shape = args, vox.shape
+    def forward(ctx, vox, v, keep, args, shape, entry):
+        loss = torch.empty(shape, dtype=torch.float32, device=v.device)
+        _lib.call(entry + "_forward", *args, loss.data_ptr(), _lib.stream_ptr(v))
+        ctx.save_for_backward(v, *keep)
+        ctx.args, ctx.shape, ctx.entry, ctx.vox_shape = args, shape, entry, vox.shape
         return loss
 
     @staticmethod
     def backward(ctx, grad_loss):
         v = ctx.saved_tensors[0]
-        g = grad_loss.reshape(v.shape[0], *ctx.args[3:5]).contiguous()
+        g = grad_loss.reshape(ctx.shape).contiguous()
         grad = torch.zeros_like(v)
-        _lib.call("genre_b200_ray_consistency_backward", *ctx.args, g.data_ptr(), grad.data_ptr(), _lib.stream_ptr(v))
+        _lib.call(ctx.entry + "_backward", *ctx.args, g.data_ptr(), grad.data_ptr(), _lib.stream_ptr(v))
         return grad.view(ctx.vox_shape), None, None, None, None, None
 
 
@@ -1018,5 +1021,134 @@ def ray_consistency_loss(vox, obs_depth, fl=CAM_FL, cam_dist=CAM_DIST, z_res=Non
         raise ValueError("ray_consistency_loss: obs_depth [%d,1,H,W] expected, got %s" % (head[0], tuple(obs_depth.shape)))
     if reduction not in ("mean", "none"):
         raise ValueError("ray_consistency_loss: reduction 'mean' or 'none', got %r" % (reduction,))
-    loss = _RayConsistency.apply(vox, v, keep, head, obs, float(miss_cost))
+    n, (H, W) = head[0], obs.shape[-2:]
+    args = (v.data_ptr(), n, head[1], H, W) + head[2:] + (obs.data_ptr(), obs.stride(0), obs.stride(-2), obs.stride(-1),
+                                                          float(miss_cost))
+    loss = _RayConsistency.apply(vox, v, keep + (obs,), args, (n, 1, H, W), "genre_b200_ray_consistency")
+    return loss.mean((1, 2, 3)) if reduction == "mean" else loss
+
+
+# ---- any camera's view of a grid: posed rendering and multi-view ray consistency -----------------------------------------
+def look_at(eye, target=(0.0, 0.0, 0.0), up=(0.0, 0.0, 1.0)):
+    """Cameras at ``eye`` [..., 3] looking at ``target`` -> (rot [..., 3, 3], eye [..., 3]), fp32 torch tensors (on the
+    input's device when ``eye`` is a tensor), in the convention of ``render_depth_views``: rot's columns are the camera's
+    axes in the grid frame, column 0 the unit vector from eye to target, column 2 ``up`` made orthogonal to it and
+    normalised, column 1 = column 2 x column 0.  Formed in fp64, rounded once.  ``look_at((-CAM_DIST, 0, 0))`` is the
+    input camera, rot = I exactly.  ValueError where ``up`` is parallel to the viewing direction."""
+    dev = eye.device if isinstance(eye, torch.Tensor) else torch.device("cpu")
+    e = torch.as_tensor(eye.detach().cpu() if isinstance(eye, torch.Tensor) else np.asarray(eye), dtype=torch.float64)
+    if e.shape[-1:] != (3,):
+        raise ValueError("look_at: eye [..., 3] expected, got %s" % (tuple(e.shape),))
+    tgt = torch.as_tensor(np.asarray(target, dtype=np.float64)).expand_as(e)
+    u = torch.as_tensor(np.asarray(up, dtype=np.float64)).expand_as(e)
+    fwd = tgt - e
+    fwd = fwd / fwd.norm(dim=-1, keepdim=True)
+    z = u - (u * fwd).sum(-1, keepdim=True) * fwd
+    zn = z.norm(dim=-1, keepdim=True)
+    if not bool((zn > 1e-6 * u.norm(dim=-1, keepdim=True)).all()) or not bool(torch.isfinite(fwd).all()):
+        raise ValueError("look_at: eye equals target, or up is parallel to the viewing direction")
+    z = z / zn
+    y = torch.linalg.cross(z, fwd, dim=-1)
+    rot = torch.stack([fwd, y, z], -1)
+    return rot.float().to(dev), e.float().to(dev)
+
+
+def _pose_tensor(x):
+    """numpy, a sequence, or a tensor on any device -> fp32 tensor on that device"""
+    if isinstance(x, torch.Tensor):
+        return x.detach().float()
+    return torch.as_tensor(np.asarray(x, dtype=np.float32))
+
+
+def _poses(n, rot, eye, fl, name):
+    """rot [N|1,V,3,3], eye [N|1,V,3], fl -> fp32 tensors on their own device (fl [N|1,V]) and V, after checking that rot
+    is a rotation within 1e-5 (orthonormal, det +1) and |eye| > sqrt(3)/2: on the host for host poses, on the device
+    for CUDA poses, which costs one synchronisation"""
+    r, e = _pose_tensor(rot), _pose_tensor(eye)
+    if r.dim() != 4 or r.shape[2:] != (3, 3) or r.shape[0] not in (1, n):
+        raise ValueError("%s: rot [N|1, V, 3, 3] expected with N = %d, got %s" % (name, n, tuple(r.shape)))
+    V = r.shape[1]
+    if V < 1:
+        raise ValueError("%s: no views" % name)
+    if e.dim() != 3 or e.shape[1:] != (V, 3) or e.shape[0] not in (1, n):
+        raise ValueError("%s: eye [N|1, %d, 3] expected with N = %d, got %s" % (name, V, n, tuple(e.shape)))
+    if isinstance(fl, (int, float)):
+        f = torch.full((1, V), float(fl), dtype=torch.float32)
+    else:
+        f = _pose_tensor(fl)
+        f = f[None] if f.dim() == 1 else f
+        if f.dim() != 2 or f.shape[1] != V or f.shape[0] not in (1, n):
+            raise ValueError("%s: fl a float, [%d] or [%d, %d] expected, got %s" % (name, V, n, V, tuple(f.shape)))
+    r64, e64 = r.double(), e.double()
+    ortho = (r64.transpose(-1, -2) @ r64 - torch.eye(3, dtype=torch.float64, device=r.device)).abs().amax((-1, -2))
+    det = torch.linalg.det(r64)
+    bad_rot = ((ortho > 1e-5) | ((det - 1).abs() > 1e-5) | ~torch.isfinite(det)).any()
+    bad_eye = ~(e64.norm(dim=-1) > math.sqrt(3.0) / 2).all()
+    bad = torch.stack([bad_rot, bad_eye.to(bad_rot.device)]).cpu()              # one synchronisation for CUDA poses
+    if bad[0]:
+        raise ValueError("%s: rot must be a rotation (orthonormal with determinant +1, within 1e-5)" % name)
+    if bad[1]:
+        raise ValueError("%s: every eye must lie outside the unit cube's bounding sphere, |eye| > sqrt(3)/2" % name)
+    return r, e, f, V
+
+
+def _view_args(vox, poses, z_res, size, name):
+    """the leading arguments of the posed entry points (from the volume pointer to the eye's strides), the volumes and
+    the pose tensors they point into (host poses copied to the device once)"""
+    r, e, f, V = poses
+    v = _volumes(vox, name)
+    if not (v.shape[1] == v.shape[2] == v.shape[3]):
+        raise ValueError("%s expects cubic volumes, got %s" % (name, tuple(vox.shape)))
+    r, e, f = (x.to(v.device).contiguous() for x in (r, e, f))
+    z = default_z_res(v.shape[1]) if z_res is None else int(z_res)
+    H, W = _image_size(size)
+
+    def nv(x):                                       # strides over (n, v); 0 over n for cameras shared by the batch
+        return (x.stride(0) if x.shape[0] > 1 else 0), x.stride(1)
+    args = (v.data_ptr(), v.shape[0], v.shape[1], V, H, W, z, f.data_ptr()) + nv(f) + (r.data_ptr(),) + nv(r) + \
+        (e.data_ptr(),) + nv(e)
+    return v, (f, r, e), args
+
+
+def render_depth_views(vox, rot, eye, fl=CAM_FL, size=(256, 256), z_res=None, bg=0.0):
+    """Render each grid from V cameras of any pose, differentiably in ``vox``: ``render_depth`` with per-view extrinsics.
+
+    vox [N,1,R,R,R] (or [N,R,R,R]) fp32 on CUDA, as ``render_depth``.  Camera v of grid n: ``rot`` [N|1, V, 3, 3] (its
+    columns the camera's axes in the grid frame: x forward, image w growing towards -y, image h towards -z; see
+    ``look_at``), ``eye`` [N|1, V, 3] (the camera's centre in the grid frame, outside the sphere of radius sqrt(3)/2 that
+    holds the unit cube), ``fl`` in pixels (a float, [V] or [N, V]).  A leading 1 shares the cameras across the batch.
+    Poses may be numpy arrays, CPU or CUDA tensors: host poses are copied to the device once; CUDA poses are validated
+    on the device at the cost of one synchronisation.  rot = I, eye = (-cam_dist, 0, 0) is ``render_depth``'s camera,
+    bit for bit.
+
+    Frames: the grid frame is cam_bp's, so for GenRe's ``pred_voxel`` the poses are relative to the input camera (which is
+    ``look_at((-CAM_DIST, 0, 0))``).  Grids in another frame (ShapeHD's canonical ``voxel_canon``) need the pose of that
+    frame relative to the camera; this package does not derive it from any dataset's camera files.
+
+    Returns (depth, silhou), each [N,V,H,W].  Gradients flow to ``vox`` only; the views of one grid add theirs."""
+    poses = _poses(vox.shape[0], rot, eye, fl, "render_depth_views")
+    v, keep, args = _view_args(vox, poses, z_res, size, "render_depth_views")
+    return _RenderCamera.apply(vox, v, keep, args, args[1:2] + args[3:6], float(bg), "genre_b200_render_views")
+
+
+def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, miss_cost=1.0, reduction="mean"):
+    """Multi-view differentiable ray consistency: ``ray_consistency_loss`` against V observed depth maps per grid, each
+    from its own camera (``rot``, ``eye``, ``fl`` as ``render_depth_views``).
+
+    obs_depth [N,V,H,W] fp32 on CUDA, ray depths from each camera's eye (any strides; <= 0 marks background).  Returns
+    the per-grid mean over all V*H*W rays [N] (``reduction='mean'``) or the per-ray loss [N,V,H,W] (``'none'``).
+    Differentiable in ``vox`` only."""
+    if reduction not in ("mean", "none"):
+        raise ValueError("ray_consistency_loss_views: reduction 'mean' or 'none', got %r" % (reduction,))
+    n = vox.shape[0]
+    poses = _poses(n, rot, eye, fl, "ray_consistency_loss_views")
+    if obs_depth.dim() != 4 or obs_depth.shape[:2] != (n, poses[3]):
+        raise ValueError("ray_consistency_loss_views: obs_depth [%d,%d,H,W] expected, got %s"
+                         % (n, poses[3], tuple(obs_depth.shape)))
+    v, keep, args = _view_args(vox, poses, z_res, obs_depth.shape[2:], "ray_consistency_loss_views")
+    _lib.require_cuda(obs_depth)
+    _lib.require_f32(obs_depth)
+    args = args + (obs_depth.data_ptr(),) + tuple(obs_depth.stride()) + (float(miss_cost),)
+    loss = _RayConsistency.apply(vox, v, keep + (obs_depth,), args, tuple(obs_depth.shape),
+                                 "genre_b200_ray_consistency_views")
     return loss.mean((1, 2, 3)) if reduction == "mean" else loss

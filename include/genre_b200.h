@@ -194,6 +194,37 @@ int genre_b200_ray_consistency_backward(const float *vox, int64_t N, int res, in
                                         const float *fl, int64_t fN, const float *camdist, int64_t dN,
                                         const float *obs, int64_t oN, int64_t oH, int64_t oW, float miss_cost,
                                         const float *grad_loss, float *grad_vox, void *stream);
+/* Posed views: the same ops from V cameras per grid, rays over [N, V, H, W], all V views of grid n
+ * reading vox[n] (the backward's atomics sum the views' gradients into grad_vox[n]).  View (n, v) has
+ *   fl[n*fN + v*fV]                 focal length in pixels
+ *   rot + n*rN + v*rV  (9 floats)   3x3 rotation, row-major, its columns the camera's axes in the grid
+ *                                   frame (x forward; image w grows towards -y, image h towards -z)
+ *   eye + n*eN + v*eV  (3 floats)   the camera's centre in the grid frame, |eye| > sqrt(3)/2
+ * (strides in elements; 0 over n shares one camera set across the batch).  Pixel (h, w) keeps the
+ * camera-frame direction u above; the ray's arithmetic is, in fp64 with every operation rounded:
+ *   u'_i = (rot[i][0]*ux + rot[i][1]*uy) + rot[i][2]*uz;   d = sqrt((ex*ex + ey*ey) + ez*ez)
+ *   t = (d - sqrt(3)/2) + k * (sqrt(3)/(Z-1));   g = (t*u'x + ex, t*u'y + ey, t*u'z + ez)
+ * then f = (g + 0.5) * R - 0.5, and f and t rounded once to fp32 as above.  rot = I and
+ * eye = (-cam_dist, 0, 0) give the fixed camera's outputs bit for bit.  Outputs and upstream gradients
+ * [N, V, H, W] dense; obs [N, V, H, W] with any strides (oN, oV, oH, oW).  1 <= V, N V H W <= 2^34. */
+int genre_b200_render_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res,
+                                    const float *fl, int64_t fN, int64_t fV, const float *rot, int64_t rN, int64_t rV,
+                                    const float *eye, int64_t eN, int64_t eV, float bg, float *depth, float *silhou,
+                                    void *stream);
+int genre_b200_render_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res,
+                                     const float *fl, int64_t fN, int64_t fV, const float *rot, int64_t rN, int64_t rV,
+                                     const float *eye, int64_t eN, int64_t eV, float bg, const float *grad_depth,
+                                     const float *grad_silhou, float *grad_vox, void *stream);
+int genre_b200_ray_consistency_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                             int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                             int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                             const float *obs, int64_t oN, int64_t oV, int64_t oH, int64_t oW,
+                                             float miss_cost, float *loss, void *stream);
+int genre_b200_ray_consistency_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                              int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                              int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                              const float *obs, int64_t oN, int64_t oV, int64_t oH, int64_t oW,
+                                              float miss_cost, const float *grad_loss, float *grad_vox, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Chamfer nearest-neighbour distance.  Replaces nnd_forward_cuda / nnd_backward_cuda

@@ -36,7 +36,10 @@
 //     t    = (d - sqrt(3)/2) + k * (sqrt(3) / (Z - 1));      g = (t*u'x + ex, t*u'y + ey, t*u'z + ez)
 // With rot = I and e = (-cam_dist, 0, 0) every value equals the fixed camera's bit for bit (products by 1 are exact,
 // products by 0 add a signed zero, and the square root of a widened fp32 square is exact).  The fixed camera is the
-// POSED = false instantiation of the same templates, with exactly the arithmetic above it.
+// POSED = false instantiation of the same templates, with exactly the arithmetic above it.  It is not replaced by the
+// posed instantiation at rot = I, which is slower on the fixed camera's calls: in kernel time, +1.0-1.9% for the render
+// forward and +1.1-2.3% for the consistency forward, whose posed instance needs 48 registers instead of 40 (5 resident
+// 256-thread CTAs per SM instead of 6); whole calls through such a routing lost 1-4% (DESIGN.md §4.2).
 #include <initializer_list>
 
 #include "render.cuh"

@@ -3,7 +3,11 @@
 default Z (445), on clamp(cam_bp(depth) * 50, 1e-5, 1 - 1e-5) volumes of synth.bench_depth_batch, observed against the
 same depth maps.  Times render_depth forward, and ray_consistency_loss forward + backward, at B = 4 and 16, and the
 unfused fp32 torch composition (grid_sample, clamp, cumprod, sums; [B,1,H,W,Z] intermediates) at B = 4.  CUDA events over
-repeated calls after warm-up; prints one JSON line (and writes it to $OUT if set) with the card's name and power limit."""
+repeated calls after warm-up.  `kernel_ms` is the device time of render_cam.cu's kernels alone (torch.profiler, a pass of
+its own) for the fixed camera's instantiation and for the posed one at the identity pose (render_depth_views and
+ray_consistency_loss_views at look_at((-CAM_DIST, 0, 0)), the same rays bit for bit): what routing render_depth and
+ray_consistency_loss through the posed kernels would cost in the kernels, apart from building the poses.  Prints one
+JSON line (and writes it to $OUT if set) with the card's name and power limit."""
 import json, os, subprocess, sys
 import torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,6 +32,21 @@ def timeit(fn, reps=20):
     for _ in range(reps): fn()
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / reps
+
+
+def kernel_ms(fn, kernel, posed, reps=10):
+    """mean device time per call of render_cam.cu's `kernel`, asserting that the POSED = `posed` instantiation ran"""
+    fn(); torch.cuda.synchronize()
+    for _ in range(3):                                   # the profiler's CUDA activity sometimes records no kernel
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps): fn()
+            torch.cuda.synchronize()
+        ev = [e for e in prof.key_averages() if kernel + "<" in e.key]
+        if ev:
+            break
+    assert len(ev) == 1 and ev[0].count == reps and ("true" if posed else "false") in ev[0].key, \
+        [(e.key, e.count) for e in ev]
+    return ev[0].device_time_total / reps / 1e3
 
 
 def inputs(B):
@@ -80,6 +99,22 @@ for B in (4, 16):
          "loss_fwd_ms": timeit(lambda: postprocess.ray_consistency_loss(vox, d)),
          "loss_fwd_bwd_ms": timeit(loss_fb, reps=10)}
     r["samples_per_s_render_fwd"] = B * H * W * Z / (r["render_fwd_ms"] * 1e-3)
+    rot, eye = (x.to(dev) for x in postprocess.look_at(torch.tensor([[[-CD, 0.0, 0.0]]])))
+    vi = vox.clone().requires_grad_(True)
+
+    def bwd(loss_of):                                    # a forward and its backward; the backward kernel is timed
+        vi.grad = None
+        loss_of(vi).sum().backward()
+    fwd_k, bwd_k = "render_camera_forward_kernel", "render_camera_backward_kernel"
+    r["kernel_ms"] = {
+        "render_fwd": {"fixed": kernel_ms(lambda: postprocess.render_depth(vox), fwd_k, False),
+                       "identity_pose": kernel_ms(lambda: postprocess.render_depth_views(vox, rot, eye), fwd_k, True)},
+        "loss_fwd": {"fixed": kernel_ms(lambda: postprocess.ray_consistency_loss(vox, d), fwd_k, False),
+                     "identity_pose": kernel_ms(lambda: postprocess.ray_consistency_loss_views(vox, d, rot, eye), fwd_k,
+                                                True)},
+        "loss_bwd": {"fixed": kernel_ms(lambda: bwd(lambda x: postprocess.ray_consistency_loss(x, d)), bwd_k, False),
+                     "identity_pose": kernel_ms(
+                         lambda: bwd(lambda x: postprocess.ray_consistency_loss_views(x, d, rot, eye)), bwd_k, True)}}
     if B == 4:
         torch.cuda.reset_peak_memory_stats()
         base = torch.cuda.memory_allocated()

@@ -50,6 +50,11 @@ _SIGNATURES = {
                                                  _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _f32, _ptr, _ptr],
     "genre_b200_ray_consistency_views_backward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64,
                                                   _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _f32, _ptr, _ptr, _ptr],
+    "genre_b200_render_views_backward_pose": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr, _i64, _i64,
+                                              _ptr, _i64, _i64, _f32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "genre_b200_ray_consistency_views_backward_pose": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr,
+                                                       _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _f32,
+                                                       _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_nnd_forward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_nnd_backward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_convt3d_s2_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr, _ptr,
@@ -119,7 +124,8 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_voxel_surface_workspace_bytes", "genre_b200_convflat_positions", "genre_b200_skinny_gemm_workspace_bytes",
     "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
     "genre_b200_surface_sample_workspace_bytes", "genre_b200_crop_to_render_workspace_bytes",
-    "genre_b200_preprocess_workspace_bytes", "genre_b200_mesh_voxelize_workspace_bytes"])
+    "genre_b200_preprocess_workspace_bytes", "genre_b200_mesh_voxelize_workspace_bytes",
+    "genre_b200_render_views_pose_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
@@ -134,6 +140,7 @@ _LAUNCHES = {
     "genre_b200_ray_consistency_forward": 1, "genre_b200_ray_consistency_backward": 1,
     "genre_b200_render_views_forward": 1, "genre_b200_render_views_backward": 1,
     "genre_b200_ray_consistency_views_forward": 1, "genre_b200_ray_consistency_views_backward": 1, "genre_b200_nnd_forward": 1, "genre_b200_nnd_backward": 1,
+    "genre_b200_render_views_backward_pose": 2, "genre_b200_ray_consistency_views_backward_pose": 2,
     "genre_b200_cam_bp_stage_project": 1, "genre_b200_voxelize_stage_splat": 1,
     "genre_b200_convt3d_s2_forward": 1, "genre_b200_conv3d_taps_forward": 1,
     "genre_b200_convt_c1_forward": 1, "genre_b200_conv3d_k4s2_forward": 1,
@@ -202,6 +209,8 @@ def load():
     lib.genre_b200_preprocess_workspace_bytes.argtypes = [_int, _int, _i64, _int]
     lib.genre_b200_mesh_voxelize_workspace_bytes.restype = _size
     lib.genre_b200_mesh_voxelize_workspace_bytes.argtypes = [_i64, _i64, _int, _int, _int]
+    lib.genre_b200_render_views_pose_workspace_bytes.restype = _size
+    lib.genre_b200_render_views_pose_workspace_bytes.argtypes = [_i64, _i64, _i64, _i64]
     _lib = lib
     return lib
 

@@ -40,6 +40,17 @@
 // posed instantiation at rot = I, which is slower on the fixed camera's calls: in kernel time, +1.0-1.9% for the render
 // forward and +1.1-2.3% for the consistency forward, whose posed instance needs 48 registers instead of 40 (5 resident
 // 256-thread CTAs per SM instead of 6); whole calls through such a routing lost 1-4% (DESIGN.md §4.2).
+//
+// Pose gradients (the *_views_backward_pose entry points; tests/render_pose_ref.py restates them): the derivative of
+// this discrete op along its own samples, which move with |e|, with two simplifications that are part of the
+// definition: the fp32 roundings of f_k and t_k count as the identity, and the trilinear interpolant is differentiated
+// piecewise (on a voxel face, the one-sided derivative of the cell make_taps_at selects).  With w_k = dV/dp_k (the
+// backward's dp: 0 where the clamp is active or raw is NaN), grad_k = R d raw / d f at f_k and c'_k = d c_k / d t_k
+// (render g_depth; consistency scale sign(t_k - obs), 0 at equality and on background rays):
+//     dV/du'_i = sum_k w_k t_k grad_k,i;   dV/dt(shift) = sum_k (w_k grad_k . u' + s_k c'_k)
+//     dV/de_i  = sum_k w_k grad_k,i + (e_i / d) dV/dt(shift)
+//     grad_rot[i][j] = sum over the view's rays of dV/du'_i u_j (the ambient gradient of the 9 entries);  grad_eye = sum dV/de
+// Not differentiated: fl, obs; no double backward.
 #include <initializer_list>
 
 #include "render.cuh"
@@ -104,9 +115,9 @@ __device__ __forceinline__ CamRay cam_ray_posed(float fl, const float *__restric
   return r;
 }
 
-// sample k of the ray: taps at its fp32 voxel coordinate, and its fp32 ray depth
+// sample k of the ray: taps at its fp32 voxel coordinate (also stored in f when given), and its fp32 ray depth
 template <bool POSED>
-__device__ __forceinline__ float cam_sample(const CamRay &r, int k, int R, Taps &taps) {
+__device__ __forceinline__ float cam_sample(const CamRay &r, int k, int R, Taps &taps, float *f = nullptr) {
   const double Rd = (double)R;
   const double t = __dadd_rn(r.t0, __dmul_rn((double)k, r.dt));
   const double gx = __dadd_rn(__dmul_rn(t, r.ux), r.ex);
@@ -116,6 +127,11 @@ __device__ __forceinline__ float cam_sample(const CamRay &r, int k, int R, Taps 
   const float fy = (float)__dadd_rn(__dmul_rn(__dadd_rn(gy, 0.5), Rd), -0.5);
   const float fz = (float)__dadd_rn(__dmul_rn(__dadd_rn(gz, 0.5), Rd), -0.5);
   make_taps_at(fx, fy, fz, R, taps);
+  if (f) {
+    f[0] = fx;
+    f[1] = fy;
+    f[2] = fz;
+  }
   return (float)t;
 }
 
@@ -125,6 +141,7 @@ struct LinearCost {
   float a, b, e;
   __device__ __forceinline__ float at(float t) const { return fmaf(a, t, b); }
   __device__ __forceinline__ float esc() const { return e; }
+  __device__ __forceinline__ float slope(float) const { return a; }  // d c_k / d t_k
 };
 
 // differentiable ray consistency against an observed ray depth (<= 0: background)
@@ -132,6 +149,9 @@ struct RayCost {
   float obs, miss;
   __device__ __forceinline__ float at(float t) const { return obs > 0.0f ? fabsf(t - obs) : miss; }
   __device__ __forceinline__ float esc() const { return obs > 0.0f ? miss : 0.0f; }
+  __device__ __forceinline__ float slope(float t) const {  // sign(t - obs), 0 at equality and on background rays
+    return obs > 0.0f ? (t > obs ? 1.0f : (t < obs ? -1.0f : 0.0f)) : 0.0f;
+  }
 };
 
 // The forward walk: returns (sum_k s_k c_k, T_Z) to every lane.  With chunk_T, chunk c's carry (T before its first
@@ -294,6 +314,156 @@ __global__ void __launch_bounds__(RC_THREADS) render_camera_backward_kernel(cons
                             s_T[warp]);
 }
 
+// ---- pose gradients of the posed views (the *_views_backward_pose entry points) ----------------------------------------
+// Their own kernel, so that CamArgs and the kernels above keep their argument block and code.
+struct PoseOut {
+  float *grad_rot, *grad_eye;  // [N, V, 9] and [N, V, 3] dense
+  double *part;                // workspace: per view, RP_TERMS rows of bpv per-CTA partial sums
+  long long bpv;               // CTAs per view
+};
+constexpr int RP_TERMS = 13;   // (dV/du') (x) u: 9;  sum_k w_k grad_k: 3;  dV/dt(shift): 1
+
+// cam_backward_ray's two walks (the same T_k, A_k, dp and voxel atomics, none without gvol) plus the ray's pose sums,
+// each lane over its own samples, with g_k = d raw / d f at f_k in voxel units (the caller scales by R):
+//   acc[0..2] = sum_k w_k t_k g_k,  acc[3..5] = sum_k w_k g_k,  acc[6] = sum_k w_k g_k . u',  acc[7] = sum_k s_k c'_k
+// w_k = dp (zero where the clamp is active or raw is NaN), c'_k = scale * d c_k / d t_k.
+template <class Cost>
+__device__ __forceinline__ void cam_backward_ray_pose(const float *__restrict__ vol, float *__restrict__ gvol, int R,
+                                                      const CamRay &ray, int Z, const Cost &cost, float scale,
+                                                      float *chunk_T, float (&acc)[8]) {
+  const int lane = threadIdx.x & 31;
+  float sum, T_Z;
+  int last = 0;
+  cam_walk<true>(vol, R, ray, Z, cost, sum, T_Z, chunk_T, &last);
+  __syncwarp();
+  const float ux = (float)ray.ux, uy = (float)ray.uy, uz = (float)ray.uz;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.0f;
+  float suffix = T_Z * cost.esc();
+  for (int c = last; c >= 0; --c) {
+    const int k = c * 32 + lane;
+    const bool live = k < Z;
+    float raw = 0.0f, p = 0.0f, ck = 0.0f, tk = 0.0f, gx = 0.0f, gy = 0.0f, gz = 0.0f;
+    Taps t;
+    if (live) {
+      float f[3];
+      tk = cam_sample<true>(ray, k, R, t, f);
+      ck = cost.at(tk);
+      raw = sample_trilinear_grad(vol, t, R, f[0], f[1], f[2], gx, gy, gz);
+      p = fminf(fmaxf(raw, RS_PMIN), RS_PMAX);
+    }
+    float total;
+    const float Tk = chunk_T[c] * warp_excl_prod32(1.0f - p, total);  // the forward's T_k, bit for bit
+    float chunk_sum;
+    const float Ak = suffix + warp_excl_suffix_sum32(live ? p * Tk * ck : 0.0f, chunk_sum);
+    suffix += chunk_sum;
+    if (live) acc[7] = fmaf(p * Tk, scale * cost.slope(tk), acc[7]);
+    if (live && raw >= RS_PMIN && raw <= RS_PMAX) {  // NaN and clamped samples pass no gradient
+      const float dp = scale * (Tk * ck - Ak / (1.0f - p));
+      if (dp != 0.0f) {
+        if (gvol) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (t.valid & (1u << i)) atomicAdd(gvol + t.base + tap_offset(i, R), dp * t.w[i]);
+        }
+        const float wx = dp * gx, wy = dp * gy, wz = dp * gz;
+        acc[0] = fmaf(wx, tk, acc[0]);
+        acc[1] = fmaf(wy, tk, acc[1]);
+        acc[2] = fmaf(wz, tk, acc[2]);
+        acc[3] += wx;
+        acc[4] += wy;
+        acc[5] += wz;
+        acc[6] = fmaf(wz, uz, fmaf(wy, uy, fmaf(wx, ux, acc[6])));
+      }
+    }
+  }
+}
+
+// One CTA per 8 rays of one view (CTAs never straddle views): each warp reduces its ray's sums, and the CTA writes the
+// RP_TERMS fp64 sums of its 8 rays, in warp order, to the workspace.  No atomics on the pose terms: bitwise repeatable.
+template <int MODE>
+__global__ void __launch_bounds__(RC_THREADS) render_views_pose_backward_kernel(const CamArgs a, const PoseOut po) {
+  __shared__ float s_T[RC_WARPS][RC_MAX_CHUNKS];
+  __shared__ double s_part[RC_WARPS][RP_TERMS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long hw = (long long)a.H * a.W;
+  const long long view = blockIdx.x / po.bpv, blk = blockIdx.x - view * po.bpv;
+  const long long pix = blk * RC_WARPS + warp;
+  double part[RP_TERMS];
+#pragma unroll
+  for (int i = 0; i < RP_TERMS; ++i) part[i] = 0.0;
+  if (pix < hw) {
+    const long long ray = view * hw + pix;
+    const float g0 = a.g0[ray], g1 = MODE == RC_RENDER ? a.g1[ray] : 0.0f;
+    if (g0 != 0.0f || g1 != 0.0f) {  // warp-uniform
+      const RayIndex ri = ray_index<true>(a, ray);
+      const size_t vol_off = (size_t)ri.n * a.R * a.R * a.R;
+      float *gvol = a.grad_vox ? a.grad_vox + vol_off : nullptr;
+      const CamRay r = ray_of<true>(a, ri);
+      float acc[8];
+      if (MODE == RC_RENDER)
+        cam_backward_ray_pose(a.vox + vol_off, gvol, a.R, r, a.Z, LinearCost{g0, g1, g0 * a.bg}, 1.0f, s_T[warp], acc);
+      else
+        cam_backward_ray_pose(a.vox + vol_off, gvol, a.R, r, a.Z, RayCost{obs_of<true>(a, ri), a.miss}, g0, s_T[warp],
+                              acc);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = warp_sum(acc[i]);
+      const CamRay u = cam_dir(a.fl[ri.n * a.fN + ri.v * a.fV], ri.h, ri.w, a.H, a.W, a.Z);  // camera-frame u
+      const double Rd = (double)a.R, uc[3] = {u.ux, u.uy, u.uz};
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) part[3 * i + j] = (double)acc[i] * Rd * uc[j];
+        part[9 + i] = (double)acc[3 + i] * Rd;
+      }
+      part[12] = (double)acc[6] * Rd + (double)acc[7];
+    }
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int i = 0; i < RP_TERMS; ++i) s_part[warp][i] = part[i];
+  }
+  __syncthreads();
+  if (threadIdx.x < RP_TERMS) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < RC_WARPS; ++w) s += s_part[w][threadIdx.x];
+    po.part[(view * RP_TERMS + threadIdx.x) * po.bpv + blk] = s;
+  }
+}
+
+// One CTA per view: sums the view's partials in a fixed order (strided per thread, then a tree), and writes
+// grad_rot[i][j] = sum (dV/du'_i) u_j and grad_eye = sum w_k grad_k + (e / |e|) dV/dt(shift), the |e| term once per view.
+__global__ void __launch_bounds__(RC_THREADS) render_views_pose_reduce_kernel(const CamArgs a, const PoseOut po) {
+  __shared__ double s[RP_TERMS][RC_THREADS];
+  const long long view = blockIdx.x;
+  const int tid = threadIdx.x;
+#pragma unroll 1
+  for (int c = 0; c < RP_TERMS; ++c) {
+    const double *p = po.part + (view * RP_TERMS + c) * po.bpv;
+    double acc = 0.0;
+    for (long long b = tid; b < po.bpv; b += RC_THREADS) acc += p[b];
+    s[c][tid] = acc;
+  }
+  __syncthreads();
+  for (int w = RC_THREADS / 2; w > 0; w >>= 1) {
+    if (tid < w)
+      for (int c = 0; c < RP_TERMS; ++c) s[c][tid] += s[c][tid + w];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    const long long n = view / a.V, v = view - n * a.V;
+    const float *e = a.eye + n * a.eN + v * a.eV;
+    const double ex = (double)e[0], ey = (double)e[1], ez = (double)e[2];
+    const double d = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)), __dmul_rn(ez, ez)));
+    const double sh = s[12][0] / d;
+    for (int i = 0; i < 9; ++i) po.grad_rot[view * 9 + i] = (float)s[i][0];
+    po.grad_eye[view * 3 + 0] = (float)(s[9][0] + ex * sh);
+    po.grad_eye[view * 3 + 1] = (float)(s[10][0] + ey * sh);
+    po.grad_eye[view * 3 + 2] = (float)(s[11][0] + ez * sh);
+  }
+}
+
 static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 constexpr long long RC_MAX_RAYS = 1ll << 34;
@@ -346,6 +516,38 @@ static int rv_check(const char *what, const float *vox, int64_t N, int res, int6
 }
 
 static unsigned rc_grid(const CamArgs &a) { return (unsigned)((a.n_rays + RC_WARPS - 1) / RC_WARPS); }
+
+static long long rp_bpv(int64_t H, int64_t W) { return ((long long)H * W + RC_WARPS - 1) / RC_WARPS; }
+
+// the pose outputs' and the workspace's checks; po.bpv is the CTAs per view
+static int rp_check(const char *what, const CamArgs &a, int64_t N, int64_t V, float *grad_vox, float *grad_rot,
+                    float *grad_eye, void *workspace, size_t workspace_bytes, PoseOut &po) {
+  const long long bpv = rp_bpv(a.H, a.W);
+  GB_REQUIRE(bpv <= ((1ll << 31) - 1) / ((long long)N * V), GENRE_B200_EINVAL,
+             "%s: %lld views of %lld CTAs unsupported (fewer than 2^31 CTAs)", what, (long long)(N * V), bpv);
+  GB_REQUIRE(grad_rot && grad_eye && workspace, GENRE_B200_EINVAL, "%s: null grad_rot, grad_eye or workspace", what);
+  GB_REQUIRE(aligned4(grad_rot) && aligned4(grad_eye) && (grad_vox == nullptr || aligned4(grad_vox)), GENRE_B200_EALIGN,
+             "%s: grad_vox, grad_rot and grad_eye must be 4-byte aligned", what);
+  GB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7u) == 0, GENRE_B200_EALIGN,
+             "%s: workspace must be 8-byte aligned", what);
+  const size_t need = (size_t)N * V * RP_TERMS * bpv * sizeof(double);
+  GB_REQUIRE(workspace_bytes >= need, GENRE_B200_EWORKSPACE, "%s: workspace too small (%zu bytes, %zu needed)", what,
+             workspace_bytes, need);
+  po.grad_rot = grad_rot;
+  po.grad_eye = grad_eye;
+  po.part = static_cast<double *>(workspace);
+  po.bpv = bpv;
+  return 0;
+}
+
+template <int MODE>
+static int rp_launch(const char *what, const CamArgs &a, const PoseOut &po, void *stream) {
+  const long long views = a.n_rays / ((long long)a.H * a.W);
+  render_views_pose_backward_kernel<MODE><<<(unsigned)(views * po.bpv), RC_THREADS, 0, as_stream(stream)>>>(a, po);
+  if (int rc = check_launch(what)) return rc;
+  render_views_pose_reduce_kernel<<<(unsigned)views, RC_THREADS, 0, as_stream(stream)>>>(a, po);
+  return check_launch(what);
+}
 
 }  // namespace gb
 
@@ -516,4 +718,55 @@ extern "C" int genre_b200_ray_consistency_views_backward(const float *vox, int64
   a.grad_vox = grad_vox;
   render_camera_backward_kernel<RC_CONSISTENCY, true><<<rc_grid(a), RC_THREADS, 0, as_stream(stream)>>>(a);
   return check_launch("ray_consistency_views backward kernel");
+}
+
+extern "C" size_t genre_b200_render_views_pose_workspace_bytes(int64_t N, int64_t V, int64_t H, int64_t W) {
+  if (N < 1 || V < 1 || H < 1 || W < 1) return 0;
+  return (size_t)N * V * RP_TERMS * rp_bpv(H, W) * sizeof(double);
+}
+
+extern "C" int genre_b200_render_views_backward_pose(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                     int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                     const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                     int64_t eN, int64_t eV, float bg, const float *grad_depth,
+                                                     const float *grad_silhou, float *grad_vox, float *grad_rot,
+                                                     float *grad_eye, void *workspace, size_t workspace_bytes,
+                                                     void *stream) {
+  CamArgs a;
+  PoseOut po;
+  const char *what = "render_views backward_pose";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, a)) return rc;
+  GB_REQUIRE(grad_depth && grad_silhou, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(aligned4(grad_depth) && aligned4(grad_silhou), GENRE_B200_EALIGN,
+             "%s: gradients must be 4-byte aligned", what);
+  if (int rc = rp_check(what, a, N, V, grad_vox, grad_rot, grad_eye, workspace, workspace_bytes, po)) return rc;
+  a.bg = bg;
+  a.g0 = grad_depth;
+  a.g1 = grad_silhou;
+  a.grad_vox = grad_vox;
+  return rp_launch<RC_RENDER>("render_views backward_pose kernels", a, po, stream);
+}
+
+extern "C" int genre_b200_ray_consistency_views_backward_pose(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, const float *obs,
+    int64_t oN, int64_t oV, int64_t oH, int64_t oW, float miss_cost, const float *grad_loss, float *grad_vox,
+    float *grad_rot, float *grad_eye, void *workspace, size_t workspace_bytes, void *stream) {
+  CamArgs a;
+  PoseOut po;
+  const char *what = "ray_consistency_views backward_pose";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, a)) return rc;
+  GB_REQUIRE(obs && grad_loss, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(aligned4(obs) && aligned4(grad_loss), GENRE_B200_EALIGN, "%s: obs and grad_loss must be 4-byte aligned",
+             what);
+  if (int rc = rp_check(what, a, N, V, grad_vox, grad_rot, grad_eye, workspace, workspace_bytes, po)) return rc;
+  a.obs = obs;
+  a.oN = oN;
+  a.oV = oV;
+  a.oH = oH;
+  a.oW = oW;
+  a.miss = miss_cost;
+  a.g0 = grad_loss;
+  a.grad_vox = grad_vox;
+  return rp_launch<RC_CONSISTENCY>("ray_consistency_views backward_pose kernels", a, po, stream);
 }

@@ -1053,6 +1053,32 @@ def look_at(eye, target=(0.0, 0.0, 0.0), up=(0.0, 0.0, 1.0)):
     return rot.float().to(dev), e.float().to(dev)
 
 
+def axis_angle_rotation(w):
+    """Rotations from axis-angle vectors w [..., 3] (the axis times the angle in radians) -> [..., 3, 3], by Rodrigues'
+    formula R = I + (sin a / a) K + (2 sin^2(a/2) / a^2) K^2, K the cross-product matrix of w, a = |w|, in w's dtype and
+    on its device, differentiable.  Below a = 1e-3 the two coefficients are their Taylor series, so R(0) = I exactly and
+    the gradient at 0 is finite.
+
+    ``render_depth_views`` and ``ray_consistency_loss_views`` accept only rotations (within 1e-5), so a plain gradient
+    step on ``rot`` fails after one step; fit a rotation through its axis-angle offset from an initial pose instead:
+
+        w = torch.zeros(N, V, 3, device="cuda", requires_grad=True)
+        rot = axis_angle_rotation(w) @ rot0          # rot0 [N|1, V, 3, 3], e.g. from look_at
+        loss = ray_consistency_loss_views(vox, obs, rot, eye0 + dt).sum()"""
+    if not isinstance(w, torch.Tensor) or not w.is_floating_point() or w.shape[-1:] != (3,):
+        raise ValueError("axis_angle_rotation: a floating-point tensor [..., 3] expected")
+    a2 = (w * w).sum(-1)
+    small = a2 < 1e-6
+    a = torch.sqrt(torch.where(small, torch.ones_like(a2), a2))
+    s = torch.where(small, 1 - a2 / 6 + a2 * a2 / 120, torch.sin(a) / a)
+    c = torch.where(small, 0.5 - a2 / 24 + a2 * a2 / 720, 2 * torch.sin(a / 2) ** 2 / (a * a))
+    x, y, z = w.unbind(-1)
+    o = torch.zeros_like(x)
+    K = torch.stack([o, -z, y, z, o, -x, -y, x, o], -1).reshape(w.shape[:-1] + (3, 3))
+    eye = torch.eye(3, dtype=w.dtype, device=w.device)
+    return eye + s[..., None, None] * K + c[..., None, None] * (K @ K)
+
+
 def _pose_tensor(x):
     """numpy, a sequence, or a tensor on any device -> fp32 tensor on that device"""
     if isinstance(x, torch.Tensor):
@@ -1110,8 +1136,58 @@ def _view_args(vox, poses, z_res, size, name):
     return v, (f, r, e), args
 
 
+class _ViewsPose(torch.autograd.Function):
+    """the posed views' renderer (``extra`` = (bg,)) or loss (``extra`` = ()) differentiable in the poses as well: the
+    forward is _RenderCamera's / _RayConsistency's launch; the backward calls ``entry``'s ``_backward_pose``, which
+    writes per-view grad_rot [N,V,9] and grad_eye [N,V,3] (summed here over n for cameras shared by the batch) and
+    accumulates grad_vox only when ``vox`` needs it.  rot_in / eye_in are the pose tensors on the device (None when not
+    differentiated): their values are the validated copies in ``keep`` that ``args`` point into."""
+    @staticmethod
+    def forward(ctx, vox, rot_in, eye_in, v, keep, args, shape, extra, entry):
+        outs = [torch.empty(shape, dtype=torch.float32, device=v.device) for _ in range(2 if extra else 1)]
+        _lib.call(entry + "_forward", *args, *extra, *(o.data_ptr() for o in outs), _lib.stream_ptr(v))
+        ctx.save_for_backward(v, *keep)
+        ctx.args, ctx.shape, ctx.extra, ctx.entry, ctx.vox_shape = args, shape, extra, entry, vox.shape
+        ctx.lead = tuple(None if x is None else x.shape[0] for x in (rot_in, eye_in))
+        return tuple(outs) if extra else outs[0]
+
+    @staticmethod
+    def backward(ctx, *grads):
+        v = ctx.saved_tensors[0]
+        N, V, H, W = ctx.shape
+        gs = [torch.zeros(ctx.shape, device=v.device) if g is None else g.reshape(ctx.shape).contiguous() for g in grads]
+        gvox = torch.zeros_like(v) if ctx.needs_input_grad[0] else None
+        grot = torch.empty((N, V, 3, 3), dtype=torch.float32, device=v.device)
+        geye = torch.empty((N, V, 3), dtype=torch.float32, device=v.device)
+        nbytes = _lib.load().genre_b200_render_views_pose_workspace_bytes(N, V, H, W)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+        _lib.call(ctx.entry + "_backward_pose", *ctx.args, *ctx.extra, *(g.data_ptr() for g in gs),
+                  None if gvox is None else gvox.data_ptr(), grot.data_ptr(), geye.data_ptr(), ws.data_ptr(), nbytes,
+                  _lib.stream_ptr(v))
+
+        def fold(g, lead, i):                        # a leading 1: one camera set for the batch, its gradients summed
+            if lead is None or not ctx.needs_input_grad[i]:
+                return None
+            return g.sum(0, keepdim=True) if lead == 1 else g
+        return (None if gvox is None else gvox.view(ctx.vox_shape), fold(grot, ctx.lead[0], 1), fold(geye, ctx.lead[1], 2),
+                None, None, None, None, None, None)
+
+
+def _pose_inputs(rot, eye, fl, dev, name):
+    """(rot, eye) as differentiable fp32 tensors on dev (None where not a tensor that requires grad), or None when no
+    pose is differentiated; ValueError for an fl that requires grad"""
+    if not torch.is_grad_enabled():
+        return None
+    if isinstance(fl, torch.Tensor) and fl.requires_grad:
+        raise ValueError("%s: fl requires grad, but the focal length is not differentiated (pass fl.detach())" % name)
+    ins = tuple(x.to(device=dev, dtype=torch.float32) if isinstance(x, torch.Tensor) and x.requires_grad else None
+                for x in (rot, eye))
+    return None if ins == (None, None) else ins
+
+
 def render_depth_views(vox, rot, eye, fl=CAM_FL, size=(256, 256), z_res=None, bg=0.0):
-    """Render each grid from V cameras of any pose, differentiably in ``vox``: ``render_depth`` with per-view extrinsics.
+    """Render each grid from V cameras of any pose, differentiably in ``vox``, ``rot`` and ``eye``: ``render_depth`` with
+    per-view extrinsics.
 
     vox [N,1,R,R,R] (or [N,R,R,R]) fp32 on CUDA, as ``render_depth``.  Camera v of grid n: ``rot`` [N|1, V, 3, 3] (its
     columns the camera's axes in the grid frame: x forward, image w growing towards -y, image h towards -z; see
@@ -1125,10 +1201,18 @@ def render_depth_views(vox, rot, eye, fl=CAM_FL, size=(256, 256), z_res=None, bg
     ``look_at((-CAM_DIST, 0, 0))``).  Grids in another frame (ShapeHD's canonical ``voxel_canon``) need the pose of that
     frame relative to the camera; this package does not derive it from any dataset's camera files.
 
-    Returns (depth, silhou), each [N,V,H,W].  Gradients flow to ``vox`` only; the views of one grid add theirs."""
+    Returns (depth, silhou), each [N,V,H,W].  Gradients flow to ``vox`` (the views of one grid add theirs) and, when
+    ``rot`` or ``eye`` is a tensor that requires grad, to it: the ambient gradient of rot's 9 entries (step through
+    ``axis_angle_rotation``, not on rot itself) and of eye's 3, along the op's own samples, which move with |eye|.  A
+    leading 1 (cameras shared by the batch) receives the sum over the batch; host poses receive theirs on the host.  Pose
+    gradients are bitwise repeatable.  ``fl`` is not differentiated (ValueError if it requires grad)."""
     poses = _poses(vox.shape[0], rot, eye, fl, "render_depth_views")
+    pose_in = _pose_inputs(rot, eye, fl, vox.device, "render_depth_views")
     v, keep, args = _view_args(vox, poses, z_res, size, "render_depth_views")
-    return _RenderCamera.apply(vox, v, keep, args, args[1:2] + args[3:6], float(bg), "genre_b200_render_views")
+    shape = args[1:2] + args[3:6]
+    if pose_in is not None:
+        return _ViewsPose.apply(vox, *pose_in, v, keep, args, shape, (float(bg),), "genre_b200_render_views")
+    return _RenderCamera.apply(vox, v, keep, args, shape, float(bg), "genre_b200_render_views")
 
 
 def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, miss_cost=1.0, reduction="mean"):
@@ -1137,7 +1221,9 @@ def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, 
 
     obs_depth [N,V,H,W] fp32 on CUDA, ray depths from each camera's eye (any strides; <= 0 marks background).  Returns
     the per-grid mean over all V*H*W rays [N] (``reduction='mean'``) or the per-ray loss [N,V,H,W] (``'none'``).
-    Differentiable in ``vox`` only."""
+    Differentiable in ``vox``, and in ``rot`` and ``eye`` as ``render_depth_views`` (not in ``fl`` or ``obs_depth``): with
+    ``vox`` frozen, descending on the pose fits a camera to an observed depth map (see ``axis_angle_rotation``); the
+    grid's gradient is then skipped."""
     if reduction not in ("mean", "none"):
         raise ValueError("ray_consistency_loss_views: reduction 'mean' or 'none', got %r" % (reduction,))
     n = vox.shape[0]
@@ -1145,10 +1231,15 @@ def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, 
     if obs_depth.dim() != 4 or obs_depth.shape[:2] != (n, poses[3]):
         raise ValueError("ray_consistency_loss_views: obs_depth [%d,%d,H,W] expected, got %s"
                          % (n, poses[3], tuple(obs_depth.shape)))
+    pose_in = _pose_inputs(rot, eye, fl, vox.device, "ray_consistency_loss_views")
     v, keep, args = _view_args(vox, poses, z_res, obs_depth.shape[2:], "ray_consistency_loss_views")
     _lib.require_cuda(obs_depth)
     _lib.require_f32(obs_depth)
     args = args + (obs_depth.data_ptr(),) + tuple(obs_depth.stride()) + (float(miss_cost),)
-    loss = _RayConsistency.apply(vox, v, keep + (obs_depth,), args, tuple(obs_depth.shape),
-                                 "genre_b200_ray_consistency_views")
+    if pose_in is not None:
+        loss = _ViewsPose.apply(vox, *pose_in, v, keep + (obs_depth,), args, tuple(obs_depth.shape), (),
+                                "genre_b200_ray_consistency_views")
+    else:
+        loss = _RayConsistency.apply(vox, v, keep + (obs_depth,), args, tuple(obs_depth.shape),
+                                     "genre_b200_ray_consistency_views")
     return loss.mean((1, 2, 3)) if reduction == "mean" else loss

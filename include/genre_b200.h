@@ -225,6 +225,31 @@ int genre_b200_ray_consistency_views_backward(const float *vox, int64_t N, int r
                                               int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
                                               const float *obs, int64_t oN, int64_t oV, int64_t oH, int64_t oW,
                                               float miss_cost, const float *grad_loss, float *grad_vox, void *stream);
+/* Pose gradients of the posed views: the backwards above plus d(sum of upstream gradient x output)/d rot and d/d eye
+ * per view, written (not accumulated) to grad_rot [N, V, 9] (row-major, the ambient gradient of the 9 entries) and
+ * grad_eye [N, V, 3], dense, per (n, v) even where rot / eye are shared over n (stride 0).  The derivative is the
+ * discrete op's along its own samples, which move with |eye|; the fp32 roundings of f and t count as the identity and
+ * the trilinear interpolant is differentiated in the cell make_taps selects.  Not differentiated: fl, obs.
+ *   grad_vox   nullable: NULL skips the voxel atomics (pose-only fitting); else accumulated exactly as the
+ *              backwards above.
+ *   workspace  genre_b200_render_views_pose_workspace_bytes(N, V, H, W) bytes, 8-byte aligned, caller-owned: one
+ *              CTA's fp64 partial sums per 8 rays of a view, summed per view in a fixed order, so grad_rot and
+ *              grad_eye are bitwise repeatable.  Two kernel launches.
+ * Null or misaligned pose outputs: GENRE_B200_EINVAL / GENRE_B200_EALIGN; a short workspace: GENRE_B200_EWORKSPACE. */
+size_t genre_b200_render_views_pose_workspace_bytes(int64_t N, int64_t V, int64_t H, int64_t W);
+int genre_b200_render_views_backward_pose(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                          int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                          int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, float bg,
+                                          const float *grad_depth, const float *grad_silhou, float *grad_vox,
+                                          float *grad_rot, float *grad_eye, void *workspace, size_t workspace_bytes,
+                                          void *stream);
+int genre_b200_ray_consistency_views_backward_pose(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                   int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                   const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                   int64_t eN, int64_t eV, const float *obs, int64_t oN, int64_t oV,
+                                                   int64_t oH, int64_t oW, float miss_cost, const float *grad_loss,
+                                                   float *grad_vox, float *grad_rot, float *grad_eye, void *workspace,
+                                                   size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Chamfer nearest-neighbour distance.  Replaces nnd_forward_cuda / nnd_backward_cuda

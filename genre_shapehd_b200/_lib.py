@@ -29,6 +29,10 @@ _SIGNATURES = {
     "genre_b200_cam_bp_backward": [_ptr] + [_i64] * 8 + [_ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _ptr, _int, _ptr,
                                                         _ptr, _ptr, _ptr],
     "genre_b200_surface_mask": [_ptr] + [_i64] * 8 + [_ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _ptr, _int, _ptr],
+    "genre_b200_cam_bp_views_forward": [_ptr] + [_i64] * 8 + [_ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr,
+                                                             _ptr, _int, _uint, _ptr, _size, _ptr],
+    "genre_b200_cam_bp_views_backward": [_ptr] + [_i64] * 8 + [_ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr,
+                                                              _ptr, _int, _ptr, _ptr],
     "genre_b200_sph_bp_forward": [_ptr] + [_i64] * 8 + [_ptr] + [_i64] * 5 + [_ptr, _ptr, _int, _ptr, _size, _ptr],
     "genre_b200_sph_bp_backward": [_ptr] + [_i64] * 8 + [_ptr] + [_i64] * 5 + [_ptr, _ptr, _int, _ptr, _ptr],
     "genre_b200_calc_prob_forward": [_ptr, _ptr, _i64, _i64, _ptr],
@@ -134,6 +138,7 @@ launch_count = 0  # kernels of this library enqueued through the binding (bench.
 # call's arguments
 _LAUNCHES = {
     "genre_b200_cam_bp_forward": 2, "genre_b200_cam_bp_backward": 1, "genre_b200_surface_mask": 1,
+    "genre_b200_cam_bp_views_forward": 2, "genre_b200_cam_bp_views_backward": 1,
     "genre_b200_sph_bp_forward": 2, "genre_b200_sph_bp_backward": 1, "genre_b200_calc_prob_forward": 1,
     "genre_b200_calc_prob_backward": 1, "genre_b200_render_spherical_forward": 1,
     "genre_b200_render_spherical_backward": 1, "genre_b200_render_camera_forward": 1, "genre_b200_render_camera_backward": 1,

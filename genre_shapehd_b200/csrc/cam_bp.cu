@@ -18,6 +18,19 @@
 //     centre  = ((float)index + 0.5) / R - 0.5
 //     dist^2  = fma(dz, dz, fma(dx, dx, dy*dy))
 // Intrinsics are never contracted by the compiler, so this file does not depend on -fmad.
+//
+// Posed views (the genre_b200_cam_bp_views_* entry points): depth [N, V, H, W], view (n, v) a camera of any pose in
+// render_depth_views' convention (render_cam.cu): rot 3x3 row-major, its columns the camera's axes in the grid frame,
+// eye e the camera's centre, fl its focal length.  The camera-frame part of the unprojection is the one above; the
+// point is then moved into the grid frame in fp32, in this order,
+//     cy = (imw * -z) / fl ;  cz = (imh * -z) / fl
+//     g_i = fma(rot[i][2], cz, fma(rot[i][1], cy, rot[i][0] * z)) + e_i
+// and everything after (index, centre distance, quantisation) is unchanged.  With rot = I and e = (-cam_dist, 0, 0)
+// every g_i equals the fixed camera's except possibly the sign of a zero, which changes no index or distance, so the
+// identity pose reproduces genre_b200_cam_bp_forward bit for bit.  All V views of grid n emit into map n (P = V H W
+// pixels per map), so a voxel holds the mean over every point any view placed in it; the integer sums make that
+// independent of the order of the views.  The backward rotates the direction (-fl, imw, imh) / len by rot in the same
+// fma order and keeps the fixed formula; it does not differentiate fl, rot or eye.
 #include "voxelize.cuh"
 
 namespace gb {
@@ -30,8 +43,35 @@ struct CamPoint {
   bool in_bounds;
 };
 
+// a camera: the fixed one uses cam_dist only, a posed view rot (row-major) and eye only
+struct CamFrame {
+  float cam_dist;
+  float r[9], e[3];
+};
+
+// a posed view's frame, read once per CTA
+__device__ __forceinline__ CamFrame cam_frame_posed(const float *__restrict__ rot, const float *__restrict__ eye) {
+  CamFrame f;
+  f.cam_dist = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 9; ++i) f.r[i] = __ldg(rot + i);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) f.e[i] = __ldg(eye + i);
+  return f;
+}
+
+// component i of rot (x, y, z): fma(r_i2, z, fma(r_i1, y, r_i0 * x))
+__device__ __forceinline__ float cam_rotate(const CamFrame &f, int i, float x, float y, float z) {
+  return __fmaf_rn(f.r[3 * i + 2], z, __fmaf_rn(f.r[3 * i + 1], y, __fmul_rn(f.r[3 * i], x)));
+}
+// camera frame (z, cy, cz) -> grid frame: g_i = fma(r_i2, cz, fma(r_i1, cy, r_i0 * z)) + e_i
+__device__ __forceinline__ float cam_to_grid(const CamFrame &f, int i, float z, float cy, float cz) {
+  return __fadd_rn(cam_rotate(f, i, z, cy, cz), f.e[i]);
+}
+
 // shared by forward and backward: pixel (h, w) with ray depth d -> point and voxel index
-__device__ __forceinline__ CamPoint cam_unproject(float d, float fl, const ExactDivisor &dfl, float cam_dist, int h,
+template <bool POSED = false>
+__device__ __forceinline__ CamPoint cam_unproject(float d, float fl, const ExactDivisor &dfl, const CamFrame &cam, int h,
                                                   int w, float Hm1, float Wm1, int R, float Rf) {
   CamPoint p;
   p.imh = __fmaf_rn(Hm1, -0.5f, (float)h);
@@ -42,7 +82,14 @@ __device__ __forceinline__ CamPoint cam_unproject(float d, float fl, const Exact
   const float z = __fmul_rn(d, cos_theta);
   p.gy = div_exact(__fmul_rn(p.imw, -z), dfl);
   p.gz = div_exact(__fmul_rn(p.imh, -z), dfl);
-  p.gx = __fadd_rn(z, -cam_dist);
+  if (POSED) {
+    const float cy = p.gy, cz = p.gz;
+    p.gx = cam_to_grid(cam, 0, z, cy, cz);
+    p.gy = cam_to_grid(cam, 1, z, cy, cz);
+    p.gz = cam_to_grid(cam, 2, z, cy, cz);
+  } else {
+    p.gx = __fadd_rn(z, -cam.cam_dist);
+  }
   p.ix = floor_i_ref(__fmul_rn(__fadd_rn(p.gx, 0.5f), Rf));
   p.iy = floor_i_ref(__fmul_rn(__fadd_rn(p.gy, 0.5f), Rf));
   p.iz = floor_i_ref(__fmul_rn(__fadd_rn(p.gz, 0.5f), Rf));
@@ -56,7 +103,8 @@ __device__ __forceinline__ CamPoint cam_unproject(float d, float fl, const Exact
 constexpr int PROJ_THREADS = 256;
 constexpr int PROJ_PIX = 4;
 
-// Offsets inside one depth map are 32-bit (checked on the host); only the per-map base is 64-bit.
+// Offsets inside one depth map are 32-bit (checked on the host); only the per-map base is 64-bit.  The posed views read
+// C, sC and fC as V, sV and fV, and their cameras from CamPoseArgs (cd_in unused).
 struct CamProjArgs {
   const float *depth;
   int C, H, W;
@@ -72,9 +120,16 @@ struct CamProjArgs {
   int fast_shift;
 };
 
-// the project stage of one CTA: pixels [bx * 1024, bx * 1024 + 1024) of map `map`
-template <bool W_FAST>
-__device__ __forceinline__ void cam_project_body(const CamProjArgs &a, int bx, int map, unsigned *s_hist) {
+struct CamPoseArgs {
+  const float *rot, *eye;  // 9 and 3 contiguous floats per view
+  long long rN, rV, eN, eV;
+};
+
+// the project stage of one CTA: pixels [bx * 1024, bx * 1024 + 1024) of one image, emitted into map `map` (fixed camera:
+// image (n, c) with map = n C + c and view = 0; posed views: image (n = map, v = view))
+template <bool W_FAST, bool POSED>
+__device__ __forceinline__ void cam_project_body(const CamProjArgs &a, const CamPoseArgs &pa, int bx, int map, int view,
+                                                 unsigned *s_hist) {
   const float *__restrict__ depth = a.depth;
   const float *__restrict__ fl_in = a.fl_in;
   const float *__restrict__ cd_in = a.cd_in;
@@ -82,15 +137,17 @@ __device__ __forceinline__ void cam_project_body(const CamProjArgs &a, int bx, i
   const long long sN = a.sN, sC = a.sC, fN = a.fN, fC = a.fC, dN = a.dN, dC = a.dC;
   const float qscale = a.qscale;
   const VoxWorkspace &ws = a.ws;
-  int n = map, c = 0;
-  if (C != 1) {
+  int n = map, c = view;
+  if (!POSED && C != 1) {
     n = map / C;
     c = map - n * C;
   }
   const int P = H * W;
   const float *dmap = depth + n * sN + c * sC;
   const float fl = fl_in[n * fN + c * fC];
-  const float cam_dist = cd_in[n * dN + c * dC];
+  CamFrame cam;
+  if (POSED) cam = cam_frame_posed(pa.rot + n * pa.rN + c * pa.rV, pa.eye + n * pa.eN + c * pa.eV);
+  else cam.cam_dist = cd_in[n * dN + c * dC];
   const ExactDivisor dfl = make_divisor(fl);
   const VoxGrid grid = make_grid(R);
   const float Hm1 = __fadd_rn((float)H, -1.0f), Wm1 = __fadd_rn((float)W, -1.0f);
@@ -99,12 +156,24 @@ __device__ __forceinline__ void cam_project_body(const CamProjArgs &a, int bx, i
   // A pixel with depth exactly 0 (GenRe's background, depth_pred_with_sph_inpaint.py:139) unprojects to
   // (-cam_dist, -+0, -+0) whatever its position: z = 0 * cos = 0, gy = (w~ * -0) / fl = -+0.  Whether that point is
   // inside the grid is therefore a property of the map, evaluated once with the same operations; when it is
-  // outside (any camera further than 0.5 from the origin) such pixels skip the whole unprojection.
+  // outside (any camera further than 0.5 from the origin) such pixels skip the whole unprojection.  A posed view's
+  // zero-depth point is its eye (g_i = +-0 + e_i), given finite rot entries.
   bool zero_in_bounds;
   {
-    const int ix0 = floor_i_ref(__fmul_rn(__fadd_rn(__fadd_rn(0.0f, -cam_dist), 0.5f), grid.Rf));
-    const int iyz0 = floor_i_ref(__fmul_rn(0.5f, grid.Rf));
-    zero_in_bounds = (ix0 >= 0) & (ix0 < R) & (iyz0 >= 0) & (iyz0 < R);
+    if (POSED) {
+      int i0[3];
+      bool finite = true;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) i0[i] = floor_i_ref(__fmul_rn(__fadd_rn(__fadd_rn(0.0f, cam.e[i]), 0.5f), grid.Rf));
+#pragma unroll
+      for (int i = 0; i < 9; ++i) finite &= fabsf(cam.r[i]) <= 3.402823466e38f;
+      zero_in_bounds = (i0[0] >= 0) & (i0[0] < R) & (i0[1] >= 0) & (i0[1] < R) & (i0[2] >= 0) & (i0[2] < R);
+      if (!finite) zero_in_bounds = true;  // 0 * inf: no shortcut
+    } else {
+      const int ix0 = floor_i_ref(__fmul_rn(__fadd_rn(__fadd_rn(0.0f, -cam.cam_dist), 0.5f), grid.Rf));
+      const int iyz0 = floor_i_ref(__fmul_rn(0.5f, grid.Rf));
+      zero_in_bounds = (ix0 >= 0) & (ix0 < R) & (iyz0 >= 0) & (iyz0 < R);
+    }
     const float afl = fabsf(fl);
     if (!(afl >= 0x1p-40f && afl <= 0x1p40f)) zero_in_bounds = true;  // degenerate focal length: no shortcut
   }
@@ -133,7 +202,7 @@ __device__ __forceinline__ void cam_project_body(const CamProjArgs &a, int bx, i
     if (!(d[k] < 0.0f) && (zero_in_bounds || d[k] != 0.0f)) {
       int h, w;
       coords(p0 + k * PROJ_THREADS, h, w);
-      const CamPoint pt = cam_unproject(d[k], fl, dfl, cam_dist, h, w, Hm1, Wm1, R, grid.Rf);
+      const CamPoint pt = cam_unproject<POSED>(d[k], fl, dfl, cam, h, w, Hm1, Wm1, R, grid.Rf);
       if (pt.in_bounds) {
         const float dx = __fadd_rn(pt.gx, -vox_centre(pt.ix, grid));
         const float dy = __fadd_rn(pt.gy, -vox_centre(pt.iy, grid));
@@ -144,7 +213,8 @@ __device__ __forceinline__ void cam_project_body(const CamProjArgs &a, int bx, i
       }
     }
   }
-  vox_emit<PROJ_PIX, PROJ_THREADS>(gv, q, map, ws, P, s_hist);
+  // a posed map holds V images: the overflow list is sized by the map's V H W pixels
+  vox_emit<PROJ_PIX, PROJ_THREADS>(gv, q, map, ws, POSED ? (long long)C * P : P, s_hist);
 }
 
 template <bool W_FAST>
@@ -152,14 +222,23 @@ __global__ void __launch_bounds__(PROJ_THREADS)
 cam_project_kernel(const CamProjArgs a) {
   extern __shared__ unsigned s_hist[];  // [ntiles] CTA-local tile histogram
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // let the splat grid start launching behind us
-  cam_project_body<W_FAST>(a, blockIdx.x, blockIdx.y, s_hist);
+  cam_project_body<W_FAST, false>(a, CamPoseArgs{}, blockIdx.x, blockIdx.y, 0, s_hist);
+}
+
+// posed views: grid (CTAs per view, V, N); every view of grid n emits into map n
+template <bool W_FAST>
+__global__ void __launch_bounds__(PROJ_THREADS)
+cam_project_views_kernel(const CamProjArgs a, const CamPoseArgs pa) {
+  extern __shared__ unsigned s_hist[];
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  cam_project_body<W_FAST, true>(a, pa, blockIdx.x, blockIdx.z, blockIdx.y, s_hist);
 }
 
 template <bool W_FAST>
 struct CamProjector {   // project stage of the overlapped kernel (voxelize.cuh vox_overlap_kernel)
   using Args = CamProjArgs;
   static __device__ __forceinline__ void run(const Args &a, int bx, int map, unsigned *s_hist) {
-    cam_project_body<W_FAST>(a, bx, map, s_hist);
+    cam_project_body<W_FAST, false>(a, CamPoseArgs{}, bx, map, 0, s_hist);
   }
 };
 
@@ -216,20 +295,57 @@ static int cam_project_launch(const float *depth, int64_t N, int64_t C, int64_t 
   return check_launch("cam_bp project kernel");
 }
 
+// the posed views' arguments: depth [N, V, H, W], each view's camera at (n, v); 0 or a GENRE_B200_E* code
+static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+static int cam_views_check(const char *what, const float *depth, int64_t N, int64_t V, int64_t H, int64_t W,
+                           const float *fl, const float *rot, const float *eye, int res) {
+  GB_REQUIRE(depth && fl && rot && eye, GENRE_B200_EINVAL, "%s: null input pointer", what);
+  GB_REQUIRE(N > 0 && V > 0 && H > 0 && W > 0, GENRE_B200_EINVAL, "%s: empty depth tensor [%lld,%lld,%lld,%lld]", what,
+             (long long)N, (long long)V, (long long)H, (long long)W);
+  GB_REQUIRE(H < (1 << 20) && W < (1 << 20), GENRE_B200_EINVAL, "%s: image too large", what);
+  GB_REQUIRE(N <= 65535 && V <= 65535, GENRE_B200_EINVAL, "%s: N = %lld and V = %lld must be at most 65535", what,
+             (long long)N, (long long)V);
+  // the splat's 20-bit count field bounds the points of one grid
+  GB_REQUIRE(V * H * W <= VOX_MAX_PIXELS, GENRE_B200_EINVAL, "%s: V*H*W = %lld must be below 2^20", what,
+             (long long)(V * H * W));
+  GB_REQUIRE(aligned4(depth) && aligned4(fl) && aligned4(rot) && aligned4(eye), GENRE_B200_EALIGN,
+             "%s: depth, fl, rot and eye must be 4-byte aligned", what);
+  return vox_check_common(N, V * H * W, res);
+}
+
+static int cam_views_project_launch(const float *depth, int64_t N, int64_t V, int64_t H, int64_t W, int64_t sN, int64_t sV,
+                                    int64_t sH, int64_t sW, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                    int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, int res,
+                                    const VoxWorkspace &w, cudaStream_t st) {
+  CamProjArgs a;
+  bool w_fast = true;
+  if (int rc = cam_proj_args(depth, N, V, H, W, sN, sV, sH, sW, fl, fN, fV, nullptr, 0, 0, res, w, &a, &w_fast)) return rc;
+  const CamPoseArgs pa{rot, eye, rN, rV, eN, eV};
+  dim3 grid((unsigned)cam_proj_ctas_per_map(H * W), (unsigned)V, (unsigned)N);
+  const size_t smem = (size_t)w.ntiles * 4;
+  if (w_fast) cam_project_views_kernel<true><<<grid, PROJ_THREADS, smem, st>>>(a, pa);
+  else cam_project_views_kernel<false><<<grid, PROJ_THREADS, smem, st>>>(a, pa);
+  return check_launch("cam_bp views project kernel");
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward: one thread per pixel, gathers cnt / grad at its voxel
 // (reference :365-471; cam_dist read with its own strides, not the :401 stride mix-up)
 // ------------------------------------------------------------------------------------------------
 constexpr int BWD_THREADS = 256;
 
+// POSED: grid (CTAs per view, V, N), C, sC, fC read as V, sV, fV; cnt and grad_tdf of grid n; grad_fl, grad_cd unused
+template <bool POSED>
 __global__ void __launch_bounds__(BWD_THREADS)
 cam_bp_backward_kernel(const float *__restrict__ depth, int C, int H, int W, long long sN, long long sC, long long sH,
                        long long sW, const float *__restrict__ fl_in, long long fN, long long fC,
                        const float *__restrict__ cd_in, long long dN, long long dC, const float *__restrict__ cnt,
                        const float *__restrict__ grad_tdf, int R, float *__restrict__ grad_depth,
-                       float *__restrict__ grad_fl, float *__restrict__ grad_cd) {
-  const int map = blockIdx.y;
-  const int n = map / C, c = map - n * C;
+                       float *__restrict__ grad_fl, float *__restrict__ grad_cd, const CamPoseArgs pa) {
+  const int map = POSED ? (int)(blockIdx.z * C + blockIdx.y) : (int)blockIdx.y;  // the image; grad_depth's index
+  const int n = POSED ? (int)blockIdx.z : map / C, c = POSED ? (int)blockIdx.y : map - n * C;
+  const int vol = POSED ? n : map;  // the volume of cnt / grad_tdf it reads
   const int P = H * W;
   const int p = blockIdx.x * BWD_THREADS + threadIdx.x;  // dense grad_depth index: h * W + w
   float g_depth = 0.0f, g_fl = 0.0f, g_cd = 0.0f;
@@ -238,10 +354,12 @@ cam_bp_backward_kernel(const float *__restrict__ depth, int C, int H, int W, lon
     const float d = depth[n * sN + c * sC + h * sH + w * sW];
     if (!(d < 0.0f)) {
       const float fl = fl_in[n * fN + c * fC];
-      const float cam_dist = cd_in[n * dN + c * dC];
+      CamFrame cam;
+      if (POSED) cam = cam_frame_posed(pa.rot + n * pa.rN + c * pa.rV, pa.eye + n * pa.eN + c * pa.eV);
+      else cam.cam_dist = cd_in[n * dN + c * dC];
       const float Rf = (float)R;
-      const CamPoint pt = cam_unproject(d, fl, make_divisor(fl), cam_dist, h, w, __fadd_rn((float)H, -1.0f),
-                                        __fadd_rn((float)W, -1.0f), R, Rf);
+      const CamPoint pt = cam_unproject<POSED>(d, fl, make_divisor(fl), cam, h, w, __fadd_rn((float)H, -1.0f),
+                                               __fadd_rn((float)W, -1.0f), R, Rf);
       if (pt.in_bounds) {
         // voxel centre: the reference's backward evaluates this in double (literals 0.5), :428-430
         const float cx = (float)((((double)(float)pt.ix + 0.5) / (double)Rf) - 0.5);
@@ -249,41 +367,54 @@ cam_bp_backward_kernel(const float *__restrict__ depth, int C, int H, int W, lon
         const float cz = (float)((((double)(float)pt.iz + 0.5) / (double)Rf) - 0.5);
         float len = pt.norm;
         if ((double)len < 1e-5) len = 1e-5f;
-        const float dirx = -fl / len, diry = pt.imw / len, dirz = pt.imh / len;
+        float dirx = -fl / len, diry = pt.imw / len, dirz = pt.imh / len;
+        if (POSED) {  // the camera-frame direction in the grid frame, in the unprojection's fma order
+          const float x = dirx, y = diry, z = dirz;
+          dirx = cam_rotate(cam, 0, x, y, z);
+          diry = cam_rotate(cam, 1, x, y, z);
+          dirz = cam_rotate(cam, 2, x, y, z);
+        }
         const float ex = pt.gx - cx, ey = pt.gy - cy, ez = pt.gz - cz;
-        float vlen = sqrtf(ex * ex + ey * ey + ez * ez);
+        // POSED states the contractions nvcc 12.9 makes of the fixed instantiation's expressions (read off its SASS), so
+        // that the identity pose reproduces it bit for bit
+        float vlen = POSED ? sqrtf(__fmaf_rn(ez, ez, __fmaf_rn(ex, ex, __fmul_rn(ey, ey)))) : sqrtf(ex * ex + ey * ey + ez * ez);
         if ((double)vlen < 1e-5) vlen = 1e-5f;
         const float ux = ex / vlen, uy = ey / vlen, uz = ez / vlen;
-        const float cos_cc = dirx * ux + diry * uy + dirz * uz;
-        const size_t v = (size_t)map * R * R * R + ((size_t)pt.ix * R + pt.iy) * R + pt.iz;
+        const float cos_cc = POSED ? __fmaf_rn(dirz, uz, __fmaf_rn(diry, uy, __fmul_rn(dirx, ux)))
+                                   : dirx * ux + diry * uy + dirz * uz;
+        const size_t v = (size_t)vol * R * R * R + ((size_t)pt.ix * R + pt.iy) * R + pt.iz;
         float ptnum = cnt[v];
         if (ptnum < 1.0f) ptnum = 1.0f;
         const float gd = grad_tdf[v];
         g_depth = -gd * cos_cc / ptnum;
-        const float len3 = len * len * len;
-        const float gfx = ux * (pt.imw * pt.imw + pt.imh * pt.imh) / len3;
-        const float gfy = uy * (pt.imw * fl) / len3;
-        const float gfz = uz * (pt.imh * fl) / len3;
-        g_fl = (gfx + gfy + gfz) * gd * d / ptnum;
-        g_cd = -ux * gd / ptnum;
+        if (!POSED) {
+          const float len3 = len * len * len;
+          const float gfx = ux * (pt.imw * pt.imw + pt.imh * pt.imh) / len3;
+          const float gfy = uy * (pt.imw * fl) / len3;
+          const float gfz = uz * (pt.imh * fl) / len3;
+          g_fl = (gfx + gfy + gfz) * gd * d / ptnum;
+          g_cd = -ux * gd / ptnum;
+        }
       }
     }
     grad_depth[(size_t)map * P + p] = g_depth;
   }
-  // block reduction of the two per-map scalars, then one atomic per CTA (reference: one per pixel, :464,469)
-  __shared__ float s_fl[BWD_THREADS / 32], s_cd[BWD_THREADS / 32];
+  if (!POSED) {
+    // block reduction of the two per-map scalars, then one atomic per CTA (reference: one per pixel, :464,469)
+    __shared__ float s_fl[BWD_THREADS / 32], s_cd[BWD_THREADS / 32];
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    g_fl += __shfl_xor_sync(0xffffffffu, g_fl, o);
-    g_cd += __shfl_xor_sync(0xffffffffu, g_cd, o);
-  }
-  if ((threadIdx.x & 31) == 0) { s_fl[threadIdx.x >> 5] = g_fl; s_cd[threadIdx.x >> 5] = g_cd; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float a = 0.f, b = 0.f;
-    for (int i = 0; i < BWD_THREADS / 32; ++i) { a += s_fl[i]; b += s_cd[i]; }
-    if (a != 0.0f) atomicAdd(grad_fl + map, a);
-    if (b != 0.0f) atomicAdd(grad_cd + map, b);
+    for (int o = 16; o > 0; o >>= 1) {
+      g_fl += __shfl_xor_sync(0xffffffffu, g_fl, o);
+      g_cd += __shfl_xor_sync(0xffffffffu, g_cd, o);
+    }
+    if ((threadIdx.x & 31) == 0) { s_fl[threadIdx.x >> 5] = g_fl; s_cd[threadIdx.x >> 5] = g_cd; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float a = 0.f, b = 0.f;
+      for (int i = 0; i < BWD_THREADS / 32; ++i) { a += s_fl[i]; b += s_cd[i]; }
+      if (a != 0.0f) atomicAdd(grad_fl + map, a);
+      if (b != 0.0f) atomicAdd(grad_cd + map, b);
+    }
   }
 }
 
@@ -358,6 +489,22 @@ using namespace gb;
 // ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
+// sum_q / count is the mean distance in units of 2^-24 voxel edges.
+//   raw  : tdf = mean               , background 1/R (cam_back_projection.py:23-24 + kernel bias :304,:829)
+//   shift: tdf = 1 - R * mean       , background 1 - R * (1/R)   (camera_backprojection_module.py:26-28)
+static void cam_tdf_affine(unsigned flags, int res, float *alpha, float *beta, float *bg) {
+  const float inv_r = (float)(1.0 / (double)res);
+  if (flags & GENRE_B200_FLAG_SHIFT_TDF) {
+    *alpha = 1.0f;
+    *beta = -(1.0f / 16777216.0f);
+    *bg = 1.0f - (float)res * inv_r;
+  } else {
+    *alpha = 0.0f;
+    *beta = (float)((1.0 / 16777216.0) / (double)res);
+    *bg = inv_r;
+  }
+}
+
 extern "C" int genre_b200_cam_bp_stage_project(const float *depth, int64_t N, int64_t C, int64_t H, int64_t W,
                                                int64_t sN, int64_t sC, int64_t sH, int64_t sW, const float *fl,
                                                int64_t fN, int64_t fC, const float *camdist, int64_t dN, int64_t dC,
@@ -381,20 +528,8 @@ extern "C" int genre_b200_cam_bp_forward(const float *depth, int64_t N, int64_t 
   GB_REQUIRE(vox_carve(workspace, workspace_bytes, N * C, H * W, res, &w), GENRE_B200_EWORKSPACE,
              "cam_bp: workspace too small or misaligned (need %zu bytes)", vox_workspace_bytes(N * C, H * W, res));
   cudaStream_t st = as_stream(stream);
-  // sum_q / count is the mean distance in units of 2^-24 voxel edges.
-  //   raw  : tdf = mean               , background 1/R (cam_back_projection.py:23-24 + kernel bias :304,:829)
-  //   shift: tdf = 1 - R * mean       , background 1 - R * (1/R)   (camera_backprojection_module.py:26-28)
-  const float inv_r = (float)(1.0 / (double)res);
   float alpha, beta, bg;
-  if (flags & GENRE_B200_FLAG_SHIFT_TDF) {
-    alpha = 1.0f;
-    beta = -(1.0f / 16777216.0f);
-    bg = 1.0f - (float)res * inv_r;
-  } else {
-    alpha = 0.0f;
-    beta = (float)((1.0 / 16777216.0) / (double)res);
-    bg = inv_r;
-  }
+  cam_tdf_affine(flags, res, &alpha, &beta, &bg);
   if (int rc = vox_clear_counts(w, N * C, st)) return rc;
   if (flags & GENRE_B200_FLAG_OVERLAP) {
     // experimental, off by default (measured slower): project and splat in ONE kernel with an interleaved block order
@@ -428,10 +563,49 @@ extern "C" int genre_b200_cam_bp_backward(const float *depth, int64_t N, int64_t
   }
   const int64_t P = H * W;
   dim3 grid((unsigned)((P + BWD_THREADS - 1) / BWD_THREADS), (unsigned)(N * C));
-  cam_bp_backward_kernel<<<grid, BWD_THREADS, 0, st>>>(depth, (int)C, (int)H, (int)W, sN, sC, sH, sW, fl, fN, fC,
-                                                       camdist, dN, dC, cnt, grad_tdf, res, grad_depth, grad_fl,
-                                                       grad_camdist);
+  cam_bp_backward_kernel<false><<<grid, BWD_THREADS, 0, st>>>(depth, (int)C, (int)H, (int)W, sN, sC, sH, sW, fl, fN,
+                                                              fC, camdist, dN, dC, cnt, grad_tdf, res, grad_depth,
+                                                              grad_fl, grad_camdist, CamPoseArgs{});
   return check_launch("cam_bp backward kernel");
+}
+
+extern "C" int genre_b200_cam_bp_views_forward(const float *depth, int64_t N, int64_t V, int64_t H, int64_t W, int64_t sN,
+                                               int64_t sV, int64_t sH, int64_t sW, const float *fl, int64_t fN,
+                                               int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                               int64_t eN, int64_t eV, float *tdf, float *cnt, int res, unsigned flags,
+                                               void *workspace, size_t workspace_bytes, void *stream) {
+  const char *what = "cam_bp_views";
+  if (int rc = cam_views_check(what, depth, N, V, H, W, fl, rot, eye, res)) return rc;
+  GB_REQUIRE(tdf != nullptr, GENRE_B200_EINVAL, "%s: tdf is null", what);
+  GB_REQUIRE((flags & ~GENRE_B200_FLAG_SHIFT_TDF) == 0u, GENRE_B200_EINVAL,
+             "%s: flags 0x%x unsupported (only GENRE_B200_FLAG_SHIFT_TDF)", what, flags);
+  const int64_t P = V * H * W;
+  VoxWorkspace w;
+  GB_REQUIRE(vox_carve(workspace, workspace_bytes, N, P, res, &w), GENRE_B200_EWORKSPACE,
+             "%s: workspace too small or misaligned (need %zu bytes)", what, vox_workspace_bytes(N, P, res));
+  cudaStream_t st = as_stream(stream);
+  float alpha, beta, bg;
+  cam_tdf_affine(flags, res, &alpha, &beta, &bg);
+  if (int rc = vox_clear_counts(w, N, st)) return rc;
+  if (int rc = cam_views_project_launch(depth, N, V, H, W, sN, sV, sH, sW, fl, fN, fV, rot, rN, rV, eye, eN, eV, res, w, st))
+    return rc;
+  return vox_splat(w, N, P, res, tdf, cnt, alpha, beta, bg, st);
+}
+
+extern "C" int genre_b200_cam_bp_views_backward(const float *depth, int64_t N, int64_t V, int64_t H, int64_t W, int64_t sN,
+                                                int64_t sV, int64_t sH, int64_t sW, const float *fl, int64_t fN,
+                                                int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                int64_t eN, int64_t eV, const float *cnt, const float *grad_tdf, int res,
+                                                float *grad_depth, void *stream) {
+  const char *what = "cam_bp_views backward";
+  if (int rc = cam_views_check(what, depth, N, V, H, W, fl, rot, eye, res)) return rc;
+  GB_REQUIRE(cnt && grad_tdf && grad_depth, GENRE_B200_EINVAL, "%s: null pointer", what);
+  const CamPoseArgs pa{rot, eye, rN, rV, eN, eV};
+  dim3 grid((unsigned)((H * W + BWD_THREADS - 1) / BWD_THREADS), (unsigned)V, (unsigned)N);
+  cam_bp_backward_kernel<true><<<grid, BWD_THREADS, 0, as_stream(stream)>>>(
+      depth, (int)V, (int)H, (int)W, sN, sV, sH, sW, fl, fN, fV, nullptr, 0, 0, cnt, grad_tdf, res, grad_depth, nullptr,
+      nullptr, pa);
+  return check_launch("cam_bp views backward kernel");
 }
 
 extern "C" int genre_b200_surface_mask(const float *depth, int64_t N, int64_t C, int64_t H, int64_t W, int64_t sN,

@@ -25,6 +25,7 @@ import math
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -1243,3 +1244,74 @@ def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, 
         loss = _RayConsistency.apply(vox, v, keep + (obs_depth,), args, tuple(obs_depth.shape),
                                      "genre_b200_ray_consistency_views")
     return loss.mean((1, 2, 3)) if reduction == "mean" else loss
+
+
+# ---- any camera's depth map into a grid: posed multi-view back-projection -------------------------------------------------
+class _BackProjectViews(torch.autograd.Function):
+    """``genre_b200_cam_bp_views_*``: ``args`` are the entry points' leading arguments (depth to eye strides), ``keep``
+    the pose tensors they point into; the count volume is written only when ``depth`` can receive a gradient"""
+    @staticmethod
+    def forward(ctx, depth, keep, args, res, shift):
+        N, V, H, W = args[1:5]
+        tdf = torch.empty((N, 1, res, res, res), dtype=torch.float32, device=depth.device)
+        cnt = torch.empty_like(tdf) if ctx.needs_input_grad[0] else None
+        ws, nbytes = _lib.workspace_for(N, V * H * W, res, depth.device)
+        _lib.call("genre_b200_cam_bp_views_forward", *args, tdf.data_ptr(), None if cnt is None else cnt.data_ptr(), res,
+                  _lib.FLAG_SHIFT_TDF if shift else 0, ws.data_ptr(), nbytes, _lib.stream_ptr(depth))
+        if cnt is not None:
+            ctx.save_for_backward(depth, cnt, *keep)
+        ctx.args, ctx.res, ctx.shift = args, res, shift
+        return tdf
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_tdf):
+        depth, cnt = ctx.saved_tensors[:2]
+        g = grad_tdf * (-float(ctx.res)) if ctx.shift else grad_tdf    # d(1 - R mean) = -R d mean
+        g = g.contiguous()
+        grad = torch.empty(depth.shape, dtype=torch.float32, device=depth.device)
+        _lib.call("genre_b200_cam_bp_views_backward", *ctx.args, cnt.data_ptr(), g.data_ptr(), ctx.res, grad.data_ptr(),
+                  _lib.stream_ptr(depth))
+        return grad, None, None, None, None
+
+
+def back_project_views(depth, rot, eye, fl=CAM_FL, res=128, shift=True):
+    """Back-project V depth maps per grid, each from its own camera, into one TDF grid: cam_bp with per-view extrinsics.
+
+    depth [N,V,H,W] fp32 on CUDA (any strides): ray depth from each view's eye, as cam_bp's input; pixels with depth < 0
+    are skipped, as in cam_bp.  ``rot`` [N|1,V,3,3], ``eye`` [N|1,V,3] and ``fl`` (a float, [V] or [N,V]) are cameras
+    exactly as in ``render_depth_views`` (same frame and validation; a leading 1 shares them across the batch; host or
+    device), so pixel (h, w) at depth d lands on ``render_depth_views``' ray of that pixel at t = d.  V*H*W must be below
+    2^20 (15 views at 256^2, 63 at 128^2).
+
+    Returns tdf [N,1,R,R,R], R = ``res``: on voxels that some view's point fell in, 1 - R * (mean point-to-centre
+    distance over the points of all views) with ``shift=True`` (what ``Camera_back_projection_layer`` feeds GenRe),
+    the raw mean with ``shift=False``; elsewhere cam_bp's background.  The output is bitwise reproducible and does not
+    depend on the order of the views.  rot = I, eye = (-cam_dist, 0, 0) (``look_at((-CAM_DIST, 0, 0))``) reproduces
+    ``Camera_back_projection_layer`` bit for bit.  For one grid per view, fold the views into the batch:
+    ``back_project_views(d.reshape(N * V, 1, H, W), rot.reshape(N * V, 1, 3, 3), eye.reshape(N * V, 1, 3))``.
+
+    Differentiable in ``depth`` (cam_bp's depth gradient along each view's ray); ``rot``, ``eye`` and ``fl`` are not
+    differentiated (ValueError if one requires grad)."""
+    name = "back_project_views"
+    if depth.dim() != 4:
+        raise ValueError("%s: depth [N,V,H,W] expected, got %s" % (name, tuple(depth.shape)))
+    N, V, H, W = depth.shape
+    if V * H * W >= 1 << 20:
+        raise ValueError("%s: V*H*W = %d must be below 2^20 (the splat's per-voxel count field)" % (name, V * H * W))
+    for x, what in ((rot, "rot"), (eye, "eye"), (fl, "fl")):
+        if isinstance(x, torch.Tensor) and x.requires_grad:
+            raise ValueError("%s: %s requires grad, but the camera is not differentiated (pass %s.detach())"
+                             % (name, what, what))
+    r, e, f, Vp = _poses(N, rot, eye, fl, name)
+    if Vp != V:
+        raise ValueError("%s: depth has %d views but rot %d" % (name, V, Vp))
+    _lib.require_cuda(depth)
+    _lib.require_f32(depth)
+    r, e, f = (x.to(depth.device).contiguous() for x in (r, e, f))
+
+    def nv(x):                                       # strides over (n, v); 0 over n for cameras shared by the batch
+        return (x.stride(0) if x.shape[0] > 1 else 0), x.stride(1)
+    args = (depth.data_ptr(), N, V, H, W) + tuple(depth.stride()) + (f.data_ptr(),) + nv(f) + (r.data_ptr(),) + nv(r) + \
+        (e.data_ptr(),) + nv(e)
+    return _BackProjectViews.apply(depth, (r, e, f), args, int(res), bool(shift))

@@ -89,6 +89,40 @@ int genre_b200_surface_mask(const float *depth, int64_t N, int64_t C, int64_t H,
                             const float *camdist, int64_t dN, int64_t dC,
                             const float *cnt, float *mask, int res, void *stream);
 
+/* Posed multi-view back-projection: V depth maps per grid, each from its own camera, fused into one TDF grid.
+ *   depth   [N, V, H, W]  any strides (sN,sV,sH,sW); ray depth from the view's eye, pixels with depth < 0 skipped
+ *   fl[n*fN + v*fV], rot + n*rN + v*rV (9 floats), eye + n*eN + v*eV (3 floats): view (n, v)'s camera in the frame
+ *           of genre_b200_render_views_forward (rot row-major, its columns the camera's axes in the grid frame: x
+ *           forward, image w towards -y, image h towards -z; eye the camera's centre).  Strides in elements; 0 over n
+ *           shares one camera set across the batch.
+ *   tdf, cnt [N, 1, R, R, R] as genre_b200_cam_bp_forward (cnt may be NULL); flags: GENRE_B200_FLAG_SHIFT_TDF only.
+ *   workspace genre_b200_voxelize_workspace_bytes(N, V*H*W, R) bytes.
+ * Pixel (h, w) of view v is unprojected into the camera frame exactly as genre_b200_cam_bp_forward does (z = d cos,
+ * cy = (imw * -z) / fl, cz = (imh * -z) / fl), then moved into the grid frame in fp32, every operation rounded to
+ * nearest in this order:  g_i = fma(rot[i][2], cz, fma(rot[i][1], cy, rot[i][0] * z)) + eye_i.  The voxel index,
+ * centre distance and quantisation are genre_b200_cam_bp_forward's, and the point lies on
+ * genre_b200_render_views_forward's ray of that pixel at t = d.  All V views of grid n are splatted into grid n: a
+ * voxel's value is the mean distance over every point any view put in it, and the integer sums make the output
+ * bitwise reproducible and independent of the order of the views.  rot = I and eye = (-cam_dist, 0, 0) reproduce
+ * genre_b200_cam_bp_forward bit for bit.  Limits: 1 <= N, V <= 65535, V*H*W < 2^20 (the splat's 20-bit count),
+ * every input pointer 4-byte aligned (else GENRE_B200_EALIGN); arguments are checked before any launch.
+ * Two kernel launches. */
+int genre_b200_cam_bp_views_forward(const float *depth, int64_t N, int64_t V, int64_t H, int64_t W,
+                                    int64_t sN, int64_t sV, int64_t sH, int64_t sW,
+                                    const float *fl, int64_t fN, int64_t fV,
+                                    const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                    float *tdf, float *cnt, int res, unsigned flags,
+                                    void *workspace, size_t workspace_bytes, void *stream);
+/* The depth gradient of the above: grad_depth [N, V, H, W] dense, fully written, from cnt and grad_tdf [N, 1, R, R, R]
+ * dense.  The formula is genre_b200_cam_bp_backward's with the ray direction (-fl, imw, imh) / len rotated by rot in
+ * the forward's fma order; at the identity pose it equals that backward's grad_depth bit for bit.  fl, rot and eye are
+ * not differentiated.  One kernel launch. */
+int genre_b200_cam_bp_views_backward(const float *depth, int64_t N, int64_t V, int64_t H, int64_t W,
+                                     int64_t sN, int64_t sV, int64_t sH, int64_t sW,
+                                     const float *fl, int64_t fN, int64_t fV,
+                                     const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                     const float *cnt, const float *grad_tdf, int res, float *grad_depth, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Spherical back-projection, spherical depth map -> voxel TDF + count.
  * Replaces spherical_back_proj_forward / _backward (back_projection.h:4-5,

@@ -464,6 +464,228 @@ __global__ void __launch_bounds__(RC_THREADS) render_views_pose_reduce_kernel(co
   }
 }
 
+// ---- surface normals of the posed views (the *normal*_views entry points; tests/render_normal_ref.py restates them) ----
+// The cameras, rays, samples t_k, f_k, taps, p_k, T_k and s_k are the posed views' above, with the same arithmetic.
+//   sample normal     g_k = Res d raw / d f at f_k (sample_trilinear_grad, the cell make_taps_at selects, zero padding),
+//                     rho_k = sqrt(|g_k|^2 + eps^2),  n_k = -g_k / rho_k  (outward: occupancy falls along n).  A NaN raw
+//                     gives p_k = 1e-5 (the clamp's) and n_k = 0.  In fp32: rho = sqrtf(fma(gz,gz, fma(gy,gy,
+//                     fma(gx,gx, eps*eps)))), n = -g / rho (one division per component).
+//   rendered normal   normal = rot^T (sum_k s_k n_k): the sum in the grid frame, rotated once per ray after the warp
+//                     reduction, normal_j = fma(rot[2][j], S_2, fma(rot[1][j], S_1, rot[0][j] S_0)).  Not renormalised;
+//                     an escaping ray contributes 0.  Camera frame: x forward, +y towards image -w, +z towards image -h.
+//   consistency       obs o [3] in the same camera frame; o = 0 (all three exactly 0) is background.  Otherwise
+//                     m = rot o / |o| formed in fp64 ((rot[i][0] o_0 + rot[i][1] o_1) + rot[i][2] o_2, divided by
+//                     sqrt((o_0^2 + o_1^2) + o_2^2)) and rounded once to fp32.  Foreground: c_k = 1 - n_k . m (the dot
+//                     product an fma chain x, y, z), c_esc = miss; background: c_k = miss, c_esc = 0.
+// Both modes are one cost family: c_k = c0 - n_k . a (render: a = -rot G, c0 = 0, per unit upstream G; consistency
+// foreground: a = m, c0 = 1), whose gradient in g is d c_k / d g_k = (a - g_k (g_k . a) / rho_k^2) / rho_k.  rot G is
+// formed like m (fp64, rounded once).  The grid gradient has two paths through the same 8 taps:
+//   p path  dp_k = scale (T_k c_k - A_k / (1 - p_k)), zero where the clamp is active or raw is NaN (the posed walk's);
+//   n path  at every sample with s_k != 0 (clamped or not, not NaN): h_k = scale s_k Res d c_k / d g_k, tap i gets
+//           h_k . grad_f w_i (the 1-D weights' derivatives, +-1 times the two other axes' weights);
+// summed into one atomicAdd per valid tap.  rot, eye, fl, obs and eps are not differentiated.
+struct NormArgs {
+  CamArgs c;          // posed cameras, Z, miss; c.g0 = upstream grad (render [N,V,3,H,W] dense, loss [N,V,H,W] dense)
+  const float *obsn;  // consistency: observed normals [N,V,3,H,W], strides (oN, oV, oC, oH, oW)
+  long long oN, oV, oC, oH, oW;
+  float eps;
+  float *out;         // forward: normal [N,V,3,H,W] or loss [N,V,H,W], dense
+};
+
+struct NormalCost {
+  float ax, ay, az, c0, esc;
+  bool fg;  // false: every stop costs `miss` (stored in c0), the normal does not enter
+  __device__ __forceinline__ float at(float nx, float ny, float nz) const {
+    return fg ? c0 - fmaf(nz, az, fmaf(ny, ay, nx * ax)) : c0;
+  }
+};
+
+// fp32(rot v (/ |v| when normalise)) in fp64, the rounding stated above
+__device__ __forceinline__ void rot_apply64(const float *__restrict__ rot, float v0, float v1, float v2, bool normalise,
+                                            float &o0, float &o1, float &o2) {
+  const double x = v0, y = v1, z = v2;
+  const double nrm = normalise ? __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z))) : 1.0;
+  double r[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double s = __dadd_rn(__dadd_rn(__dmul_rn((double)__ldg(rot + 3 * i), x), __dmul_rn((double)__ldg(rot + 3 * i + 1), y)),
+                               __dmul_rn((double)__ldg(rot + 3 * i + 2), z));
+    r[i] = normalise ? __ddiv_rn(s, nrm) : s;
+  }
+  o0 = (float)r[0];
+  o1 = (float)r[1];
+  o2 = (float)r[2];
+}
+
+// sample k: p_k, the raw interpolant, g_k (grid frame, per unit length, 0 where raw is NaN), rho_k, n_k and the taps
+struct NormSample {
+  float raw, p, gx, gy, gz, rho, nx, ny, nz, t;
+  float f[3];
+};
+__device__ __forceinline__ void normal_sample(const float *__restrict__ vol, int R, const CamRay &ray, int k, float eps,
+                                              Taps &taps, NormSample &s) {
+  s.t = cam_sample<true>(ray, k, R, taps, s.f);
+  float dx, dy, dz;
+  s.raw = sample_trilinear_grad(vol, taps, R, s.f[0], s.f[1], s.f[2], dx, dy, dz);
+  s.p = fminf(fmaxf(s.raw, RS_PMIN), RS_PMAX);
+  const float Rf = (float)R;
+  const bool nan = s.raw != s.raw;
+  s.gx = nan ? 0.0f : dx * Rf;
+  s.gy = nan ? 0.0f : dy * Rf;
+  s.gz = nan ? 0.0f : dz * Rf;
+  s.rho = sqrtf(fmaf(s.gz, s.gz, fmaf(s.gy, s.gy, fmaf(s.gx, s.gx, eps * eps))));
+  s.nx = -s.gx / s.rho;
+  s.ny = -s.gy / s.rho;
+  s.nz = -s.gz / s.rho;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(RC_THREADS) render_normal_forward_kernel(const NormArgs a) {
+  const long long ray = (long long)blockIdx.x * RC_WARPS + (threadIdx.x >> 5);
+  if (ray >= a.c.n_rays) return;
+  const int lane = threadIdx.x & 31;
+  const RayIndex ri = ray_index<true>(a.c, ray);
+  const float *vol = a.c.vox + (size_t)ri.n * a.c.R * a.c.R * a.c.R;
+  const float *rot = a.c.rot + ri.n * a.c.rN + ri.v * a.c.rV;
+  const CamRay r = ray_of<true>(a.c, ri);
+  NormalCost cost{0.0f, 0.0f, 0.0f, a.c.miss, 0.0f, false};
+  if (MODE == RC_CONSISTENCY) {
+    const float *o = a.obsn + ri.n * a.oN + ri.v * a.oV + ri.h * a.oH + ri.w * a.oW;
+    const float o0 = o[0], o1 = o[a.oC], o2 = o[2 * a.oC];
+    if (o0 != 0.0f || o1 != 0.0f || o2 != 0.0f) {
+      rot_apply64(rot, o0, o1, o2, true, cost.ax, cost.ay, cost.az);
+      cost.c0 = 1.0f;
+      cost.esc = a.c.miss;
+      cost.fg = true;
+    }
+  }
+  float carry = 1.0f, acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f;
+  for (int c = 0; c * 32 < a.c.Z; ++c) {
+    const int k = c * 32 + lane;
+    NormSample s;
+    s.p = 0.0f;  // lanes past the end behave like p = 0 (factor 1, no contribution)
+    if (k < a.c.Z) {
+      Taps t;
+      normal_sample(vol, a.c.R, r, k, a.eps, t, s);
+    }
+    float total;
+    const float before = carry * warp_excl_prod32(1.0f - s.p, total);
+    if (k < a.c.Z) {
+      const float sk = s.p * before;
+      if (MODE == RC_RENDER) {
+        acc0 = fmaf(sk, s.nx, acc0);
+        acc1 = fmaf(sk, s.ny, acc1);
+        acc2 = fmaf(sk, s.nz, acc2);
+      } else {
+        acc0 = fmaf(sk, cost.at(s.nx, s.ny, s.nz), acc0);
+      }
+    }
+    carry *= total;
+    if (carry == 0.0f) break;  // warp-uniform
+  }
+  acc0 = warp_sum(acc0);
+  if (MODE == RC_RENDER) {
+    acc1 = warp_sum(acc1);
+    acc2 = warp_sum(acc2);
+    if (lane < 3) {
+      const long long hw = (long long)a.c.H * a.c.W, nv = ray / hw, pix = ray - nv * hw;
+      const float v = fmaf(__ldg(rot + 6 + lane), acc2, fmaf(__ldg(rot + 3 + lane), acc1, __ldg(rot + lane) * acc0));
+      a.out[(nv * 3 + lane) * hw + pix] = v;
+    }
+  } else if (lane == 0) {
+    a.out[ray] = fmaf(carry, cost.esc, acc0);
+  }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(RC_THREADS) render_normal_backward_kernel(const NormArgs a) {
+  __shared__ float s_T[RC_WARPS][RC_MAX_CHUNKS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long ray = (long long)blockIdx.x * RC_WARPS + warp;
+  if (ray >= a.c.n_rays) return;
+  const RayIndex ri = ray_index<true>(a.c, ray);
+  const long long hw = (long long)a.c.H * a.c.W, nv = ray / hw, pix = ray - nv * hw;
+  const float *rot = a.c.rot + ri.n * a.c.rN + ri.v * a.c.rV;
+  NormalCost cost{0.0f, 0.0f, 0.0f, a.c.miss, 0.0f, false};
+  float scale;
+  if (MODE == RC_RENDER) {
+    const float G0 = a.c.g0[nv * 3 * hw + pix], G1 = a.c.g0[(nv * 3 + 1) * hw + pix], G2 = a.c.g0[(nv * 3 + 2) * hw + pix];
+    if (G0 == 0.0f && G1 == 0.0f && G2 == 0.0f) return;  // warp-uniform
+    rot_apply64(rot, -G0, -G1, -G2, false, cost.ax, cost.ay, cost.az);
+    cost.c0 = 0.0f;
+    cost.fg = true;
+    scale = 1.0f;
+  } else {
+    scale = a.c.g0[ray];
+    if (scale == 0.0f) return;  // warp-uniform
+    const float *o = a.obsn + ri.n * a.oN + ri.v * a.oV + ri.h * a.oH + ri.w * a.oW;
+    const float o0 = o[0], o1 = o[a.oC], o2 = o[2 * a.oC];
+    if (o0 != 0.0f || o1 != 0.0f || o2 != 0.0f) {
+      rot_apply64(rot, o0, o1, o2, true, cost.ax, cost.ay, cost.az);
+      cost.c0 = 1.0f;
+      cost.esc = a.c.miss;
+      cost.fg = true;
+    }
+  }
+  const size_t vol_off = (size_t)ri.n * a.c.R * a.c.R * a.c.R;  // every view of grid n scatters into grad_vox[n]
+  const float *vol = a.c.vox + vol_off;
+  float *gvol = a.c.grad_vox + vol_off;
+  const int R = a.c.R, Z = a.c.Z;
+  const CamRay r = ray_of<true>(a.c, ri);
+  // first walk: the chunk carries and T_Z (p depends on raw alone, so the plain walk's T_k are the forward's)
+  float unused, T_Z;
+  int last = 0;
+  cam_walk<true>(vol, R, r, Z, LinearCost{0.0f, 0.0f, 0.0f}, unused, T_Z, s_T[warp], &last);
+  __syncwarp();
+  const float hR = scale * (float)R;
+  float suffix = T_Z * cost.esc;
+  for (int c = last; c >= 0; --c) {
+    const int k = c * 32 + lane;
+    const bool live = k < Z;
+    NormSample s;
+    Taps t;
+    s.p = 0.0f;
+    float ck = 0.0f;
+    if (live) {
+      normal_sample(vol, R, r, k, a.eps, t, s);
+      ck = cost.at(s.nx, s.ny, s.nz);
+    }
+    float total;
+    const float Tk = s_T[warp][c] * warp_excl_prod32(1.0f - s.p, total);  // the forward's T_k, bit for bit
+    const float sk = s.p * Tk;
+    float chunk_sum;
+    const float Ak = suffix + warp_excl_suffix_sum32(live ? sk * ck : 0.0f, chunk_sum);
+    suffix += chunk_sum;
+    if (!live || s.raw != s.raw) continue;  // NaN samples pass nothing
+    const float dp = (s.raw >= RS_PMIN && s.raw <= RS_PMAX) ? scale * (Tk * ck - Ak / (1.0f - s.p)) : 0.0f;
+    float hx = 0.0f, hy = 0.0f, hz = 0.0f;
+    if (cost.fg && sk != 0.0f) {
+      const float inv = 1.0f / s.rho;
+      const float ga = fmaf(s.gz, cost.az, fmaf(s.gy, cost.ay, s.gx * cost.ax));
+      const float coef = ga * inv * inv;
+      const float w = hR * sk * inv;
+      hx = w * fmaf(-s.gx, coef, cost.ax);
+      hy = w * fmaf(-s.gy, coef, cost.ay);
+      hz = w * fmaf(-s.gz, coef, cost.az);
+    }
+    if (dp == 0.0f && hx == 0.0f && hy == 0.0f && hz == 0.0f) continue;
+    const float x0f = floorf(s.f[0]), y0f = floorf(s.f[1]), z0f = floorf(s.f[2]);
+    const float wx[2] = {(x0f + 1.0f) - s.f[0], s.f[0] - x0f};
+    const float wy[2] = {(y0f + 1.0f) - s.f[1], s.f[1] - y0f};
+    const float wz[2] = {(z0f + 1.0f) - s.f[2], s.f[2] - z0f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (!(t.valid & (1u << i))) continue;
+      const int bx = (i >> 2) & 1, by = (i >> 1) & 1, bz = i & 1;
+      const float dwx = (bx ? 1.0f : -1.0f) * (wy[by] * wz[bz]);
+      const float dwy = (by ? 1.0f : -1.0f) * (wx[bx] * wz[bz]);
+      const float dwz = (bz ? 1.0f : -1.0f) * (wx[bx] * wy[by]);
+      const float v = fmaf(hz, dwz, fmaf(hy, dwy, fmaf(hx, dwx, dp * t.w[i])));
+      if (v != 0.0f) atomicAdd(gvol + t.base + tap_offset(i, R), v);
+    }
+  }
+}
+
 static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 constexpr long long RC_MAX_RAYS = 1ll << 34;
@@ -769,4 +991,99 @@ extern "C" int genre_b200_ray_consistency_views_backward_pose(
   a.g0 = grad_loss;
   a.grad_vox = grad_vox;
   return rp_launch<RC_CONSISTENCY>("ray_consistency_views backward_pose kernels", a, po, stream);
+}
+
+// ---- surface normals of the posed views ----------------------------------------------------------------------------
+static int rn_check(const char *what, float eps, NormArgs &n) {
+  GB_REQUIRE(eps > 0.0f && eps <= 3.4e38f, GENRE_B200_EINVAL, "%s: eps %g must be positive and finite", what, (double)eps);
+  n.eps = eps;
+  return 0;
+}
+
+template <int MODE, bool FORWARD>
+static int rn_launch(const char *what, const NormArgs &n, void *stream) {
+  const unsigned grid = rc_grid(n.c);
+  if (FORWARD)
+    render_normal_forward_kernel<MODE><<<grid, RC_THREADS, 0, as_stream(stream)>>>(n);
+  else
+    render_normal_backward_kernel<MODE><<<grid, RC_THREADS, 0, as_stream(stream)>>>(n);
+  return check_launch(what);
+}
+
+extern "C" int genre_b200_render_normal_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                      int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                      const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                      int64_t eN, int64_t eV, float eps, float *normal, void *stream) {
+  NormArgs n{};
+  const char *what = "render_normal_views";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, n.c)) return rc;
+  if (int rc = rn_check(what, eps, n)) return rc;
+  GB_REQUIRE(normal, GENRE_B200_EINVAL, "%s: null output", what);
+  GB_REQUIRE(aligned4(normal), GENRE_B200_EALIGN, "%s: normal must be 4-byte aligned", what);
+  n.out = normal;
+  return rn_launch<RC_RENDER, true>("render_normal_views forward kernel", n, stream);
+}
+
+extern "C" int genre_b200_render_normal_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H,
+                                                       int64_t W, int z_res, const float *fl, int64_t fN, int64_t fV,
+                                                       const float *rot, int64_t rN, int64_t rV, const float *eye,
+                                                       int64_t eN, int64_t eV, float eps, const float *grad_normal,
+                                                       float *grad_vox, void *stream) {
+  NormArgs n{};
+  const char *what = "render_normal_views backward";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, n.c)) return rc;
+  if (int rc = rn_check(what, eps, n)) return rc;
+  GB_REQUIRE(grad_normal && grad_vox, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(aligned4(grad_normal) && aligned4(grad_vox), GENRE_B200_EALIGN, "%s: gradients must be 4-byte aligned",
+             what);
+  n.c.g0 = grad_normal;
+  n.c.grad_vox = grad_vox;
+  return rn_launch<RC_RENDER, false>("render_normal_views backward kernel", n, stream);
+}
+
+static int nc_obs(const char *what, const float *obs_normal, int64_t oN, int64_t oV, int64_t oC, int64_t oH, int64_t oW,
+                  float miss_cost, NormArgs &n) {
+  GB_REQUIRE(obs_normal, GENRE_B200_EINVAL, "%s: null obs_normal", what);
+  GB_REQUIRE(aligned4(obs_normal), GENRE_B200_EALIGN, "%s: obs_normal must be 4-byte aligned", what);
+  n.obsn = obs_normal;
+  n.oN = oN;
+  n.oV = oV;
+  n.oC = oC;
+  n.oH = oH;
+  n.oW = oW;
+  n.c.miss = miss_cost;
+  return 0;
+}
+
+extern "C" int genre_b200_normal_consistency_views_forward(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_normal, int64_t oN, int64_t oV, int64_t oC, int64_t oH, int64_t oW, float miss_cost, float eps,
+    float *loss, void *stream) {
+  NormArgs n{};
+  const char *what = "normal_consistency_views";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, n.c)) return rc;
+  if (int rc = rn_check(what, eps, n)) return rc;
+  if (int rc = nc_obs(what, obs_normal, oN, oV, oC, oH, oW, miss_cost, n)) return rc;
+  GB_REQUIRE(loss, GENRE_B200_EINVAL, "%s: null output", what);
+  GB_REQUIRE(aligned4(loss), GENRE_B200_EALIGN, "%s: loss must be 4-byte aligned", what);
+  n.out = loss;
+  return rn_launch<RC_CONSISTENCY, true>("normal_consistency_views forward kernel", n, stream);
+}
+
+extern "C" int genre_b200_normal_consistency_views_backward(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_normal, int64_t oN, int64_t oV, int64_t oC, int64_t oH, int64_t oW, float miss_cost, float eps,
+    const float *grad_loss, float *grad_vox, void *stream) {
+  NormArgs n{};
+  const char *what = "normal_consistency_views backward";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, n.c)) return rc;
+  if (int rc = rn_check(what, eps, n)) return rc;
+  if (int rc = nc_obs(what, obs_normal, oN, oV, oC, oH, oW, miss_cost, n)) return rc;
+  GB_REQUIRE(grad_loss && grad_vox, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(aligned4(grad_loss) && aligned4(grad_vox), GENRE_B200_EALIGN, "%s: gradients must be 4-byte aligned", what);
+  n.c.g0 = grad_loss;
+  n.c.grad_vox = grad_vox;
+  return rn_launch<RC_CONSISTENCY, false>("normal_consistency_views backward kernel", n, stream);
 }

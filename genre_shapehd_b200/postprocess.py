@@ -1246,6 +1246,94 @@ def ray_consistency_loss_views(vox, obs_depth, rot, eye, fl=CAM_FL, z_res=None, 
     return loss.mean((1, 2, 3)) if reduction == "mean" else loss
 
 
+# ---- surface normals of the posed views: rendered normal maps and multi-view normal consistency --------------------------
+class _NormalViews(torch.autograd.Function):
+    """``genre_b200_render_normal_views_*`` or ``genre_b200_normal_consistency_views_*``: ``args`` are every argument
+    before the output (the forward) or the upstream gradient (the backward), ``shape`` the dense output shape"""
+    @staticmethod
+    def forward(ctx, vox, v, keep, args, shape, entry):
+        out = torch.empty(shape, dtype=torch.float32, device=v.device)
+        _lib.call(entry + "_forward", *args, out.data_ptr(), _lib.stream_ptr(v))
+        ctx.save_for_backward(v, *keep)
+        ctx.args, ctx.shape, ctx.entry, ctx.vox_shape = args, shape, entry, vox.shape
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        v = ctx.saved_tensors[0]
+        g = grad_out.reshape(ctx.shape).contiguous()
+        grad = torch.zeros_like(v)
+        _lib.call(ctx.entry + "_backward", *ctx.args, g.data_ptr(), grad.data_ptr(), _lib.stream_ptr(v))
+        return grad.view(ctx.vox_shape), None, None, None, None, None
+
+
+def _normal_poses(vox, rot, eye, fl, eps, name):
+    """_poses for the normal ops, which differentiate no camera argument, after checking eps"""
+    for x, what in ((rot, "rot"), (eye, "eye"), (fl, "fl")):
+        if isinstance(x, torch.Tensor) and x.requires_grad:
+            raise ValueError("%s: %s requires grad, but the normal ops do not differentiate the camera (pass %s.detach())"
+                             % (name, what, what))
+    if not (isinstance(eps, (int, float)) and math.isfinite(eps) and eps > 0):
+        raise ValueError("%s: eps must be a positive finite float, got %r" % (name, eps))
+    return _poses(vox.shape[0], rot, eye, fl, name)
+
+
+def render_normal_views(vox, rot, eye, fl=CAM_FL, size=(256, 256), z_res=None, eps=1.0):
+    """Render each grid's surface normals from V cameras of any pose, differentiably in ``vox``.
+
+    vox, rot, eye, fl, size, z_res as ``render_depth_views`` (the same rays, samples and stop probabilities).  At each
+    sample the normal is n = -g / sqrt(|g|^2 + eps^2), g the gradient of the trilinear occupancy per unit length: it
+    points out of the occupied region, and ``eps`` (occupancy per unit length, > 0) keeps it and its gradient bounded
+    in empty space, where g is near 0.  A surface at R = 128 has |g| of about 16 to 128, which eps = 1 barely touches.
+    Returns normal [N,V,3,H,W]: the expected normal sum_k s_k n_k of each ray in its camera's frame (x forward, +y towards
+    image -w, +z towards image -h; a surface facing the camera has normal_x < 0), not renormalised, so it shrinks with
+    coverage like the expected depth; an escaping ray contributes 0.  Divide by its norm for unit normals.
+
+    Differentiable in ``vox`` only: ``rot``, ``eye`` and ``fl`` are not differentiated (ValueError if one requires
+    grad), nor ``eps``."""
+    name = "render_normal_views"
+    poses = _normal_poses(vox, rot, eye, fl, eps, name)
+    v, keep, args = _view_args(vox, poses, z_res, size, name)
+    N, V, H, W = args[1], args[3], args[4], args[5]
+    return _NormalViews.apply(vox, v, keep, args + (float(eps),), (N, V, 3, H, W), "genre_b200_render_normal_views")
+
+
+def normal_consistency_loss_views(vox, obs_normal, rot, eye, fl=CAM_FL, z_res=None, miss_cost=1.0, eps=1.0,
+                                  reduction="mean"):
+    """Multi-view normal consistency: the ray-consistency loss of ``ray_consistency_loss_views`` with surface normals in
+    place of depth, the normal term of MarrNet's reprojection consistency for perspective cameras of any pose.
+
+    obs_normal [N,V,3,H,W] fp32 on CUDA (any strides): observed normals in each view's camera frame, as
+    ``render_normal_views`` returns them; a pixel whose three components are all exactly 0 is background (MarrNet
+    zeroes the normal maps there).  Each foreground observation is normalised (predicted normal maps are not unit
+    length after resizing).  Per ray, the expected cost of where it stops: on a foreground ray a stop costs 1 - n . m
+    (n the sample's normal as ``render_normal_views``, m the unit observed normal, both in the grid frame) and escaping
+    costs ``miss_cost``; on a background ray every stop costs ``miss_cost`` and escaping is free.  Returns the per-grid
+    mean over all V*H*W rays [N] (``reduction='mean'``) or the per-ray loss [N,V,H,W] (``'none'``).
+
+    Differentiable in ``vox`` only (through the stop probabilities and the normals); ``rot``, ``eye``, ``fl`` (ValueError
+    if one requires grad), ``obs_normal`` and ``eps`` are not differentiated."""
+    name = "normal_consistency_loss_views"
+    if reduction not in ("mean", "none"):
+        raise ValueError("%s: reduction 'mean' or 'none', got %r" % (name, reduction))
+    n = vox.shape[0]
+    if not isinstance(obs_normal, torch.Tensor) or obs_normal.dim() != 5 or obs_normal.shape[0] != n \
+            or obs_normal.shape[2] != 3:
+        raise ValueError("%s: obs_normal [%d,V,3,H,W] expected, got %s"
+                         % (name, n, tuple(obs_normal.shape) if isinstance(obs_normal, torch.Tensor) else type(obs_normal)))
+    _lib.require_f32(obs_normal)
+    poses = _normal_poses(vox, rot, eye, fl, eps, name)
+    if obs_normal.shape[1] != poses[3]:
+        raise ValueError("%s: obs_normal has %d views but rot %d" % (name, obs_normal.shape[1], poses[3]))
+    v, keep, args = _view_args(vox, poses, z_res, obs_normal.shape[3:], name)
+    _lib.require_cuda(obs_normal)
+    args = args + (obs_normal.data_ptr(),) + tuple(obs_normal.stride()) + (float(miss_cost), float(eps))
+    N, V, H, W = args[1], args[3], args[4], args[5]
+    loss = _NormalViews.apply(vox, v, keep + (obs_normal,), args, (N, V, H, W), "genre_b200_normal_consistency_views")
+    return loss.mean((1, 2, 3)) if reduction == "mean" else loss
+
+
 # ---- any camera's depth map into a grid: posed multi-view back-projection -------------------------------------------------
 class _BackProjectViews(torch.autograd.Function):
     """``genre_b200_cam_bp_views_*``: ``args`` are the entry points' leading arguments (depth to eye strides), ``keep``

@@ -284,6 +284,40 @@ int genre_b200_ray_consistency_views_backward_pose(const float *vox, int64_t N, 
                                                    int64_t oH, int64_t oW, float miss_cost, const float *grad_loss,
                                                    float *grad_vox, float *grad_rot, float *grad_eye, void *workspace,
                                                    size_t workspace_bytes, void *stream);
+/* Surface normals of the posed views: the cameras, rays, samples, p_k, T_k and s_k above, arguments laid out as the
+ * views entries, plus eps > 0 (finite; else GENRE_B200_EINVAL), in occupancy per unit length.  At sample k,
+ *   g_k = R d raw / d f (the interpolant's gradient per unit length in the grid frame, in the cell the taps come from,
+ *         zero padding),  rho_k = sqrt(|g_k|^2 + eps^2),  n_k = -g_k / rho_k  (outward);  a NaN raw gives n_k = 0.
+ * render_normal:       normal [N, V, 3, H, W] dense = rot^T sum_k s_k n_k (summed in the grid frame, rotated once per
+ *                      ray): the expected normal in the camera frame (x forward, +y towards image -w, +z towards
+ *                      image -h), not renormalised; an escaping ray contributes 0.  grad_normal [N, V, 3, H, W] dense.
+ * normal_consistency:  obs_normal [N, V, 3, H, W] in that camera frame, any strides (oN, oV, oC, oH, oW); a pixel
+ *                      whose 3 components are all exactly 0 is background.  Elsewhere m = rot obs / |obs| (fp64,
+ *                      rounded once to fp32), and stops cost c_k = 1 - n_k . m, escape miss_cost; on background every
+ *                      stop costs miss_cost and escape is free.  loss and grad_loss [N, V, H, W] dense.
+ * The backwards accumulate into grad_vox (as above) both the path through p_k (zero where the clamp is active) and the
+ * path through n_k (at every sample with s_k != 0), one atomic per valid tap; rot, eye, fl, obs_normal and eps are not
+ * differentiated.  Limits as the views entries: 2 <= R <= 1024, 1 <= z_res <= 4096, N V H W <= 2^34.  One kernel
+ * launch each; the forwards are bitwise repeatable and each ray's value does not depend on the batch. */
+int genre_b200_render_normal_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                           int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                           int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, float eps,
+                                           float *normal, void *stream);
+int genre_b200_render_normal_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                            int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                            int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV, float eps,
+                                            const float *grad_normal, float *grad_vox, void *stream);
+int genre_b200_normal_consistency_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                                int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                                int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                                const float *obs_normal, int64_t oN, int64_t oV, int64_t oC, int64_t oH,
+                                                int64_t oW, float miss_cost, float eps, float *loss, void *stream);
+int genre_b200_normal_consistency_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                                 int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                                 int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                                 const float *obs_normal, int64_t oN, int64_t oV, int64_t oC,
+                                                 int64_t oH, int64_t oW, float miss_cost, float eps,
+                                                 const float *grad_loss, float *grad_vox, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Chamfer nearest-neighbour distance.  Replaces nnd_forward_cuda / nnd_backward_cuda

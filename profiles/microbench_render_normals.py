@@ -1,0 +1,96 @@
+#!/usr/bin/env python
+"""Surface normals of the posed views (csrc/render_cam.cu's render_normal_views and normal_consistency_views) at GenRe's
+training shape: 256^2 maps, R = 128, default Z (445), on clamp(cam_bp(depth) * 50, 1e-5, 1 - 1e-5) volumes of
+synth.bench_depth_batch, N = 4 grids x V = 8 orbit views (microbench_render_views.py's cameras).  Times
+render_normal_views forward, normal_consistency_loss_views forward, and its forward + backward, with
+render_depth_views / ray_consistency_loss_views timed in the same run as the yardstick.  CUDA events over repeated
+calls after warm-up; then, in a separate pass, each kernel's time from torch.profiler.  Prints one JSON line (and
+writes it to $OUT if set) with the card's name and power limit."""
+import json, math, os, subprocess, sys
+import torch
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+import genre_shapehd_b200
+genre_shapehd_b200.install()
+from genre_shapehd_b200 import postprocess
+from genre_shapehd_b200.synth import bench_depth_batch
+from toolbox.cam_bp.cam_bp.modules.camera_backprojection_module import Camera_back_projection_layer
+dev = torch.device("cuda:0"); torch.cuda.set_device(dev)
+H = W = 256
+R = 128
+N, V = 4, 8
+Z = postprocess.default_z_res(R)
+
+
+def timeit(fn, reps=20):
+    for _ in range(3): fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps): fn()
+    e1.record(); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:                                           # the measurement stands without the label
+        q = "unknown (%s)" % e
+    return q
+
+
+d = torch.from_numpy(bench_depth_batch(N)).to(dev)
+with torch.no_grad():
+    vox = torch.clamp(Camera_back_projection_layer()(d) * 50, 1e-5, 1 - 1e-5)
+az = torch.arange(V, dtype=torch.float64) * (2 * math.pi / V) + math.pi
+el = torch.tensor([math.radians(20) * (-1) ** v for v in range(V)], dtype=torch.float64)
+eyes = postprocess.CAM_DIST * torch.stack([torch.cos(el) * torch.cos(az), torch.cos(el) * torch.sin(az), torch.sin(el)], -1)
+rot, eye = postprocess.look_at(eyes)
+rot, eye = rot[None].to(dev), eye[None].to(dev)                    # one camera set shared by the batch
+with torch.no_grad():
+    obs_d = postprocess.render_depth_views(vox, rot, eye)[0]         # the grids' own depth and normal maps
+    obs_n = postprocess.render_normal_views(vox, rot, eye)
+
+res = {"card": card(), "H": H, "W": W, "R": R, "Z": Z, "N": N, "V": V, "rays": N * V * H * W}
+g = vox.clone().requires_grad_(True)
+for name, render, loss in (
+        ("normals", lambda x: postprocess.render_normal_views(x, rot, eye),
+         lambda x: postprocess.normal_consistency_loss_views(x, obs_n, rot, eye)),
+        ("depth", lambda x: postprocess.render_depth_views(x, rot, eye),
+         lambda x: postprocess.ray_consistency_loss_views(x, obs_d, rot, eye))):
+    def loss_fb():
+        g.grad = None
+        loss(g).sum().backward()
+    with torch.no_grad():
+        r = {"render_fwd_ms": timeit(lambda: render(vox)), "loss_fwd_ms": timeit(lambda: loss(vox))}
+    r["loss_fwd_bwd_ms"] = timeit(loss_fb, reps=10)
+    res[name] = r
+
+# kernel times, in a pass of their own
+from torch.profiler import ProfilerActivity, profile
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(5):
+        with torch.no_grad():
+            postprocess.render_normal_views(vox, rot, eye)
+            postprocess.render_depth_views(vox, rot, eye)
+        for fn in (lambda x: postprocess.normal_consistency_loss_views(x, obs_n, rot, eye),
+                   lambda x: postprocess.ray_consistency_loss_views(x, obs_d, rot, eye)):
+            g.grad = None
+            fn(g).sum().backward()
+    torch.cuda.synchronize()
+kern = {}
+for e in prof.key_averages():
+    if "render_normal" in e.key or "render_camera" in e.key:
+        t = getattr(e, "device_time_total", None)
+        if t is None:
+            t = e.cuda_time_total
+        kern[e.key] = round(t / max(e.count, 1) / 1000.0, 4)
+res["kernel_ms"] = kern
+line = json.dumps(res)
+print(line)
+if os.environ.get("OUT"):
+    os.makedirs(os.path.dirname(os.path.abspath(os.environ["OUT"])), exist_ok=True)
+    with open(os.environ["OUT"], "w") as f:
+        f.write(line + "\n")

@@ -69,6 +69,17 @@ _SIGNATURES = {
     "genre_b200_normal_consistency_views_backward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr,
                                                      _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _i64,
                                                      _f32, _f32, _ptr, _ptr, _ptr],
+    "genre_b200_sketch_consistency_views_forward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr,
+                                                    _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _ptr,
+                                                    _i64, _i64, _i64, _i64, _i64, _f32, _f32, _f32, _f32, _ptr, _ptr],
+    "genre_b200_sketch_consistency_views_backward": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64, _ptr,
+                                                     _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i64, _ptr,
+                                                     _i64, _i64, _i64, _i64, _i64, _f32, _f32, _f32, _f32, _ptr, _ptr,
+                                                     _ptr],
+    "genre_b200_sketch_consistency_views_backward_pose": [_ptr, _i64, _int, _i64, _i64, _i64, _int, _ptr, _i64, _i64,
+                                                          _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64,
+                                                          _i64, _ptr, _i64, _i64, _i64, _i64, _i64, _f32, _f32, _f32,
+                                                          _f32, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_nnd_forward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_nnd_backward": [_ptr, _ptr, _i64, _i64, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_convt3d_s2_forward": [_ptr, _int, _ptr, _int, _i64, _i64, _i64, _i64, _ptr, _int, _int, _int, _ptr, _ptr,
@@ -158,6 +169,8 @@ _LAUNCHES = {
     "genre_b200_render_views_backward_pose": 2, "genre_b200_ray_consistency_views_backward_pose": 2,
     "genre_b200_render_normal_views_forward": 1, "genre_b200_render_normal_views_backward": 1,
     "genre_b200_normal_consistency_views_forward": 1, "genre_b200_normal_consistency_views_backward": 1,
+    "genre_b200_sketch_consistency_views_forward": 1, "genre_b200_sketch_consistency_views_backward": 1,
+    "genre_b200_sketch_consistency_views_backward_pose": 2,
     "genre_b200_cam_bp_stage_project": 1, "genre_b200_voxelize_stage_splat": 1,
     "genre_b200_convt3d_s2_forward": 1, "genre_b200_conv3d_taps_forward": 1,
     "genre_b200_convt_c1_forward": 1, "genre_b200_conv3d_k4s2_forward": 1,

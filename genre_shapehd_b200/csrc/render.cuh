@@ -100,6 +100,43 @@ __device__ __forceinline__ float sample_trilinear_grad(const float *__restrict__
   return acc;
 }
 
+// sample_trilinear_grad's raw and d raw / d f (the same operations in the same order, bit for bit), and the three mixed
+// second partials hxy = d2 raw / df_x df_y, hxz, hyz of the same cell (the interpolant's Hessian in f; its diagonal is
+// 0).  Each mixed partial is the cell's second difference across its two axes, weighted along the third.
+__device__ __forceinline__ float sample_trilinear_hess(const float *__restrict__ vol, const Taps &t, int R, float fx,
+                                                       float fy, float fz, float &dx, float &dy, float &dz, float &hxy,
+                                                       float &hxz, float &hyz) {
+  float v[8], acc = 0.0f;
+  if (t.valid == 0xFFu) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      v[i] = __ldg(vol + t.base + tap_offset(i, R));
+      acc = fmaf(v[i], t.w[i], acc);
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      v[i] = 0.0f;
+      if (t.valid & (1u << i)) {
+        v[i] = __ldg(vol + t.base + tap_offset(i, R));
+        acc = fmaf(v[i], t.w[i], acc);
+      }
+    }
+  }
+  const float x0f = floorf(fx), y0f = floorf(fy), z0f = floorf(fz);
+  const float wx1 = fx - x0f, wx0 = (x0f + 1.0f) - fx;
+  const float wy1 = fy - y0f, wy0 = (y0f + 1.0f) - fy;
+  const float wz1 = fz - z0f, wz0 = (z0f + 1.0f) - fz;
+  // tap i: bit 2 = x, bit 1 = y, bit 0 = z
+  dx = fmaf(v[7] - v[3], wy1 * wz1, fmaf(v[6] - v[2], wy1 * wz0, fmaf(v[5] - v[1], wy0 * wz1, (v[4] - v[0]) * (wy0 * wz0))));
+  dy = fmaf(v[7] - v[5], wx1 * wz1, fmaf(v[6] - v[4], wx1 * wz0, fmaf(v[3] - v[1], wx0 * wz1, (v[2] - v[0]) * (wx0 * wz0))));
+  dz = fmaf(v[7] - v[6], wx1 * wy1, fmaf(v[5] - v[4], wx1 * wy0, fmaf(v[3] - v[2], wx0 * wy1, (v[1] - v[0]) * (wx0 * wy0))));
+  hxy = fmaf((v[7] - v[3]) - (v[5] - v[1]), wz1, ((v[6] - v[2]) - (v[4] - v[0])) * wz0);
+  hxz = fmaf((v[7] - v[3]) - (v[6] - v[2]), wy1, ((v[5] - v[1]) - (v[4] - v[0])) * wy0);
+  hyz = fmaf((v[7] - v[5]) - (v[6] - v[4]), wx1, ((v[3] - v[1]) - (v[2] - v[0])) * wx0);
+  return acc;
+}
+
 // exclusive product over the warp's lanes; total = the product of all 32
 __device__ __forceinline__ float warp_excl_prod32(float v, float &total) {
   float incl = v;

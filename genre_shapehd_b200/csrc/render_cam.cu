@@ -686,6 +686,272 @@ __global__ void __launch_bounds__(RC_THREADS) render_normal_backward_kernel(cons
   }
 }
 
+// ---- depth and normal sketches together (the sketch_consistency_views entry points; tests/sketch_pose_ref.py restates
+// them) --------------------------------------------------------------------------------------------------------------
+// The cameras, rays, samples t_k, f_k, p_k, T_k, s_k are ray_consistency_views', bit for bit, and the sample normal
+// n_k = -g_k / rho_k is render_normal_views'.  Each ray's cost is a weighted sum of the two consistency costs, each term
+// with its own background rule:
+//   depth   obs_d > 0: c^d_k = |t_k - obs_d|, c^d_esc = miss;   obs_d <= 0: c^d_k = miss, c^d_esc = 0
+//   normal  obs_n != 0: c^n_k = 1 - n_k . m, c^n_esc = miss (m as normal_consistency_views');  obs_n = 0: miss, 0
+//   c_k = fma(wn, c^n_k, wd c^d_k),   c_esc = fma(wn, c^n_esc, wd c^d_esc)
+// so in exact arithmetic a ray's loss is wd L_depth + wn L_normal.  The grid gradient is the normal backward's two
+// paths with this cost: the p path dp_k (clamp and NaN rules as there) and the n path h_k = scale wn s_k Res dc^n/dg_k.
+// Pose gradients (the _backward_pose entry point) keep the definition of the file header; per sample, the position
+// gradient is
+//   q_k = w_k g_k + Res Hf_k h_k     (w_k = dp_k; g_k = Res d raw / d f; Hf_k = d2 raw / df2 in the cell make_taps_at
+//                                     selects, zero diagonal; the n path at every non-NaN sample with s_k != 0)
+// i.e. w_k grad_k + Res^2 Hf_k b_k with b_k = scale wn s_k (m - g (g . m) / rho^2) / rho.  From q_k the per-ray terms
+//   dV/du' = sum_k t_k q_k,   dV/dt(shift) = sum_k (q_k . u' + s_k c'_k)  (c'_k = scale wd sign(t_k - obs_d): the normal
+//   cost does not depend on t),   dV/de = sum_k q_k + (e / |e|) dV/dt(shift)
+// and the frame term of m = rot o / |o|: a foreground-normal ray adds -scale wn S_i o_j / |o| to grad_rot[i][j], with
+// S = sum_k s_k n_k (the ray's grid-frame sum, as render_normal_views').  The terms go to the pose backward's RP_TERMS
+// per-CTA partials and render_views_pose_reduce_kernel sums them, so they are bitwise repeatable.
+struct SketchArgs {
+  NormArgs n;      // n.c: posed cameras, Z, miss, obs_d (c.obs, strides c.oN, c.oV, c.oH, c.oW), c.g0 = grad_loss,
+                   // c.grad_vox; n.obsn: obs_n; n.eps; n.out = loss
+  float wd, wn;
+};
+
+struct SketchCost {
+  RayCost d;
+  NormalCost n;
+  float wd, wn;
+  __device__ __forceinline__ float at(float t, float nx, float ny, float nz) const {
+    return fmaf(wn, n.at(nx, ny, nz), wd * d.at(t));
+  }
+  __device__ __forceinline__ float esc() const { return fmaf(wn, n.esc, wd * d.esc()); }
+  __device__ __forceinline__ float slope(float t) const { return wd * d.slope(t); }  // d c_k / d t_k
+};
+
+// the ray's costs; o = its observed normal (camera frame)
+__device__ __forceinline__ SketchCost sketch_cost(const SketchArgs &a, const RayIndex &ri, const float *rot, float (&o)[3]) {
+  SketchCost c;
+  c.d = RayCost{obs_of<true>(a.n.c, ri), a.n.c.miss};
+  c.n = NormalCost{0.0f, 0.0f, 0.0f, a.n.c.miss, 0.0f, false};
+  c.wd = a.wd;
+  c.wn = a.wn;
+  const float *op = a.n.obsn + ri.n * a.n.oN + ri.v * a.n.oV + ri.h * a.n.oH + ri.w * a.n.oW;
+  o[0] = op[0];
+  o[1] = op[a.n.oC];
+  o[2] = op[2 * a.n.oC];
+  if (o[0] != 0.0f || o[1] != 0.0f || o[2] != 0.0f) {
+    rot_apply64(rot, o[0], o[1], o[2], true, c.n.ax, c.n.ay, c.n.az);
+    c.n.c0 = 1.0f;
+    c.n.esc = a.n.c.miss;
+    c.n.fg = true;
+  }
+  return c;
+}
+
+// normal_sample, and with HESS the interpolant's mixed second partials in f (0 otherwise)
+template <bool HESS>
+__device__ __forceinline__ void sketch_sample(const float *__restrict__ vol, int R, const CamRay &ray, int k, float eps,
+                                              Taps &taps, NormSample &s, float &hxy, float &hxz, float &hyz) {
+  if (!HESS) {
+    normal_sample(vol, R, ray, k, eps, taps, s);
+    hxy = hxz = hyz = 0.0f;
+    return;
+  }
+  s.t = cam_sample<true>(ray, k, R, taps, s.f);
+  float dx, dy, dz;
+  s.raw = sample_trilinear_hess(vol, taps, R, s.f[0], s.f[1], s.f[2], dx, dy, dz, hxy, hxz, hyz);
+  s.p = fminf(fmaxf(s.raw, RS_PMIN), RS_PMAX);
+  const float Rf = (float)R;
+  const bool nan = s.raw != s.raw;
+  s.gx = nan ? 0.0f : dx * Rf;
+  s.gy = nan ? 0.0f : dy * Rf;
+  s.gz = nan ? 0.0f : dz * Rf;
+  s.rho = sqrtf(fmaf(s.gz, s.gz, fmaf(s.gy, s.gy, fmaf(s.gx, s.gx, eps * eps))));
+  s.nx = -s.gx / s.rho;
+  s.ny = -s.gy / s.rho;
+  s.nz = -s.gz / s.rho;
+}
+
+__global__ void __launch_bounds__(RC_THREADS) sketch_consistency_forward_kernel(const SketchArgs a) {
+  const CamArgs &c = a.n.c;
+  const long long ray = (long long)blockIdx.x * RC_WARPS + (threadIdx.x >> 5);
+  if (ray >= c.n_rays) return;
+  const int lane = threadIdx.x & 31;
+  const RayIndex ri = ray_index<true>(c, ray);
+  const float *vol = c.vox + (size_t)ri.n * c.R * c.R * c.R;
+  const CamRay r = ray_of<true>(c, ri);
+  float o[3];
+  const SketchCost cost = sketch_cost(a, ri, c.rot + ri.n * c.rN + ri.v * c.rV, o);
+  float carry = 1.0f, acc = 0.0f;
+  for (int ch = 0; ch * 32 < c.Z; ++ch) {
+    const int k = ch * 32 + lane;
+    NormSample s;
+    s.p = 0.0f;  // lanes past the end behave like p = 0 (factor 1, no contribution)
+    if (k < c.Z) {
+      Taps t;
+      normal_sample(vol, c.R, r, k, a.n.eps, t, s);
+    }
+    float total;
+    const float before = carry * warp_excl_prod32(1.0f - s.p, total);
+    if (k < c.Z) acc = fmaf(s.p * before, cost.at(s.t, s.nx, s.ny, s.nz), acc);
+    carry *= total;
+    if (carry == 0.0f) break;  // warp-uniform
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) a.n.out[ray] = fmaf(carry, cost.esc(), acc);
+}
+
+// One ray's two walks: the grid gradient into gvol (skipped when null) and, with POSE, the ray's pose partials
+// (RP_TERMS, the layout of render_views_pose_backward_kernel) in part, identical in every lane.
+template <bool POSE>
+__device__ __forceinline__ void sketch_backward_ray(const SketchArgs &a, long long ray, float scale, float *chunk_T,
+                                                    double (&part)[RP_TERMS]) {
+  const CamArgs &c = a.n.c;
+  const int lane = threadIdx.x & 31;
+  const RayIndex ri = ray_index<true>(c, ray);
+  const float *rot = c.rot + ri.n * c.rN + ri.v * c.rV;
+  float o[3];
+  const SketchCost cost = sketch_cost(a, ri, rot, o);
+  const size_t vol_off = (size_t)ri.n * c.R * c.R * c.R;  // every view of grid n scatters into grad_vox[n]
+  const float *vol = c.vox + vol_off;
+  float *gvol = POSE && !c.grad_vox ? nullptr : c.grad_vox + vol_off;  // null: pose only
+  const int R = c.R, Z = c.Z;
+  const float Rf = (float)R;
+  const CamRay r = ray_of<true>(c, ri);
+  // first walk: the chunk carries and T_Z (p depends on raw alone, so the plain walk's T_k are the forward's)
+  float unused, T_Z;
+  int last = 0;
+  cam_walk<true>(vol, R, r, Z, LinearCost{0.0f, 0.0f, 0.0f}, unused, T_Z, chunk_T, &last);
+  __syncwarp();
+  const float hR = scale * a.wn * Rf;
+  const float ux = (float)r.ux, uy = (float)r.uy, uz = (float)r.uz;
+  // acc[0..2] = sum_k t_k q_k, acc[3..5] = sum_k q_k, acc[6] = sum_k q_k . u', acc[7] = sum_k s_k c'_k, acc[8..10] = S
+  float acc[11];
+#pragma unroll
+  for (int i = 0; i < 11; ++i) acc[i] = 0.0f;
+  float suffix = T_Z * cost.esc();
+  for (int ch = last; ch >= 0; --ch) {
+    const int k = ch * 32 + lane;
+    const bool live = k < Z;
+    NormSample s;
+    Taps t;
+    s.p = 0.0f;
+    float ck = 0.0f, hxy = 0.0f, hxz = 0.0f, hyz = 0.0f;
+    if (live) {
+      sketch_sample<POSE>(vol, R, r, k, a.n.eps, t, s, hxy, hxz, hyz);
+      ck = cost.at(s.t, s.nx, s.ny, s.nz);
+    }
+    float total;
+    const float Tk = chunk_T[ch] * warp_excl_prod32(1.0f - s.p, total);  // the forward's T_k, bit for bit
+    const float sk = s.p * Tk;
+    float chunk_sum;
+    const float Ak = suffix + warp_excl_suffix_sum32(live ? sk * ck : 0.0f, chunk_sum);
+    suffix += chunk_sum;
+    if (POSE && live) {
+      acc[7] = fmaf(sk, scale * cost.slope(s.t), acc[7]);
+      acc[8] = fmaf(sk, s.nx, acc[8]);
+      acc[9] = fmaf(sk, s.ny, acc[9]);
+      acc[10] = fmaf(sk, s.nz, acc[10]);
+    }
+    if (!live || s.raw != s.raw) continue;  // NaN samples pass nothing
+    const float dp = (s.raw >= RS_PMIN && s.raw <= RS_PMAX) ? scale * (Tk * ck - Ak / (1.0f - s.p)) : 0.0f;
+    float hx = 0.0f, hy = 0.0f, hz = 0.0f;
+    if (cost.n.fg && sk != 0.0f) {
+      const float inv = 1.0f / s.rho;
+      const float ga = fmaf(s.gz, cost.n.az, fmaf(s.gy, cost.n.ay, s.gx * cost.n.ax));
+      const float coef = ga * inv * inv;
+      const float w = hR * sk * inv;
+      hx = w * fmaf(-s.gx, coef, cost.n.ax);
+      hy = w * fmaf(-s.gy, coef, cost.n.ay);
+      hz = w * fmaf(-s.gz, coef, cost.n.az);
+    }
+    if (dp == 0.0f && hx == 0.0f && hy == 0.0f && hz == 0.0f) continue;
+    if (POSE) {
+      const float qx = fmaf(dp, s.gx, Rf * fmaf(hxz, hz, hxy * hy));
+      const float qy = fmaf(dp, s.gy, Rf * fmaf(hyz, hz, hxy * hx));
+      const float qz = fmaf(dp, s.gz, Rf * fmaf(hyz, hy, hxz * hx));
+      acc[0] = fmaf(qx, s.t, acc[0]);
+      acc[1] = fmaf(qy, s.t, acc[1]);
+      acc[2] = fmaf(qz, s.t, acc[2]);
+      acc[3] += qx;
+      acc[4] += qy;
+      acc[5] += qz;
+      acc[6] = fmaf(qz, uz, fmaf(qy, uy, fmaf(qx, ux, acc[6])));
+      if (!gvol) continue;
+    }
+    const float x0f = floorf(s.f[0]), y0f = floorf(s.f[1]), z0f = floorf(s.f[2]);
+    const float wx[2] = {(x0f + 1.0f) - s.f[0], s.f[0] - x0f};
+    const float wy[2] = {(y0f + 1.0f) - s.f[1], s.f[1] - y0f};
+    const float wz[2] = {(z0f + 1.0f) - s.f[2], s.f[2] - z0f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (!(t.valid & (1u << i))) continue;
+      const int bx = (i >> 2) & 1, by = (i >> 1) & 1, bz = i & 1;
+      const float dwx = (bx ? 1.0f : -1.0f) * (wy[by] * wz[bz]);
+      const float dwy = (by ? 1.0f : -1.0f) * (wx[bx] * wz[bz]);
+      const float dwz = (bz ? 1.0f : -1.0f) * (wx[bx] * wy[by]);
+      const float v = fmaf(hz, dwz, fmaf(hy, dwy, fmaf(hx, dwx, dp * t.w[i])));
+      if (v != 0.0f) atomicAdd(gvol + t.base + tap_offset(i, R), v);
+    }
+  }
+  if constexpr (POSE) {
+#pragma unroll
+    for (int i = 0; i < 11; ++i) acc[i] = warp_sum(acc[i]);
+    const CamRay u = cam_dir(c.fl[ri.n * c.fN + ri.v * c.fV], ri.h, ri.w, c.H, c.W, c.Z);  // camera-frame u
+    const double uc[3] = {u.ux, u.uy, u.uz};
+    double oh[3] = {0.0, 0.0, 0.0}, fs = 0.0;  // the frame term's o / |o| (fp64) and -scale wn
+    if (cost.n.fg) {
+      const double x = o[0], y = o[1], z = o[2];
+      const double nrm = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
+      oh[0] = x / nrm;
+      oh[1] = y / nrm;
+      oh[2] = z / nrm;
+      fs = -(double)scale * (double)a.wn;
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+#pragma unroll
+      for (int j = 0; j < 3; ++j) part[3 * i + j] = (double)acc[i] * uc[j] + fs * (double)acc[8 + i] * oh[j];
+      part[9 + i] = (double)acc[3 + i];
+    }
+    part[12] = (double)acc[6] + (double)acc[7];
+  }
+}
+
+// POSE = false: one warp per ray over [N, V, H, W], the grid gradient only.  POSE = true: the layout of
+// render_views_pose_backward_kernel (CTAs never straddle views; each writes its 8 rays' RP_TERMS fp64 sums, in warp
+// order, to the workspace; grad_vox optional).
+template <bool POSE>
+__global__ void __launch_bounds__(RC_THREADS) sketch_consistency_backward_kernel(const SketchArgs a, const PoseOut po) {
+  __shared__ float s_T[RC_WARPS][RC_MAX_CHUNKS];
+  const int warp = threadIdx.x >> 5;
+  double part[RP_TERMS];
+  if constexpr (!POSE) {
+    const long long ray = (long long)blockIdx.x * RC_WARPS + warp;
+    if (ray >= a.n.c.n_rays) return;
+    const float scale = a.n.c.g0[ray];
+    if (scale != 0.0f) sketch_backward_ray<false>(a, ray, scale, s_T[warp], part);  // warp-uniform
+    return;
+  }
+  __shared__ double s_part[RC_WARPS][RP_TERMS];
+  const long long hw = (long long)a.n.c.H * a.n.c.W;
+  const long long view = blockIdx.x / po.bpv, blk = blockIdx.x - view * po.bpv;
+  const long long pix = blk * RC_WARPS + warp;
+#pragma unroll
+  for (int i = 0; i < RP_TERMS; ++i) part[i] = 0.0;
+  if (pix < hw) {
+    const long long ray = view * hw + pix;
+    const float scale = a.n.c.g0[ray];
+    if (scale != 0.0f) sketch_backward_ray<true>(a, ray, scale, s_T[warp], part);  // warp-uniform
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int i = 0; i < RP_TERMS; ++i) s_part[warp][i] = part[i];
+  }
+  __syncthreads();
+  if (threadIdx.x < RP_TERMS) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < RC_WARPS; ++w) s += s_part[w][threadIdx.x];
+    po.part[(view * RP_TERMS + threadIdx.x) * po.bpv + blk] = s;
+  }
+}
+
 static bool aligned4(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 constexpr long long RC_MAX_RAYS = 1ll << 34;
@@ -1086,4 +1352,90 @@ extern "C" int genre_b200_normal_consistency_views_backward(
   n.c.g0 = grad_loss;
   n.c.grad_vox = grad_vox;
   return rn_launch<RC_CONSISTENCY, false>("normal_consistency_views backward kernel", n, stream);
+}
+
+// ---- depth and normal sketches together -----------------------------------------------------------------------------
+static int sk_check(const char *what, const float *obs_depth, int64_t odN, int64_t odV, int64_t odH, int64_t odW,
+                    const float *obs_normal, int64_t onN, int64_t onV, int64_t onC, int64_t onH, int64_t onW, float wd,
+                    float wn, float miss_cost, float eps, SketchArgs &s) {
+  if (int rc = rn_check(what, eps, s.n)) return rc;
+  if (int rc = nc_obs(what, obs_normal, onN, onV, onC, onH, onW, miss_cost, s.n)) return rc;
+  GB_REQUIRE(obs_depth, GENRE_B200_EINVAL, "%s: null obs_depth", what);
+  GB_REQUIRE(aligned4(obs_depth), GENRE_B200_EALIGN, "%s: obs_depth must be 4-byte aligned", what);
+  const float fmax = 3.402823466e38f;
+  GB_REQUIRE(wd >= 0.0f && wd <= fmax && wn >= 0.0f && wn <= fmax && (wd > 0.0f || wn > 0.0f), GENRE_B200_EINVAL,
+             "%s: weights %g, %g must be finite and >= 0, one of them > 0", what, (double)wd, (double)wn);
+  s.n.c.obs = obs_depth;
+  s.n.c.oN = odN;
+  s.n.c.oV = odV;
+  s.n.c.oH = odH;
+  s.n.c.oW = odW;
+  s.wd = wd;
+  s.wn = wn;
+  return 0;
+}
+
+extern "C" int genre_b200_sketch_consistency_views_forward(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_depth, int64_t odN, int64_t odV, int64_t odH, int64_t odW, const float *obs_normal, int64_t onN,
+    int64_t onV, int64_t onC, int64_t onH, int64_t onW, float depth_weight, float normal_weight, float miss_cost,
+    float eps, float *loss, void *stream) {
+  SketchArgs s{};
+  const char *what = "sketch_consistency_views";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, s.n.c)) return rc;
+  if (int rc = sk_check(what, obs_depth, odN, odV, odH, odW, obs_normal, onN, onV, onC, onH, onW, depth_weight,
+                        normal_weight, miss_cost, eps, s))
+    return rc;
+  GB_REQUIRE(loss, GENRE_B200_EINVAL, "%s: null output", what);
+  GB_REQUIRE(aligned4(loss), GENRE_B200_EALIGN, "%s: loss must be 4-byte aligned", what);
+  s.n.out = loss;
+  sketch_consistency_forward_kernel<<<rc_grid(s.n.c), RC_THREADS, 0, as_stream(stream)>>>(s);
+  return check_launch("sketch_consistency_views forward kernel");
+}
+
+extern "C" int genre_b200_sketch_consistency_views_backward(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_depth, int64_t odN, int64_t odV, int64_t odH, int64_t odW, const float *obs_normal, int64_t onN,
+    int64_t onV, int64_t onC, int64_t onH, int64_t onW, float depth_weight, float normal_weight, float miss_cost,
+    float eps, const float *grad_loss, float *grad_vox, void *stream) {
+  SketchArgs s{};
+  const char *what = "sketch_consistency_views backward";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, s.n.c)) return rc;
+  if (int rc = sk_check(what, obs_depth, odN, odV, odH, odW, obs_normal, onN, onV, onC, onH, onW, depth_weight,
+                        normal_weight, miss_cost, eps, s))
+    return rc;
+  GB_REQUIRE(grad_loss && grad_vox, GENRE_B200_EINVAL, "%s: null pointer", what);
+  GB_REQUIRE(aligned4(grad_loss) && aligned4(grad_vox), GENRE_B200_EALIGN, "%s: gradients must be 4-byte aligned", what);
+  s.n.c.g0 = grad_loss;
+  s.n.c.grad_vox = grad_vox;
+  sketch_consistency_backward_kernel<false><<<rc_grid(s.n.c), RC_THREADS, 0, as_stream(stream)>>>(s, PoseOut{});
+  return check_launch("sketch_consistency_views backward kernel");
+}
+
+extern "C" int genre_b200_sketch_consistency_views_backward_pose(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_depth, int64_t odN, int64_t odV, int64_t odH, int64_t odW, const float *obs_normal, int64_t onN,
+    int64_t onV, int64_t onC, int64_t onH, int64_t onW, float depth_weight, float normal_weight, float miss_cost,
+    float eps, const float *grad_loss, float *grad_vox, float *grad_rot, float *grad_eye, void *workspace,
+    size_t workspace_bytes, void *stream) {
+  SketchArgs s{};
+  PoseOut po;
+  const char *what = "sketch_consistency_views backward_pose";
+  if (int rc = rv_check(what, vox, N, res, V, H, W, z_res, fl, fN, fV, rot, rN, rV, eye, eN, eV, s.n.c)) return rc;
+  if (int rc = sk_check(what, obs_depth, odN, odV, odH, odW, obs_normal, onN, onV, onC, onH, onW, depth_weight,
+                        normal_weight, miss_cost, eps, s))
+    return rc;
+  GB_REQUIRE(grad_loss, GENRE_B200_EINVAL, "%s: null grad_loss", what);
+  GB_REQUIRE(aligned4(grad_loss), GENRE_B200_EALIGN, "%s: grad_loss must be 4-byte aligned", what);
+  if (int rc = rp_check(what, s.n.c, N, V, grad_vox, grad_rot, grad_eye, workspace, workspace_bytes, po)) return rc;
+  s.n.c.g0 = grad_loss;
+  s.n.c.grad_vox = grad_vox;
+  const long long views = (long long)N * V;
+  sketch_consistency_backward_kernel<true><<<(unsigned)(views * po.bpv), RC_THREADS, 0, as_stream(stream)>>>(s, po);
+  if (int rc = check_launch("sketch_consistency_views backward_pose kernel")) return rc;
+  render_views_pose_reduce_kernel<<<(unsigned)views, RC_THREADS, 0, as_stream(stream)>>>(s.n.c, po);
+  return check_launch("sketch_consistency_views pose reduce kernel");
 }

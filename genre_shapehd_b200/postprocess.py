@@ -1334,6 +1334,70 @@ def normal_consistency_loss_views(vox, obs_normal, rot, eye, fl=CAM_FL, z_res=No
     return loss.mean((1, 2, 3)) if reduction == "mean" else loss
 
 
+def _nonneg_weight(x, what, name):
+    if not (isinstance(x, (int, float)) and math.isfinite(x) and x >= 0):
+        raise ValueError("%s: %s must be a finite float >= 0, got %r" % (name, what, x))
+    return float(x)
+
+
+def sketch_consistency_loss_views(vox, obs_depth, obs_normal, rot, eye, fl=CAM_FL, z_res=None, depth_weight=1.0,
+                                  normal_weight=1.0, miss_cost=1.0, eps=1.0, reduction="mean"):
+    """Depth and normal consistency in one pass: MarrNet's reprojection consistency (the depth term plus the normal
+    term) for perspective cameras of any pose, differentiable in the grid and in the poses.
+
+    vox, rot, eye, fl, z_res as ``ray_consistency_loss_views``; obs_depth [N,V,H,W] as there (<= 0 marks background)
+    and obs_normal [N,V,3,H,W] as ``normal_consistency_loss_views`` (all three components 0 marks background), both
+    fp32 on CUDA with any strides and the same H, W.  Each ray is walked once: a stop costs
+    ``depth_weight * c_depth + normal_weight * c_normal`` and escaping the same weighted sum, each term with its own
+    background rule, so the result equals ``depth_weight * ray_consistency_loss_views(...) + normal_weight *
+    normal_consistency_loss_views(...)`` up to rounding, at the cost of about one walk instead of two.  The weights are
+    finite floats >= 0, one of them > 0.  Returns the per-grid mean over all V*H*W rays [N] (``reduction='mean'``) or
+    the per-ray loss [N,V,H,W] (``'none'``).
+
+    Differentiable in ``vox`` (through the stop probabilities and the normals) and, when ``rot`` or ``eye`` is a tensor
+    that requires grad, in it, as ``ray_consistency_loss_views`` (bitwise repeatable; with ``vox`` frozen the grid's
+    gradient is skipped).  The normal term's pose gradient moves each sample's normal with the sample (the trilinear
+    interpolant's second derivatives) and turns the observed normal with the camera, so the normal map's orientation
+    informs the fit; ``normal_weight`` alone with ``depth_weight=0`` fits a pose to a normal map.  Not differentiated:
+    ``fl`` (ValueError if it requires grad), the observations, ``eps`` and the weights."""
+    name = "sketch_consistency_loss_views"
+    if reduction not in ("mean", "none"):
+        raise ValueError("%s: reduction 'mean' or 'none', got %r" % (name, reduction))
+    wd = _nonneg_weight(depth_weight, "depth_weight", name)
+    wn = _nonneg_weight(normal_weight, "normal_weight", name)
+    if wd == 0 and wn == 0:
+        raise ValueError("%s: depth_weight and normal_weight are both 0" % name)
+    if not (isinstance(eps, (int, float)) and math.isfinite(eps) and eps > 0):
+        raise ValueError("%s: eps must be a positive finite float, got %r" % (name, eps))
+    n = vox.shape[0]
+    if not isinstance(obs_depth, torch.Tensor) or obs_depth.dim() != 4 or obs_depth.shape[0] != n:
+        raise ValueError("%s: obs_depth [%d,V,H,W] expected, got %s"
+                         % (name, n, tuple(obs_depth.shape) if isinstance(obs_depth, torch.Tensor) else type(obs_depth)))
+    if not isinstance(obs_normal, torch.Tensor) or obs_normal.dim() != 5 or obs_normal.shape[0] != n \
+            or obs_normal.shape[2] != 3:
+        raise ValueError("%s: obs_normal [%d,V,3,H,W] expected, got %s"
+                         % (name, n, tuple(obs_normal.shape) if isinstance(obs_normal, torch.Tensor) else type(obs_normal)))
+    if obs_normal.shape[1] != obs_depth.shape[1] or obs_normal.shape[3:] != obs_depth.shape[2:]:
+        raise ValueError("%s: obs_depth %s and obs_normal %s disagree in V, H or W"
+                         % (name, tuple(obs_depth.shape), tuple(obs_normal.shape)))
+    pose_in = _pose_inputs(rot, eye, fl, vox.device, name)
+    _lib.require_f32(obs_depth, obs_normal)
+    _lib.require_cuda(obs_depth, obs_normal)
+    poses = _poses(n, rot, eye, fl, name)
+    if obs_depth.shape[1] != poses[3]:
+        raise ValueError("%s: the observations have %d views but rot %d" % (name, obs_depth.shape[1], poses[3]))
+    v, keep, args = _view_args(vox, poses, z_res, obs_depth.shape[2:], name)
+    args = args + (obs_depth.data_ptr(),) + tuple(obs_depth.stride()) + (obs_normal.data_ptr(),) + \
+        tuple(obs_normal.stride()) + (wd, wn, float(miss_cost), float(eps))
+    keep = keep + (obs_depth, obs_normal)
+    entry = "genre_b200_sketch_consistency_views"
+    if pose_in is not None:
+        loss = _ViewsPose.apply(vox, *pose_in, v, keep, args, tuple(obs_depth.shape), (), entry)
+    else:
+        loss = _RayConsistency.apply(vox, v, keep, args, tuple(obs_depth.shape), entry)
+    return loss.mean((1, 2, 3)) if reduction == "mean" else loss
+
+
 # ---- any camera's depth map into a grid: posed multi-view back-projection -------------------------------------------------
 class _BackProjectViews(torch.autograd.Function):
     """``genre_b200_cam_bp_views_*``: ``args`` are the entry points' leading arguments (depth to eye strides), ``keep``

@@ -318,6 +318,42 @@ int genre_b200_normal_consistency_views_backward(const float *vox, int64_t N, in
                                                  const float *obs_normal, int64_t oN, int64_t oV, int64_t oC,
                                                  int64_t oH, int64_t oW, float miss_cost, float eps,
                                                  const float *grad_loss, float *grad_vox, void *stream);
+/* Depth and normal sketches together: ray_consistency_views and normal_consistency_views fused into one walk per ray,
+ * differentiable in the grid and the poses.  The leading arguments are the views entries'; then obs_depth
+ * [N, V, H, W] (any strides (odN, odV, odH, odW); <= 0 is background), obs_normal [N, V, 3, H, W] (any strides; all
+ * three exactly 0 is background), the weights wd = depth_weight and wn = normal_weight (finite, >= 0, one of them > 0;
+ * else GENRE_B200_EINVAL), miss_cost and eps (as normal_consistency_views).  The samples t_k, p_k, T_k, s_k are
+ * ray_consistency_views' and n_k is render_normal_views', bit for bit; each stop costs
+ *   c_k = fma(wn, c^n_k, wd c^d_k)   and escaping   c_esc = fma(wn, c^n_esc, wd c^d_esc),
+ * c^d and c^n the two entries' costs, each with its own background rule, so a ray's loss is wd L_depth + wn L_normal.
+ * loss and grad_loss [N, V, H, W] dense.  The backward accumulates into grad_vox the path through p_k and the path
+ * through n_k (weighted by wn), one atomic per valid tap.  _backward_pose also writes grad_rot and grad_eye as the
+ * *_views_backward_pose entries (same workspace, grad_vox nullable, two kernel launches, bitwise repeatable), with the
+ * normal term's position gradient through the interpolant's in-cell second derivatives and the frame term of
+ * m = rot obs / |obs|.  Not differentiated: fl, obs_depth, obs_normal, eps, the weights.  Limits as the views entries. */
+int genre_b200_sketch_consistency_views_forward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                                int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                                int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                                const float *obs_depth, int64_t odN, int64_t odV, int64_t odH,
+                                                int64_t odW, const float *obs_normal, int64_t onN, int64_t onV,
+                                                int64_t onC, int64_t onH, int64_t onW, float depth_weight,
+                                                float normal_weight, float miss_cost, float eps, float *loss,
+                                                void *stream);
+int genre_b200_sketch_consistency_views_backward(const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W,
+                                                 int z_res, const float *fl, int64_t fN, int64_t fV, const float *rot,
+                                                 int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+                                                 const float *obs_depth, int64_t odN, int64_t odV, int64_t odH,
+                                                 int64_t odW, const float *obs_normal, int64_t onN, int64_t onV,
+                                                 int64_t onC, int64_t onH, int64_t onW, float depth_weight,
+                                                 float normal_weight, float miss_cost, float eps,
+                                                 const float *grad_loss, float *grad_vox, void *stream);
+int genre_b200_sketch_consistency_views_backward_pose(
+    const float *vox, int64_t N, int res, int64_t V, int64_t H, int64_t W, int z_res, const float *fl, int64_t fN,
+    int64_t fV, const float *rot, int64_t rN, int64_t rV, const float *eye, int64_t eN, int64_t eV,
+    const float *obs_depth, int64_t odN, int64_t odV, int64_t odH, int64_t odW, const float *obs_normal, int64_t onN,
+    int64_t onV, int64_t onC, int64_t onH, int64_t onW, float depth_weight, float normal_weight, float miss_cost,
+    float eps, const float *grad_loss, float *grad_vox, float *grad_rot, float *grad_eye, void *workspace,
+    size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Chamfer nearest-neighbour distance.  Replaces nnd_forward_cuda / nnd_backward_cuda

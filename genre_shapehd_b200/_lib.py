@@ -134,6 +134,7 @@ _SIGNATURES = {
     "genre_b200_voxel_translate": [_ptr, _i64, _int, _int, _int, _ptr, _ptr, _ptr, _ptr],
     "genre_b200_surface_sample": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_surface_sample_backward": [_ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _ptr],
+    "genre_b200_emd_forward": [_ptr, _ptr, _i64, _i64, _f64, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_crop_to_render": [_ptr, _ptr, _int, _ptr, _ptr, _int, _i64, _int, _f64, _f64, _ptr, _ptr, _ptr, _ptr, _size,
                                   _ptr],
     "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
@@ -150,7 +151,7 @@ EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + [
     "genre_b200_isosurface_workspace_bytes", "genre_b200_raycast_workspace_bytes", "genre_b200_voxel_fill_workspace_bytes",
     "genre_b200_surface_sample_workspace_bytes", "genre_b200_crop_to_render_workspace_bytes",
     "genre_b200_preprocess_workspace_bytes", "genre_b200_mesh_voxelize_workspace_bytes",
-    "genre_b200_render_views_pose_workspace_bytes"])
+    "genre_b200_render_views_pose_workspace_bytes", "genre_b200_emd_workspace_bytes"])
 
 _lib = None
 launch_count = 0  # kernels of this library enqueued through the binding (bench.py reports it as gpu_launches)
@@ -184,7 +185,7 @@ _LAUNCHES = {
     "genre_b200_raycast_count": 3, "genre_b200_raycast_build": 2, "genre_b200_raycast_first_hit": 1,
     "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
     "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,
-    "genre_b200_surface_sample": 3, "genre_b200_crop_to_render": 2,
+    "genre_b200_surface_sample": 3, "genre_b200_crop_to_render": 2, "genre_b200_emd_forward": 1,
     # min/max (not rgb) + cubic, + gray, mean and jitter for train-mode rgb
     "genre_b200_preprocess": lambda kind, train, *_: 1 + (kind != 0) + (3 if kind == 0 and train else 0),
     # count, scan and columns only when there are faces, then the expand kernel
@@ -241,6 +242,8 @@ def load():
     lib.genre_b200_mesh_voxelize_workspace_bytes.argtypes = [_i64, _i64, _int, _int, _int]
     lib.genre_b200_render_views_pose_workspace_bytes.restype = _size
     lib.genre_b200_render_views_pose_workspace_bytes.argtypes = [_i64, _i64, _i64, _i64]
+    lib.genre_b200_emd_workspace_bytes.restype = _size
+    lib.genre_b200_emd_workspace_bytes.argtypes = [_i64, _i64]
     _lib = lib
     return lib
 

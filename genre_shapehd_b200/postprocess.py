@@ -677,7 +677,82 @@ def chamfer_fscore(p, q, tau=0.01):
     return {"acc": acc, "comp": comp, "chamfer": (acc + comp) / 2, "precision": prec, "recall": rec, "fscore": fscore}
 
 
-def voxel_metrics(pred, gt, level=0.5, gt_level=0.5, n_points=1024, tau=0.01, seed=0):
+def _emd_forward(p, q, eps):
+    """the auction kernel -> (emd [B] fp64, match [B,n] int32, counters [B,2] int32: rounds and phases per pair)"""
+    b, n = p.shape[0], p.shape[1]
+    nbytes = _lib.load().genre_b200_emd_workspace_bytes(b, n)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=p.device)
+    out = torch.empty((b,), dtype=torch.float64, device=p.device)
+    match = torch.empty((b, n), dtype=torch.int32, device=p.device)
+    _lib.call("genre_b200_emd_forward", p.data_ptr(), q.data_ptr(), b, n, float(eps), match.data_ptr(), out.data_ptr(),
+              ws.data_ptr(), nbytes, _lib.stream_ptr(p))
+    return out, match, ws[:8 * b].view(torch.int32).view(b, 2)
+
+
+def _emd_grad(p, q, match, grad_emd):
+    """dEMD/dp_i = (p_i - q_s(i)) / (n c_i) with c_i the matched distance (0 where c_i = 0), and the negative of it for
+    q_s(i), times grad_emd, in fp64 by a gather and a scatter through the bijection (deterministic).  Pairs with match -1
+    get no gradient."""
+    n = p.shape[1]
+    ok = (match[:, :1] >= 0)
+    idx = torch.where(ok, match, torch.zeros_like(match)).long()[..., None].expand(-1, -1, 3)
+    d = p.double() - torch.gather(q.double(), 1, idx)
+    c = torch.sqrt((d * d).sum(2, keepdim=True))
+    g = torch.where((c > 0) & ok[..., None], d / (n * torch.where(c > 0, c, torch.ones_like(c))), torch.zeros_like(d))
+    g = g * grad_emd.double()[:, None, None]
+    gq = torch.zeros_like(g).scatter_(1, idx, -g)
+    return g.to(p.dtype), torch.where(ok[..., None], gq, torch.zeros_like(gq)).to(q.dtype)
+
+
+class _EMD(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, p, q, eps):
+        out, match, _ = _emd_forward(p, q, eps)
+        ctx.save_for_backward(p, q, match)
+        ctx.mark_non_differentiable(match)
+        return out, match
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_emd, _):
+        p, q, match = ctx.saved_tensors
+        gp, gq = _emd_grad(p, q, match, grad_emd)
+        return (gp if ctx.needs_input_grad[0] else None), (gq if ctx.needs_input_grad[1] else None), None
+
+
+def emd(p, q, eps=1e-5):
+    """Earth mover's distance between B pairs of equal-size point sets, by an auction on the device (one CTA per pair).
+
+    p, q [B,n,3] fp32 on CUDA, 1 <= n <= 4096.  Returns (emd [B] fp64, match [B,n] int32): match[b] is a bijection, point
+    p_i paired with q_match[i], and emd the mean of the matched fp32 Euclidean distances, summed in fp64.
+
+    ``eps`` is in the points' units.  The auction runs eps-scaling phases down to the effective
+    eps_eff = max(eps, 2^-32 D), with D the diagonal of the pair's bounding box: below that floor an fp64 price could stop
+    rising and the auction would not end.  The matching is eps-optimal, not necessarily optimal:
+    opt <= emd <= opt + eps_eff, up to the fp64 rounding of the sum.  Every step is stated in include/genre_b200.h and
+    restated bit for bit in tests/emd_ref.py; the result is deterministic and does not depend on the rest of the batch.
+    A pair with a NaN or infinite coordinate (or one above 2^62 in magnitude) gets emd NaN and match -1, as does a pair
+    that reaches the auction's round cap (a safety net far beyond what any pair of <= 4096 points needs).
+
+    Differentiable in p and q with the matching held fixed: dEMD/dp_i = (p_i - q_match[i]) / (n c_i), the negative for
+    q_match[i], 0 where the matched distance c_i is 0.  A gather and a scatter through the bijection, so the gradient is
+    deterministic.  Pairs with match -1 get no gradient."""
+    _lib.require_cuda(p, q)
+    _lib.require_f32(p, q)
+    if p.dim() != 3 or p.shape[2] != 3 or p.shape != q.shape:
+        raise ValueError("emd: p and q [B,n,3] of the same shape expected, got %s and %s" % (tuple(p.shape), tuple(q.shape)))
+    eps = float(eps)
+    if not (np.isfinite(eps) and eps > 0):
+        raise ValueError("emd: eps must be finite and > 0, got %r" % eps)
+    if _lib.load().genre_b200_emd_workspace_bytes(p.shape[0], p.shape[1]) == 0:
+        raise ValueError("emd: %d pairs of %d points unsupported (1 <= B <= 65535, 1 <= n <= 4096)" % tuple(p.shape[:2]))
+    p, q = p.contiguous(), q.contiguous()
+    if torch.is_grad_enabled() and (p.requires_grad or q.requires_grad):
+        return _EMD.apply(p, q, eps)
+    return _emd_forward(p, q, eps)[:2]
+
+
+def voxel_metrics(pred, gt, level=0.5, gt_level=0.5, n_points=1024, tau=0.01, seed=0, emd=False, emd_eps=1e-5):
     """Surface metrics of predicted voxel grids against ground-truth grids, batched on the device.
 
     pred, gt [B,1,D,H,W] or [B,D,H,W] fp32 values (not logits) of the same shape.  The protocol, stated because it is not
@@ -692,14 +767,18 @@ def voxel_metrics(pred, gt, level=0.5, gt_level=0.5, n_points=1024, tau=0.01, se
     Returns the dict of ``chamfer_fscore`` with ``iou`` added (all [B] fp64) and ``valid`` [B] bool, False where either surface
     is empty (no face of non-zero area); those samples get NaN surface metrics (their IoU is still defined) and their NaN
     points never reach the nearest-neighbour kernel.  The two marching-cubes calls synchronise once each, as documented
-    there; nothing else does."""
+    there; nothing else does.
+
+    ``emd=True`` adds ``emd`` [B] fp64: ``emd(points on pred, points on gt, emd_eps)`` on the same points as the Chamfer keys
+    (the mean matched distance of an eps-optimal bijection, within emd_eps of the optimum), NaN where ``valid`` is False.
+    The default leaves the call, its result and its cost unchanged."""
     a, g = _volumes(pred, "voxel_metrics"), _volumes(gt, "voxel_metrics")
     if a.shape != g.shape:
         raise ValueError("voxel_metrics: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(g.shape)))
     seeds = _seeds(seed, a.shape[0], a.device)
     pp, fp = _grid_surface_points(a, level, n_points, seeds)
     pg, fg = _grid_surface_points(g, gt_level, n_points, seeds)
-    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, g, level, gt_level)[0].double())
+    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, g, level, gt_level)[0].double(), emd_eps if emd else None)
 
 
 def _grid_surface_points(v, level, n_points, seeds):
@@ -710,16 +789,45 @@ def _grid_surface_points(v, level, n_points, seeds):
     return sample_surface(*marching_cubes(v, level, spacing, shift), n_points, seeds)
 
 
-def _point_metrics(pp, fp, pg, fg, tau, iou):
-    """chamfer_fscore of two point batches, NaN where either surface is empty (face -1), with ``iou`` and ``valid`` added"""
+def _point_metrics(pp, fp, pg, fg, tau, iou, emd_eps=None):
+    """chamfer_fscore of two point batches, NaN where either surface is empty (face -1), with ``iou`` and ``valid`` added,
+    and ``emd`` at emd_eps unless that is None"""
     valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
     keep = valid[:, None, None]
-    out = chamfer_fscore(torch.where(keep, pp, torch.zeros_like(pp)), torch.where(keep, pg, torch.zeros_like(pg)), tau)
+    p1, p2 = torch.where(keep, pp, torch.zeros_like(pp)), torch.where(keep, pg, torch.zeros_like(pg))
+    out = chamfer_fscore(p1, p2, tau)
+    if emd_eps is not None:
+        out["emd"] = emd(p1, p2, emd_eps)[0]
     nan = torch.full((pp.shape[0],), float("nan"), dtype=torch.float64, device=pp.device)
     out = {k: torch.where(valid, v, nan) for k, v in out.items()}
     out["iou"] = iou
     out["valid"] = valid
     return out
+
+
+def _loss_points(name, pred, gt, level, n_points, seed, same_count=False):
+    """the two point batches of chamfer_loss / emd_loss, with the samples where either side has no surface replaced by
+    zeros -> (p1 [B,n_points,3], p2 [B,M,3], valid [B] bool); same_count: gt points must have M = n_points"""
+    a = _volumes(pred, name)
+    b = a.shape[0]
+    seeds = _seeds(seed, b, a.device)
+    pp, fp = _grid_surface_points(a, level, n_points, seeds)
+    if gt.dim() == 3:
+        _lib.require_cuda(gt)
+        _lib.require_f32(gt)
+        if gt.shape[0] != b or gt.shape[2] != 3 or (same_count and gt.shape[1] != n_points):
+            raise ValueError("%s: gt points [%d,%s,3] expected, got %s" % (name, b, n_points if same_count else "M",
+                                                                          tuple(gt.shape)))
+        pg = gt
+        valid = (fp[:, 0] >= 0) & ~torch.isnan(gt).any(2).any(1)
+    else:
+        g = _volumes(gt, name)
+        if g.shape != a.shape:
+            raise ValueError("%s: pred %s and gt %s differ in shape" % (name, tuple(a.shape), tuple(g.shape)))
+        pg, fg = _grid_surface_points(g, 0.5, n_points, seeds)
+        valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
+    keep = valid[:, None, None]
+    return torch.where(keep, pp, torch.zeros_like(pp)), torch.where(keep, pg, torch.zeros_like(pg)), valid
 
 
 def chamfer_loss(pred, gt, level=0.5, n_points=1024, seed=0, eps=1e-10):
@@ -742,29 +850,27 @@ def chamfer_loss(pred, gt, level=0.5, n_points=1024, seed=0, eps=1e-10):
     edge whose two values both lie close to ``level`` the gradient grows like 1 / (v1 - v0)^2; no clipping is built in.
     Marching cubes on pred synchronises once; a grid gt adds its own."""
     from .toolbox.nndistance.functions.nnd import NNDFunction
-    a = _volumes(pred, "chamfer_loss")
-    b = a.shape[0]
-    seeds = _seeds(seed, b, a.device)
-    pp, fp = _grid_surface_points(a, level, n_points, seeds)
-    if gt.dim() == 3:
-        _lib.require_cuda(gt)
-        _lib.require_f32(gt)
-        if gt.shape[0] != b or gt.shape[2] != 3:
-            raise ValueError("chamfer_loss: gt points [%d,M,3] expected, got %s" % (b, tuple(gt.shape)))
-        pg = gt
-        valid = (fp[:, 0] >= 0) & ~torch.isnan(gt).any(2).any(1)
-    else:
-        g = _volumes(gt, "chamfer_loss")
-        if g.shape != a.shape:
-            raise ValueError("chamfer_loss: pred %s and gt %s differ in shape" % (tuple(a.shape), tuple(g.shape)))
-        pg, fg = _grid_surface_points(g, 0.5, n_points, seeds)
-        valid = (fp[:, 0] >= 0) & (fg[:, 0] >= 0)
-    keep = valid[:, None, None]
-    p1 = torch.where(keep, pp, torch.zeros_like(pp))
-    p2 = torch.where(keep, pg, torch.zeros_like(pg))
+    p1, p2, valid = _loss_points("chamfer_loss", pred, gt, level, n_points, seed)
     d1, d2, _, _ = NNDFunction.apply(p1, p2)
     loss = torch.sqrt(d1 + eps).mean(1) + torch.sqrt(d2 + eps).mean(1)
     return torch.where(valid, loss, torch.zeros_like(loss)), valid
+
+
+def emd_loss(pred, gt, level=0.5, n_points=1024, seed=0, eps=1e-5):
+    """Differentiable earth mover's distance of predicted grids against ground-truth grids or points, for training.
+
+    The points, ``gt``'s two forms and the validity rule are exactly ``chamfer_loss``'s, except that points [B,n_points,3]
+    are required of a points ``gt`` (the matching is a bijection).  loss_b = ``emd(points on pred, points on gt, eps)``, the
+    mean matched distance of an eps-optimal bijection (``eps`` in the unit cube's units), rounded to fp32.  Returns
+    (loss [B] fp32, valid [B] bool); where valid is False the loss is 0 and no gradient flows from that sample.
+
+    Its gradient pulls every predicted point towards its own matched target point, with the matching held fixed, and
+    reaches pred through ``sample_surface`` and ``marching_cubes`` as chamfer_loss's does (the same caveats: it moves
+    existing surface only, and grows on edges whose two values both lie close to ``level``).  Marching cubes on pred
+    synchronises once; a grid gt adds its own."""
+    p1, p2, valid = _loss_points("emd_loss", pred, gt, level, n_points, seed, same_count=True)
+    loss = emd(p1, p2, eps)[0]
+    return torch.where(valid, loss, torch.zeros_like(loss)).float(), valid
 
 
 # ---- meshes to grids: conservative voxelisation, scoring against ground-truth meshes, .obj input ---------------------------
@@ -812,14 +918,15 @@ def voxelize_mesh(verts, faces, vert_off, face_off, shape=128):
     return out
 
 
-def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=1024, tau=0.01, seed=0, six_way=True):
+def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=1024, tau=0.01, seed=0, six_way=True, emd=False,
+                 emd_eps=1e-5):
     """``voxel_metrics`` of predicted grids against ground-truth triangle meshes given in the same frame (the centred unit
     cube, ``voxelize_mesh``'s; aligning and normalising the meshes is the caller's).
 
     pred [B,1,D,H,W] or [B,D,H,W] fp32 values; the meshes packed as for ``voxelize_mesh``, one per sample.
       * points on the prediction: ``marching_cubes(pred, level)`` in voxel_metrics' frame, then ``sample_surface``;
       * points on the ground truth: ``sample_surface`` of the meshes, with the same seeds;
-      * chamfer / F-score, ``valid`` and the NaNs of invalid samples exactly as ``voxel_metrics``;
+      * chamfer / F-score, ``valid``, the NaNs of invalid samples and the opt-in ``emd`` exactly as ``voxel_metrics``;
       * iou = voxel_iou(pred, voxel_fill(voxelize_mesh(meshes, (D, H, W)), six_way), level, 0.5).
     Given the ground truth as ``marching_cubes(gt)`` in voxel_metrics' frame, every metric but ``iou`` equals voxel_metrics'
     bit for bit.  The marching-cubes call synchronises once; nothing else does."""
@@ -832,7 +939,8 @@ def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=102
     pp, fp = _grid_surface_points(a, level, n_points, seeds)
     pg, fg = sample_surface(verts, faces, vert_off, face_off, n_points, seeds)
     solid = voxel_fill(voxelize_mesh(verts, faces, vert_off, face_off, tuple(a.shape[1:])), six_way)
-    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, solid[:, 0].float(), level, 0.5)[0].double())
+    return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, solid[:, 0].float(), level, 0.5)[0].double(),
+                          emd_eps if emd else None)
 
 
 def read_obj(path):

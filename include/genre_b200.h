@@ -819,6 +819,40 @@ int genre_b200_surface_sample_backward(const int32_t *faces, int64_t F, const in
                                        const float *grad_points, int64_t V, float *grad_verts, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Earth mover's distance between B pairs of equal-size point sets: an auction (Bertsekas) with eps-scaling and Jacobi
+ * bidding, one CTA per pair, everything but p in shared memory.  The assignment is a bijection whose mean cost is within the
+ * final eps_eff of the optimum (eps-complementary slackness): opt <= emd <= opt + eps_eff, up to the fp64 rounding of the sum.
+ *   inputs  p, q [B, n, 3] fp32, dense; 1 <= n <= 4096, 1 <= B <= 65535, eps finite and > 0.  Persons are p's points,
+ *           objects q's.
+ *   cost    c_ij = sqrt((dx*dx + dy*dy) + dz*dz) in fp32, d = p_i - q_j, one rounding per operation, no FMA, sqrt correctly
+ *           rounded.  Everything after it is fp64, one rounding per operation, no FMA.
+ *   refusal a pair with a coordinate that is NaN or of magnitude above 2^62 (where an fp32 squared distance could overflow)
+ *           never enters the auction: match -1 for all its points, emd NaN, rounds = phases = 0.
+ *   eps     lo_a / hi_a = the smallest / largest fp32 coordinate a over both sets, e_a = (double)hi_a - (double)lo_a,
+ *           D = sqrt((e0*e0 + e1*e1) + e2*e2); eps_eff = max(eps, D * 2^-32) (below that a bid could fail to raise an
+ *           fp64 price, and the auction would never end).  Phase k = 0, 1, ... runs at eps_0 = max(D * 0.25, eps_eff),
+ *           eps_{k+1} = max(eps_k * 0.25, eps_eff); the phase run at eps_eff is the last.  Prices start at 0 and carry
+ *           over; every phase starts with no person assigned.
+ *   round   (Jacobi) every unassigned person i bids at once, against the prices at the round's start:
+ *             v_ij = (-(double)c_ij) - price_j;  v1 = max_j v_ij, j1 = the lowest j attaining it;  v2 = max over j != j1
+ *             (n = 1: v2 = v1);  bid_i = (price_j1 + (v1 - v2)) + eps_k.
+ *           Every object with bids goes to its highest bid, the lowest i among equal bids; its price becomes that bid and its
+ *           previous owner, if any, is unassigned.  The phase ends after the first round that leaves nobody unassigned.
+ *   cap     2^22 rounds per pair over all phases: a pair whose 2^22-th round still leaves a person unassigned gets the
+ *           refusal's output (with its counts).  Far above what point sets of <= 4096 points need; it is a safety net.
+ *   output  match [B, n] int32, match[b, i] = the object of person i: a permutation of 0..n-1.  emd [B] fp64 = S / n with
+ *           S the fp64 sum of the matched costs (double)c_{i, match[i]}, zero-padded to N2 = the smallest power of two
+ *           >= n and summed by halving: a_i += a_{i + h} for h = N2/2, N2/4, ..., 1 (S = c_0 when n = 1).
+ *           The result depends only on the pair: deterministic, independent of scheduling and of the rest of the batch.
+ *           tests/emd_ref.py restates the whole contract in numpy, bit for bit.
+ *   workspace: genre_b200_emd_workspace_bytes(B, n) bytes (0: unsupported), 16-byte aligned, caller-owned.  Its first 8 B bytes
+ *           receive int32 [B, 2]: the rounds and the phases each pair ran (a debug counter).
+ * ------------------------------------------------------------------------------------------- */
+size_t genre_b200_emd_workspace_bytes(int64_t B, int64_t n);
+int genre_b200_emd_forward(const float *p, const float *q, int64_t B, int64_t n, double eps, int32_t *match, double *emd,
+                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Conservative voxelisation of batched triangle meshes, the inverse of genre_b200_isosurface_*: ground-truth meshes become
  * grids for voxel_iou / voxel_fill and training targets without a CPU tool.
  *   meshes  the packed format of genre_b200_isosurface_*: verts [V, 3] fp32, faces [F, 3] int32 indexing the sample's own

@@ -135,6 +135,8 @@ _SIGNATURES = {
     "genre_b200_surface_sample": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _size, _ptr],
     "genre_b200_surface_sample_backward": [_ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _ptr],
     "genre_b200_emd_forward": [_ptr, _ptr, _i64, _i64, _f64, _ptr, _ptr, _ptr, _size, _ptr],
+    "genre_b200_distance_transform": [_ptr, _i64, _int, _f32, _ptr, _ptr],
+    "genre_b200_pose_score": [_ptr, _i64, _int, _ptr, _i64, _ptr, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _f32, _ptr, _ptr],
     "genre_b200_crop_to_render": [_ptr, _ptr, _int, _ptr, _ptr, _int, _i64, _int, _f64, _f64, _ptr, _ptr, _ptr, _ptr, _size,
                                   _ptr],
     "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
@@ -186,6 +188,7 @@ _LAUNCHES = {
     "genre_b200_voxel_fill": 3, "genre_b200_voxel_transform": 1, "genre_b200_voxel_stats": 3,
     "genre_b200_voxel_downsample": 1, "genre_b200_voxel_translate": 1,
     "genre_b200_surface_sample": 3, "genre_b200_crop_to_render": 2, "genre_b200_emd_forward": 1,
+    "genre_b200_distance_transform": 3, "genre_b200_pose_score": 1,
     # min/max (not rgb) + cubic, + gray, mean and jitter for train-mode rgb
     "genre_b200_preprocess": lambda kind, train, *_: 1 + (kind != 0) + (3 if kind == 0 and train else 0),
     # count, scan and columns only when there are faces, then the expand kernel

@@ -20,6 +20,10 @@ points drawn from their surfaces (the metric of the reference's nndistance op), 
 ``voxelize_mesh`` / ``mesh_metrics`` / ``read_obj`` / ``pack_meshes`` go the other way, from triangle meshes (ShapeNet and
 Pix3D ship their shapes as meshes) to grids: conservative voxelisation on the device, and the same metrics against
 ground-truth meshes.
+
+``distance_transform`` / ``depth_points`` / ``pose_candidates`` / ``score_poses`` / ``estimate_pose`` find the camera pose
+of a canonical-frame grid from an observed depth map: exact distance fields, a batched score of candidate cameras
+covering SO(3), and a refinement by ray consistency.
 """
 import math
 
@@ -1575,3 +1579,302 @@ def back_project_views(depth, rot, eye, fl=CAM_FL, res=128, shift=True):
     args = (depth.data_ptr(), N, V, H, W) + tuple(depth.stride()) + (f.data_ptr(),) + nv(f) + (r.data_ptr(),) + nv(r) + \
         (e.data_ptr(),) + nv(e)
     return _BackProjectViews.apply(depth, (r, e, f), args, int(res), bool(shift))
+
+
+# ---- the camera pose of a canonical-frame grid from a depth map: distance transforms, candidate scoring, refinement ------
+def distance_transform(vox, level=0.5):
+    """Exact Euclidean distance transform: vox [N,1,R,R,R] or [N,R,R,R] fp32 on CUDA, 1 <= R <= 256 -> the distance, in
+    voxel units, from every voxel to the nearest voxel of its grid with value >= ``level``, in vox's shape.  It equals
+    ``scipy.ndimage.distance_transform_edt(v < level)`` per sample: the kernel's squared distances are exact integers and
+    this is their fp32 square root.  A grid with no voxel >= level is +inf everywhere.  Divide by R for grid units, as a
+    truncated-distance target or to measure a shell's thickness."""
+    v = _volumes(vox, "distance_transform")
+    n, r = v.shape[0], v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]) or not 1 <= r <= 256:
+        raise ValueError("distance_transform expects cubic volumes of side 1 .. 256, got %s" % (tuple(vox.shape),))
+    if not (isinstance(level, (int, float)) and math.isfinite(level)):
+        raise ValueError("distance_transform: level must be a finite float, got %r" % (level,))
+    out = torch.empty_like(v)
+    _lib.call("genre_b200_distance_transform", v.data_ptr(), n, r, float(level), out.data_ptr(), _lib.stream_ptr(v))
+    return out.sqrt_().view(vox.shape)
+
+
+POSE_MAX_POINTS = 4096
+
+
+def depth_points(depth, fl=CAM_FL, n_points=2048, seed=0):
+    """Observed depth maps -> camera-frame surface points for ``score_poses``.
+
+    depth [N,1,H,W] or [N,H,W] fp32 on CUDA: ray depths from the eye, as ``back_project_views`` takes them; pixels with
+    depth > 0 are foreground.  Pixel (h, w) at depth d becomes the point ``back_project_views`` places for it with rot = I
+    and eye = 0: (d c, -d c (w - (W-1)/2) / fl, -d c (h - (H-1)/2) / fl), c = fl / sqrt(fl^2 + (w - (W-1)/2)^2 +
+    (h - (H-1)/2)^2), in the camera frame (x forward, +y towards image -w, +z towards image -h).  A sample with more
+    than ``n_points`` (1 .. 4096) foreground pixels keeps a seeded draw of ``n_points`` of them without replacement,
+    made on the device; the kept points are in pixel order.  Returns (points [N,P,3], counts [N] int32): rows
+    0 .. counts[n]-1 of sample n are its points, the rest 0; P = min(n_points, the largest foreground count).
+    ValueError for a sample with no foreground pixel."""
+    _lib.require_cuda(depth)
+    _lib.require_f32(depth)
+    d = depth[:, 0] if depth.dim() == 4 and depth.shape[1] == 1 else depth
+    if d.dim() != 3:
+        raise ValueError("depth_points: depth [N,1,H,W] or [N,H,W] expected, got %s" % (tuple(depth.shape),))
+    if not (isinstance(n_points, int) and 1 <= n_points <= POSE_MAX_POINTS):
+        raise ValueError("depth_points: n_points must be an int in [1, %d], got %r" % (POSE_MAX_POINTS, n_points))
+    N, H, W = d.shape
+    dev = d.device
+    d = d.reshape(N, H * W)
+    fg = d > 0
+    cnt = fg.sum(1)
+    if bool((cnt == 0).any()):
+        raise ValueError("depth_points: sample %d has no foreground pixel (depth > 0)" % int((cnt == 0).nonzero()[0]))
+    P = min(n_points, int(cnt.max()))
+    g = torch.Generator(device=dev).manual_seed(int(seed))
+    key = torch.rand(N, H * W, generator=g, device=dev)
+    key = torch.where(fg, key, torch.full_like(key, 2.0))           # background after every foreground pixel
+    pick = key.topk(P, dim=1, largest=False).indices
+    ok = fg.gather(1, pick)
+    pick = torch.where(ok, pick, torch.full_like(pick, H * W)).sort(1).values   # kept pixels first, in pixel order
+    ok = pick < H * W
+    pick = pick.clamp_max(H * W - 1)
+    h, w = (pick // W).float(), (pick % W).float()
+    imh, imw = h - (H - 1) / 2.0, w - (W - 1) / 2.0
+    f = float(fl)
+    z = d.gather(1, pick) * (f / torch.sqrt(f * f + (imw * imw + imh * imh)))
+    pts = torch.stack([z, -z * imw / f, -z * imh / f], -1)
+    pts = torch.where(ok[..., None], pts, torch.zeros_like(pts)).contiguous()
+    return pts, ok.sum(1).to(torch.int32)
+
+
+def pose_candidates(n_dirs=800, n_rolls=30, dist=CAM_DIST):
+    """A set of K = n_dirs * n_rolls cameras covering SO(3): (rot [K,3,3], eye [K,3]) fp32 on the CPU, in the convention of
+    ``render_depth_views``.  The viewing directions are a Fibonacci sphere of n_dirs points u_i; camera (i, j) sits at
+    eye = dist * u_i, looks at the origin (rot's column 0 = -u_i) and is rolled about that axis by 2 pi j / n_rolls.
+    The frames are built in fp64 from a branch-free orthonormal basis of the forward axis (no up vector, so the poles
+    are as good as anywhere) and rounded once.
+
+    The defaults, 800 directions x 30 rolls = 24,000 cameras, cover SO(3) to 8 degrees: every rotation lies within a
+    geodesic angle of 8 degrees of a candidate (neighbouring directions are about 7 degrees apart, rolls 12 degrees).
+    The largest angle to the nearest candidate over 10^6 seeded uniform rotations, computed on the CPU, is 7.90
+    degrees.  That is inside the 9 degree start from which ``ray_consistency_loss_views`` is known to descend to the
+    pose, and the local search of ``estimate_pose`` narrows it further."""
+    if not (isinstance(n_dirs, int) and isinstance(n_rolls, int) and n_dirs >= 1 and n_rolls >= 1):
+        raise ValueError("pose_candidates: n_dirs and n_rolls must be positive ints, got %r, %r" % (n_dirs, n_rolls))
+    if not (isinstance(dist, (int, float)) and math.isfinite(dist) and dist > math.sqrt(3.0) / 2):
+        raise ValueError("pose_candidates: dist must be finite and above sqrt(3)/2, got %r" % (dist,))
+    i = torch.arange(n_dirs, dtype=torch.float64)
+    zc = 1 - (2 * i + 1) / n_dirs
+    rr = torch.sqrt((1 - zc * zc).clamp_min(0))
+    phi = i * (math.pi * (3 - math.sqrt(5.0)))
+    u = torch.stack([rr * torch.cos(phi), rr * torch.sin(phi), zc], -1)
+    fwd = -u
+    # Duff et al., "Building an orthonormal basis, revisited" (JCGT 2017): b perpendicular to fwd, continuous but at
+    # fwd_z = 0's sign flip
+    s = torch.where(fwd[:, 2] >= 0, 1.0, -1.0).double()
+    a = -1 / (s + fwd[:, 2])
+    b = fwd[:, 0] * fwd[:, 1] * a
+    z0 = torch.stack([1 + s * fwd[:, 0] ** 2 * a, s * b, -s * fwd[:, 0]], -1)
+    y0 = torch.linalg.cross(z0, fwd, dim=-1)
+    th = torch.arange(n_rolls, dtype=torch.float64) * (2 * math.pi / n_rolls)
+    c, sn = torch.cos(th)[None, :, None], torch.sin(th)[None, :, None]
+    z = c * z0[:, None] + sn * y0[:, None]                                      # [n_dirs, n_rolls, 3]
+    f = fwd[:, None].expand_as(z)
+    y = torch.linalg.cross(z, f, dim=-1)
+    rot = torch.stack([f, y, z], -1).reshape(-1, 3, 3)
+    eye = (u * float(dist))[:, None].expand(-1, n_rolls, -1).reshape(-1, 3)
+    return rot.float(), eye.float()
+
+
+def _score_args(field, points, counts, rot, eye, tau):
+    """validated arguments of genre_b200_pose_score, and the tensors they point into"""
+    name = "score_poses"
+    v = _volumes(field, name)
+    n, r = v.shape[0], v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]) or not 1 <= r <= 256:
+        raise ValueError("%s expects cubic fields of side 1 .. 256, got %s" % (name, tuple(field.shape)))
+    _lib.require_cuda(points, counts)
+    _lib.require_f32(points)
+    if points.dim() != 3 or points.shape[0] != n or points.shape[2] != 3:
+        raise ValueError("%s: points [%d,P,3] expected, got %s" % (name, n, tuple(points.shape)))
+    P = points.shape[1]
+    if not 1 <= P <= POSE_MAX_POINTS:
+        raise ValueError("%s: P = %d points per sample, 1 .. %d supported" % (name, P, POSE_MAX_POINTS))
+    if counts.dtype != torch.int32 or counts.shape != (n,):
+        raise ValueError("%s: counts [%d] int32 expected, got %s %s" % (name, n, tuple(counts.shape), counts.dtype))
+    counts = counts.contiguous()                             # the kernel reads counts[n] densely (an expand is stride 0)
+    if not (isinstance(tau, (int, float)) and math.isfinite(tau) and tau > 0):
+        raise ValueError("%s: tau must be a positive finite float, got %r" % (name, tau))
+    rt, et, _, K = _poses(n, rot, eye, 1.0, name)
+    bad = torch.stack([(counts < 1).any(), (counts > P).any()]).cpu()
+    if bad.any():
+        raise ValueError("%s: every count must lie in [1, P = %d]" % (name, P))
+    rt, et = (x.to(v.device).contiguous() for x in (rt, et))
+    pts = points.contiguous()
+    lead = lambda x: x.stride(0) if x.shape[0] > 1 else 0   # noqa: E731 -- 0: candidates shared by the batch
+    args = (v.data_ptr(), n, r, pts.data_ptr(), P, counts.data_ptr(), rt.data_ptr(), lead(rt), rt.stride(1),
+            et.data_ptr(), lead(et), et.stride(1), K, float(tau))
+    return v, (pts, counts, rt, et), args
+
+
+def score_poses(field, points, counts, rot, eye, tau):
+    """Score K candidate cameras per grid against observed points: score[n, k] = the mean over the points p of sample n
+    of c(rot_k p + eye_k), where c is the square of ``field`` interpolated trilinearly at that grid-frame position when
+    it lies inside the grid's voxel centres, and tau^2 outside (the renderers' zero padding would read as "on the
+    surface" there).  Lower is better.
+
+    field [N,R,R,R] (or [N,1,R,R,R]) fp32 on CUDA, a distance to the grid's surface in grid units clamped to ``tau``
+    (as ``estimate_pose`` builds it); points [N,P,3] and counts [N] int32 as ``depth_points`` returns them (P <= 4096);
+    rot [N|1,K,3,3] and eye [N|1,K,3] cameras as ``render_depth_views`` takes them (validated the same way; a leading 1
+    shares them across the batch).  Returns score [N,K] fp32.  Each score is summed in point order by one thread: it is
+    bitwise repeatable and the same whichever other candidates the call holds.  Not differentiable."""
+    v, keep, args = _score_args(field, points, counts, rot, eye, tau)
+    score = torch.empty((args[1], args[12]), dtype=torch.float32, device=v.device)
+    _lib.call("genre_b200_pose_score", *args, score.data_ptr(), _lib.stream_ptr(v))
+    return score
+
+
+def _surface_field(vox, level=0.5, tau=0.1):
+    """the field ``estimate_pose`` scores against: the distance in grid units to the shell of ``vox >= level`` (its
+    occupied voxels with an empty 26-neighbour or on the border), clamped to ``tau``; [N,R,R,R]"""
+    v = _volumes(vox, "estimate_pose")
+    r = v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]) or r % 32 or r > 256:
+        raise ValueError("estimate_pose: cubic grids of side a multiple of 32 up to 256 expected, got %s"
+                         % (tuple(vox.shape),))
+    shell = voxel_surface((v >= level).float(), iterations=1, transpose_flip=False)
+    return (distance_transform(shell) / r).clamp_(max=float(tau))
+
+
+def _cam_turn(rot, eye, w):
+    """turn cameras about the grid's centre by the axis-angle w given in each camera's own frame: rot A(w), and the eye
+    carried along by the same world rotation rot A(w) rot^T"""
+    A = axis_angle_rotation(w)
+    r = rot @ A
+    return r, (r @ (rot.transpose(-1, -2) @ eye[..., None]))[..., 0]
+
+
+def _refine_poses(vox, obs_depth, rot0, eye0, fl=CAM_FL, steps=200, lr=0.01):
+    """Fit M camera poses per grid to one observed depth map by ``ray_consistency_loss_views`` with the grid frozen:
+    Adam on each camera's axis-angle offset w (turning it about the grid's centre, rot = A(w) rot0, eye = A(w) eye0)
+    and eye offset de.  vox [N,1,R,R,R], obs_depth [N,1,H,W] or [N,H,W] (the M poses are M views of the grid against
+    the same map, expanded with stride 0), rot0 [N,M,3,3], eye0 [N,M,3] on CUDA.  Returns (rot [N,M,3,3], eye [N,M,3],
+    loss [N,M]): the fitted poses and each one's per-ray mean loss after the last step."""
+    obs = obs_depth[:, 0] if obs_depth.dim() == 4 else obs_depth
+    N, M = rot0.shape[:2]
+    obs = obs[:, None].expand(N, M, obs.shape[-2], obs.shape[-1])
+    vox = vox.detach()
+    w = torch.zeros(N, M, 3, device=rot0.device, requires_grad=True)
+    de = torch.zeros(N, M, 3, device=rot0.device, requires_grad=True)
+    opt = torch.optim.Adam([w, de], lr=lr)
+    for _ in range(steps):
+        opt.zero_grad()
+        A = axis_angle_rotation(w)
+        loss = ray_consistency_loss_views(vox, obs, A @ rot0, (A @ eye0[..., None])[..., 0] + de, fl, reduction="none")
+        loss.mean((2, 3)).sum().backward()
+        opt.step()
+    with torch.no_grad():
+        A = axis_angle_rotation(w)
+        rot, eye = A @ rot0, (A @ eye0[..., None])[..., 0] + de
+        loss = ray_consistency_loss_views(vox, obs, rot, eye, fl, reduction="none").mean((2, 3))
+    return rot, eye, loss
+
+
+def estimate_pose(vox, obs_depth, fl=CAM_FL, level=0.5, dist=CAM_DIST, n_dirs=800, n_rolls=30, n_points=2048,
+                  tau=0.1, keep=4, rounds=6, turn=math.radians(8.0), shift=0.05, steps=200, lr=0.01, seed=0):
+    """The camera pose of each grid that best explains an observed depth map, searched over all of SO(3).
+
+    vox [N,1,R,R,R] (or [N,R,R,R]) fp32 occupancy on CUDA in its own (e.g. canonical) frame, R a multiple of 32 up to
+    256; obs_depth [N,1,H,W] or [N,H,W] ray depths from the camera (<= 0 background), as ``ray_consistency_loss_views``
+    takes them, with focal length ``fl``.  Returns (rot [N,3,3], eye [N,3], loss [N]): the pose in the convention of
+    ``render_depth_views`` and its final ``ray_consistency_loss_views`` per-ray mean.  Four steps:
+
+      1. field = the distance field: the distance to the shell of ``vox >= level``, in grid units,
+         clamped to ``tau`` (``voxel_surface`` and ``distance_transform``); points = ``depth_points(obs_depth, fl,
+         n_points, seed)``.
+      2. ``score_poses`` of the ``pose_candidates(n_dirs, n_rolls, dist)`` cameras, shared by the batch; the ``keep``
+         lowest scores of each sample survive (ties to the lower candidate index).
+      3. ``rounds`` rounds of a pattern search on the score, each one ``score_poses`` call: each survivor's pose and its
+         12 neighbours, turned by +-``turn`` about each of its camera's axes (about the grid's centre) and moved by
+         +-``shift`` along each axis.  Per axis the better of the three is taken and the survivor moves by all of those
+         steps at once; then ``turn`` and ``shift`` halve.  The best pose scored so far is kept.
+      4. an Adam fit of the survivors together by ``ray_consistency_loss_views`` (``steps`` Adam steps at ``lr``), and the pose with the lowest final
+         loss is returned (the lowest survivor index on ties).  The depth- and visibility-aware loss, not the score,
+         settles front/back ambiguities between survivors.
+
+    Defaults and why:
+      n_dirs=800, n_rolls=30: covering radius 8 degrees on SO(3) (see ``pose_candidates``), so the nearest candidate
+        is within the 9 degrees from which the refinement is known to descend even before the local search;
+      n_points=2048: the score's cost is linear in it, and 2048 surface points sample a 128^2 silhouette densely;
+      tau=0.1: a tenth of the grid; a point 8 degrees off at the grid's corner (0.87 from the centre) moves 0.12, so
+        the clamp keeps the score's basin about as wide as the candidate spacing while bounding what outliers cost;
+      keep=4: survivors that reach the refinement, a few basins deep for near-ties (front/back) at 4 views' cost;
+      rounds=6, turn=8 degrees, shift=0.05: the turn starts at the covering radius and ends at 0.25 degrees; the
+        shift covers the eye's offset from the candidates' sphere of radius ``dist`` (the eye need not look exactly
+        at the centre) and ends at 0.0016;
+      steps=200, lr=0.01: the pose fit of the existing recovery test, which settles from 9 degrees away.
+
+    The score matches the observed points to the grid's surface, so a shape symmetric under a rotation returns one
+    pose of its symmetry class; intrinsics and scale are not estimated."""
+    name = "estimate_pose"
+    v = _volumes(vox, name)
+    N, r = v.shape[0], v.shape[1]
+    if not (v.shape[1] == v.shape[2] == v.shape[3]) or r % 32 or r > 256:
+        raise ValueError("%s: cubic grids of side a multiple of 32 up to 256 expected, got %s" % (name, tuple(vox.shape)))
+    if not (isinstance(keep, int) and isinstance(rounds, int) and isinstance(steps, int) and keep >= 1 and rounds >= 0
+            and steps >= 0):
+        raise ValueError("%s: keep >= 1, rounds >= 0 and steps >= 0 must be ints" % name)
+    obs = obs_depth[:, 0] if obs_depth.dim() == 4 and obs_depth.shape[1] == 1 else obs_depth
+    if obs.dim() != 3 or obs.shape[0] != N:
+        raise ValueError("%s: obs_depth [%d,1,H,W] expected, got %s" % (name, N, tuple(obs_depth.shape)))
+    dev = v.device
+    with torch.no_grad():
+        field = _surface_field(v, level, tau)
+        pts, cnt = depth_points(obs, fl, n_points, seed)
+        rot_c, eye_c = pose_candidates(n_dirs, n_rolls, dist)
+        if keep > rot_c.shape[0]:
+            raise ValueError("%s: keep = %d exceeds the %d candidates" % (name, keep, rot_c.shape[0]))
+        sc = score_poses(field, pts, cnt, rot_c[None].to(dev), eye_c[None].to(dev), tau)
+        top = torch.sort(sc, dim=1, stable=True).indices[:, :keep]                    # [N, M]
+        rot, eye = rot_c.to(dev)[top], eye_c.to(dev)[top]
+        best_s = torch.full((N, keep), math.inf, device=dev)
+        best_r, best_e = rot.clone(), eye.clone()
+        I3 = torch.eye(3, device=dev)
+        moves = torch.cat([I3, -I3])                                                   # +-axis, [6, 3]
+        for i in range(rounds):
+            t, dt = turn / 2 ** i, shift / 2 ** i
+            rr, ee = _cam_turn(rot[:, :, None], eye[:, :, None], (moves * t)[None, None])  # [N, M, 6, ...]
+            re = rot[:, :, None].expand(-1, -1, 6, -1, -1)
+            ems = eye[:, :, None] + dt * (rot[:, :, None] @ moves[None, None, :, :, None])[..., 0]
+            cr = torch.cat([rot[:, :, None], rr, re], 2)                               # [N, M, 13, 3, 3]
+            ce = torch.cat([eye[:, :, None], ee, ems], 2)
+            s = score_poses(field, pts, cnt, cr.reshape(N, -1, 3, 3), ce.reshape(N, -1, 3), tau).view(N, keep, 13)
+            j = s.argmin(2)                                                            # the lowest index on ties
+            sj = s.gather(2, j[..., None])[..., 0]
+            better = sj < best_s
+            best_s = torch.where(better, sj, best_s)
+            best_r = torch.where(better[..., None, None], cr.gather(2, j[..., None, None, None].expand(-1, -1, 1, 3, 3))[:, :, 0],
+                                 best_r)
+            best_e = torch.where(better[..., None], ce.gather(2, j[..., None, None].expand(-1, -1, 1, 3))[:, :, 0], best_e)
+            # per axis: -1, 0 or +1 step, whichever of the three scores lowest (0 on ties)
+            s0 = s[..., :1]
+            sa, sb = s[..., 1:7], s[..., 7:13]
+            step = lambda lo_p, lo_m: torch.where((lo_p < s0) & (lo_p <= lo_m), 1.0, torch.where(lo_m < s0, -1.0, 0.0))  # noqa: E731
+            wr = step(sa[..., :3], sa[..., 3:])
+            wt = step(sb[..., :3], sb[..., 3:])
+            rot, eye = _cam_turn(rot, eye, wr * t)
+            eye = eye + dt * (rot @ wt[..., None])[..., 0]
+        if rounds:
+            rot, eye = best_r, best_e
+        rot = _orthonormalise(rot)
+    rot, eye, loss = _refine_poses(v[:, None], obs[:, None], rot, eye, fl, steps, lr)
+    j = loss.argmin(1)                                                                 # the lowest index on ties
+    ar = torch.arange(N, device=dev)
+    return rot[ar, j], eye[ar, j], loss[ar, j]
+
+
+def _orthonormalise(rot):
+    """Gram-Schmidt in fp64, rounded once, as ``look_at`` forms its frames: composed fp32 turns drift from orthonormality"""
+    r = rot.double()
+    x = r[..., 0] / r[..., 0].norm(dim=-1, keepdim=True)
+    z = r[..., 2] - (r[..., 2] * x).sum(-1, keepdim=True) * x
+    z = z / z.norm(dim=-1, keepdim=True)
+    return torch.stack([x, torch.linalg.cross(z, x, dim=-1), z], -1).float()

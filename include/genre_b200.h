@@ -853,6 +853,40 @@ int genre_b200_emd_forward(const float *p, const float *q, int64_t B, int64_t n,
                            void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Exact Euclidean distance transform of N cubic grids (separable lower envelopes, Felzenszwalb & Huttenlocher 2012):
+ *   vox     [N, R, R, R] fp32, dense; 1 <= R <= 256, 1 <= N <= 65535, level not NaN.
+ *   out_sq  [N, R, R, R] fp32, dense, must not alias vox: for every voxel, the squared Euclidean distance in voxel units
+ *           to the nearest voxel of the same grid with value >= level.  Every value is an integer, at most 3 (R-1)^2
+ *           < 2^24, so it is exact; a grid with no such voxel is +inf everywhere.  Parabola intersections are compared by
+ *           int64 cross-multiplication: the result is exact and independent of scheduling and of the rest of the batch.
+ *   Three kernels (one per axis), all in place on out_sq; no workspace.
+ * ------------------------------------------------------------------------------------------- */
+int genre_b200_distance_transform(const float *vox, int64_t N, int res, float level, float *out_sq, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Scores of K candidate cameras per grid against observed camera-frame points (no backward: a search, not a loss).
+ *   field   [N, R, R, R] fp32, dense: a distance to the grid's surface in grid units, finite (the caller clamps it to tau);
+ *           1 <= R <= 256, 1 <= N <= 65535.
+ *   points  [N, P, 3] fp32, dense: points in the camera frame (x forward, +y towards image -w, +z towards image -h);
+ *           1 <= P <= 4096.  counts [N] int32: rows 0 .. counts[n]-1 of sample n are its points.  A count outside
+ *           [1, P] is not dereferenced: that sample's scores are NaN (callers check the counts on the host first).
+ *   rot     element (n, k) at rot + n rN + k rK, a dense row-major 3x3 whose columns are the camera's axes in the grid
+ *           frame; eye at eye + n eN + k eK, 3 floats: the camera's centre.  rN = eN = 0 shares the candidates across the
+ *           batch.  The convention of genre_b200_render_views_*.  1 <= K <= 2^30, strides >= 0, tau > 0 finite.
+ *   score   [N, K] fp32: score[n, k] = (sum_p c_p) / counts[n], with, in fp32, one rounding per operation:
+ *             x_i = fma(rot[i][2], p_z, fma(rot[i][1], p_y, rot[i][0] * p_x)) + eye_i
+ *             f_i = (x_i + 0.5) * R - 0.5
+ *             c_p = v * v, v = the trilinear interpolation of field at f (render.cuh's make_taps_at /
+ *                   sample_trilinear<false>), if 0 <= f_i <= R - 1 on all three axes; else c_p = tau * tau.
+ *           The sum starts at 0 and adds c_0, c_1, ... in point order on one thread, so a candidate's score is bitwise
+ *           repeatable and does not depend on K, on the other candidates or on the launch tiling.
+ *   Every buffer 4-byte aligned (else GENRE_B200_EALIGN); arguments are checked before the launch.
+ * ------------------------------------------------------------------------------------------- */
+int genre_b200_pose_score(const float *field, int64_t N, int res, const float *points, int64_t P, const int32_t *counts,
+                          const float *rot, int64_t rN, int64_t rK, const float *eye, int64_t eN, int64_t eK, int64_t K,
+                          float tau, float *score, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Conservative voxelisation of batched triangle meshes, the inverse of genre_b200_isosurface_*: ground-truth meshes become
  * grids for voxel_iou / voxel_fill and training targets without a CPU tool.
  *   meshes  the packed format of genre_b200_isosurface_*: verts [V, 3] fp32, faces [F, 3] int32 indexing the sample's own

@@ -1584,9 +1584,10 @@ def back_project_views(depth, rot, eye, fl=CAM_FL, res=128, shift=True):
 # ---- the camera pose of a canonical-frame grid from a depth map: distance transforms, candidate scoring, refinement ------
 def distance_transform(vox, level=0.5):
     """Exact Euclidean distance transform: vox [N,1,R,R,R] or [N,R,R,R] fp32 on CUDA, 1 <= R <= 256 -> the distance, in
-    voxel units, from every voxel to the nearest voxel of its grid with value >= ``level``, in vox's shape.  It equals
-    ``scipy.ndimage.distance_transform_edt(v < level)`` per sample: the kernel's squared distances are exact integers and
-    this is their fp32 square root.  A grid with no voxel >= level is +inf everywhere.  Divide by R for grid units, as a
+    voxel units, from every voxel to the nearest voxel of its grid with value >= ``level``, in vox's shape; a NaN voxel is
+    never such a voxel.  It equals ``scipy.ndimage.distance_transform_edt(~(v >= level))`` per sample (not ``v < level``,
+    which counts NaN voxels as features): the kernel's squared distances are exact integers and this is their fp32
+    square root.  A grid with no voxel >= level is +inf everywhere.  Divide by R for grid units, as a
     truncated-distance target or to measure a shell's thickness."""
     v = _volumes(vox, "distance_transform")
     n, r = v.shape[0], v.shape[1]

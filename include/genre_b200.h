@@ -856,7 +856,8 @@ int genre_b200_emd_forward(const float *p, const float *q, int64_t B, int64_t n,
  * Exact Euclidean distance transform of N cubic grids (separable lower envelopes, Felzenszwalb & Huttenlocher 2012):
  *   vox     [N, R, R, R] fp32, dense; 1 <= R <= 256, 1 <= N <= 65535, level not NaN.
  *   out_sq  [N, R, R, R] fp32, dense, must not alias vox: for every voxel, the squared Euclidean distance in voxel units
- *           to the nearest voxel of the same grid with value >= level.  Every value is an integer, at most 3 (R-1)^2
+ *           to the nearest voxel of the same grid with value >= level (a NaN voxel never is one; level may be +-inf).
+ *           Every value is an integer, at most 3 (R-1)^2
  *           < 2^24, so it is exact; a grid with no such voxel is +inf everywhere.  Parabola intersections are compared by
  *           int64 cross-multiplication: the result is exact and independent of scheduling and of the rest of the batch.
  *   Three kernels (one per axis), all in place on out_sq; no workspace.

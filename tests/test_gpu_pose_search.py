@@ -17,7 +17,7 @@ FL = 418.3
 
 
 def _edt_ref(v, level=0.5):
-    m = v < level
+    m = ~(v >= level)                                   # the features are v >= level: a NaN voxel is never one
     if m.all():
         return np.full(v.shape, np.inf)
     return ndimage.distance_transform_edt(m)

@@ -142,6 +142,7 @@ _SIGNATURES = {
     "genre_b200_preprocess": [_int, _int, _ptr, _ptr, _int, _i64, _i64, _i64, _i64, _int, _f64, _ptr, _ptr, _ptr, _ptr, _ptr,
                               _size, _ptr],
     "genre_b200_mesh_voxelize": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _int, _int, _int, _ptr, _ptr, _size, _ptr],
+    "genre_b200_winding_number": [_ptr, _i64, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _i64, _int, _int, _int, _ptr, _ptr],
 }
 
 # every symbol include/genre_b200.h declares (tests check the library exports all of them)
@@ -193,6 +194,9 @@ _LAUNCHES = {
     "genre_b200_preprocess": lambda kind, train, *_: 1 + (kind != 0) + (3 if kind == 0 and train else 0),
     # count, scan and columns only when there are faces, then the expand kernel
     "genre_b200_mesh_voxelize": lambda verts, V, faces, F, *_: 4 if F > 0 else 1,
+    # one kernel unless there are no queries
+    "genre_b200_winding_number": lambda verts, V, faces, F, vo, fo, N, points, P, pN, D, H, W, *_:
+        int((P if points else D * H * W) > 0),
 }
 
 

@@ -74,6 +74,29 @@ __device__ __forceinline__ void split_hi_lo8(const float (&x)[8], uint4 &hi, uin
   lo = pack_half8(l);
 }
 
+// The face rule of genre_b200_mesh_voxelize and genre_b200_winding_number: a face (p[0], p[1], p[2]) is kept iff every
+// vertex coordinate is finite and its fp64 normal e1 x e2 (e1 = p1 - p0, e2 = p2 - p0 from the fp32 vertices, one rounding
+// per operation, nx = e1y*e2z - e1z*e2y, ...: genre_b200_surface_sample's weight order) is not exactly 0.  A skipped face
+// contributes nothing.
+__device__ __forceinline__ bool mesh_face_kept(const float (&p)[3][3]) {
+  bool finite = true;
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int a = 0; a < 3; ++a) finite = finite && isfinite(p[k][a]);
+  if (!finite) return false;
+  double e1[3], e2[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    e1[a] = __dsub_rn((double)p[1][a], (double)p[0][a]);
+    e2[a] = __dsub_rn((double)p[2][a], (double)p[0][a]);
+  }
+  const double nx = __dsub_rn(__dmul_rn(e1[1], e2[2]), __dmul_rn(e1[2], e2[1]));
+  const double ny = __dsub_rn(__dmul_rn(e1[2], e2[0]), __dmul_rn(e1[0], e2[2]));
+  const double nz = __dsub_rn(__dmul_rn(e1[0], e2[1]), __dmul_rn(e1[1], e2[0]));
+  return !(nx == 0.0 && ny == 0.0 && nz == 0.0);
+}
+
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));

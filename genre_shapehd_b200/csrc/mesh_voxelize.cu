@@ -9,7 +9,8 @@
 //           rounding per operation, no contraction, in the order written.  Grid units: g_a = (p_a + 0.5) * n_a, so the voxel
 //           is the box [i_a, i_a + 1].
 //   skip    a face with a non-finite vertex coordinate, or whose normal e1 x e2 (e1 = b - a, e2 = c - a, components as in
-//           csrc/surface_sample.cu: nx = e1y*e2z - e1z*e2y, ...) is exactly 0 in all three components.
+//           csrc/surface_sample.cu: nx = e1y*e2z - e1z*e2y, ...) is exactly 0 in all three components (common.cuh's
+//           mesh_face_kept, shared with csrc/winding.cu).
 //   test    a voxel is set iff the closed triangle and the closed cube intersect, by the separating-axis test in grid units
 //           (touching is overlap: a separation needs a strict inequality):
 //             box axes   voxel i_a lies in [max(ceil(min_k g_ka) - 1, 0), min(floor(max_k g_ka), n_a - 1)] on every axis;
@@ -64,27 +65,13 @@ struct MvFace {
 __device__ __forceinline__ bool mv_face(const float *__restrict__ vb, const int *__restrict__ fp, const int (&dims)[3],
                                         MvFace &F) {
   float p[3][3];
-  bool finite = true;
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     const float *q = vb + 3 * __ldg(fp + k);
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      p[k][a] = __ldg(q + a);
-      finite = finite && isfinite(p[k][a]);
-    }
+    for (int a = 0; a < 3; ++a) p[k][a] = __ldg(q + a);
   }
-  if (!finite) return false;
-  double e1[3], e2[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    e1[a] = __dsub_rn((double)p[1][a], (double)p[0][a]);
-    e2[a] = __dsub_rn((double)p[2][a], (double)p[0][a]);
-  }
-  const double nx = __dsub_rn(__dmul_rn(e1[1], e2[2]), __dmul_rn(e1[2], e2[1]));
-  const double ny = __dsub_rn(__dmul_rn(e1[2], e2[0]), __dmul_rn(e1[0], e2[2]));
-  const double nz = __dsub_rn(__dmul_rn(e1[0], e2[1]), __dmul_rn(e1[1], e2[0]));
-  if (nx == 0.0 && ny == 0.0 && nz == 0.0) return false;
+  if (!mesh_face_kept(p)) return false;
 #pragma unroll
   for (int k = 0; k < 3; ++k)
 #pragma unroll

@@ -907,7 +907,8 @@ def voxelize_mesh(verts, faces, vert_off, face_off, shape=128):
 
     The rule is conservative: every path of closed cubes from the inside of a closed mesh to the outside meets a set voxel,
     so ``voxel_fill(voxelize_mesh(...))`` is the solid of a closed mesh.  An open mesh leaks: its fill is its shell plus
-    whatever it does enclose.  Deterministic, batch-equivariant, and nothing is copied to the host (graph-capturable)."""
+    whatever it does enclose; ``mesh_occupancy`` gives the solid of open and self-intersecting meshes.  Deterministic,
+    batch-equivariant, and nothing is copied to the host (graph-capturable)."""
     b, verts, faces, vert_off, face_off = _mesh_args("voxelize_mesh", verts, faces, vert_off, face_off)
     d, h, w = (int(shape),) * 3 if np.ndim(shape) == 0 else (int(s) for s in shape)
     nbytes = _lib.load().genre_b200_mesh_voxelize_workspace_bytes(b, faces.shape[0], d, h, w)
@@ -922,8 +923,69 @@ def voxelize_mesh(verts, faces, vert_off, face_off, shape=128):
     return out
 
 
+def winding_number(verts, faces, vert_off, face_off, points=None, shape=None):
+    """Generalized winding numbers (Jacobson, Kavan & Sorkine-Hornung 2013) of every sample's triangle mesh, on the device:
+    w(q) = the sum of the signed solid angles of the faces seen from q, over 4 pi.  1 inside and 0 outside a closed,
+    consistently oriented mesh; across holes and self-intersections it changes smoothly, so |w| > 0.5 is the intended solid.
+
+    The meshes are packed as for ``voxelize_mesh``.  Give exactly one of
+      * ``points`` [B|1, P, 3] fp32 on the mesh's device (one table per sample, or one shared): returns w [B, P] fp32;
+      * ``shape``, an int or (D, H, W), every dimension in [1, 512]: w at the voxel centres of ``voxelize_mesh``'s frame,
+        c_a = fl(fl(i_a + 0.5) / n_a) - 0.5 in fp32, as [B, 1, D, H, W] fp32 (``points`` fed those centres gives the same
+        bits).
+    The sum is exact over every (query, face) pair, no tree or far-field approximation: its cost is P (or D*H*W) times the
+    sample's faces.  Faces with a non-finite vertex or an exactly zero normal contribute nothing (``voxelize_mesh``'s rule);
+    a query on a face's plane gets 0 from that face.  The fp32 terms are summed in fp64 in face order, so the result is
+    bitwise repeatable and does not depend on the batch; include/genre_b200.h states the arithmetic and tests/winding_ref.py
+    bounds its error.  One kernel, nothing copied to the host (graph-capturable)."""
+    b, verts, faces, vert_off, face_off = _mesh_args("winding_number", verts, faces, vert_off, face_off)
+    if (points is None) == (shape is None):
+        raise ValueError("winding_number: give exactly one of points and shape")
+    if faces.shape[0] >= 1 << 31:
+        raise ValueError("winding_number: %d faces, fewer than 2^31 expected" % faces.shape[0])
+    mesh = (verts.data_ptr(), verts.shape[0], faces.data_ptr(), faces.shape[0], vert_off.data_ptr(), face_off.data_ptr(), b)
+    stream = _lib.stream_ptr(verts)
+    if points is not None:
+        _lib.require_cuda(points)
+        _lib.require_f32(points)
+        if points.dim() != 3 or points.shape[2] != 3 or points.shape[0] not in (1, b):
+            raise ValueError("winding_number: points [B|1, P, 3] expected with B = %d, got %s" % (b, tuple(points.shape)))
+        if points.device != verts.device:
+            raise ValueError("winding_number: points on %s, meshes on %s" % (points.device, verts.device))
+        pts = points.contiguous()
+        p = pts.shape[1]
+        out = torch.empty((b, p), dtype=torch.float32, device=verts.device)
+        if p > 0:                             # an empty tensor's data pointer is null, which means grid mode
+            _lib.call("genre_b200_winding_number", *mesh, pts.data_ptr(), p, 0 if pts.shape[0] == 1 else 3 * p, 0, 0, 0,
+                      out.data_ptr(), stream)
+        return out
+    d, h, w = (int(shape),) * 3 if np.ndim(shape) == 0 else (int(s) for s in shape)
+    if not all(1 <= s <= 512 for s in (d, h, w)):
+        raise ValueError("winding_number: grid %dx%dx%d unsupported (every dimension in [1, 512])" % (d, h, w))
+    out = torch.empty((b, 1, d, h, w), dtype=torch.float32, device=verts.device)
+    _lib.call("genre_b200_winding_number", *mesh, None, 0, 0, d, h, w, out.data_ptr(), stream)
+    return out
+
+
+def mesh_occupancy(verts, faces, vert_off, face_off, shape=128):
+    """The solid of every sample's triangle mesh as an occupancy grid, for open and self-intersecting meshes too:
+    [B,1,D,H,W] fp32, 1.0 where ``voxelize_mesh`` sets the voxel (the shell) or |w| > 0.5 at its centre (``winding_number``
+    in grid mode), 0.0 elsewhere.  The meshes and ``shape`` as for ``voxelize_mesh``.
+
+    Counting the shell keeps thin parts that no voxel centre lies inside; taking |w| gives a mesh whose faces all wind the
+    other way the same solid.  On a closed, consistently oriented mesh this is ``voxel_fill(voxelize_mesh(...))`` except
+    for exterior pockets the shell seals off, which the fill counts and this does not.  A hole loses only what it uncovers:
+    inside a box with a missing face w stays above 0.5 everywhere, while a sphere missing a cap also loses the dome beyond
+    the cap's rim plane.  What it does not fix: patches of inconsistent orientation, where w can be near 0 inside (their
+    solid angles cancel).  The cost is ``winding_number``'s, D*H*W times the faces of a sample.  Nothing is copied to the
+    host (graph-capturable)."""
+    occ = voxelize_mesh(verts, faces, vert_off, face_off, shape)
+    w = winding_number(verts, faces, vert_off, face_off, shape=shape)
+    return occ.masked_fill_(w.abs() > 0.5, 1.0)
+
+
 def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=1024, tau=0.01, seed=0, six_way=True, emd=False,
-                 emd_eps=1e-5):
+                 emd_eps=1e-5, gt_solid="fill"):
     """``voxel_metrics`` of predicted grids against ground-truth triangle meshes given in the same frame (the centred unit
     cube, ``voxelize_mesh``'s; aligning and normalising the meshes is the caller's).
 
@@ -931,9 +993,13 @@ def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=102
       * points on the prediction: ``marching_cubes(pred, level)`` in voxel_metrics' frame, then ``sample_surface``;
       * points on the ground truth: ``sample_surface`` of the meshes, with the same seeds;
       * chamfer / F-score, ``valid``, the NaNs of invalid samples and the opt-in ``emd`` exactly as ``voxel_metrics``;
-      * iou = voxel_iou(pred, voxel_fill(voxelize_mesh(meshes, (D, H, W)), six_way), level, 0.5).
+      * iou = voxel_iou(pred, solid, level, 0.5) with solid = voxel_fill(voxelize_mesh(meshes, (D, H, W)), six_way) for
+        ``gt_solid="fill"`` (the default), or mesh_occupancy(meshes, (D, H, W)) for ``gt_solid="winding"``, which keeps the
+        solid of open and self-intersecting meshes (``six_way`` is then unused).  Every other key is the same either way.
     Given the ground truth as ``marching_cubes(gt)`` in voxel_metrics' frame, every metric but ``iou`` equals voxel_metrics'
     bit for bit.  The marching-cubes call synchronises once; nothing else does."""
+    if gt_solid not in ("fill", "winding"):
+        raise ValueError("mesh_metrics: gt_solid must be 'fill' or 'winding', got %r" % (gt_solid,))
     a = _volumes(pred, "mesh_metrics")
     b = a.shape[0]
     nb, verts, faces, vert_off, face_off = _mesh_args("mesh_metrics", verts, faces, vert_off, face_off)
@@ -942,7 +1008,10 @@ def mesh_metrics(pred, verts, faces, vert_off, face_off, level=0.5, n_points=102
     seeds = _seeds(seed, b, a.device)
     pp, fp = _grid_surface_points(a, level, n_points, seeds)
     pg, fg = sample_surface(verts, faces, vert_off, face_off, n_points, seeds)
-    solid = voxel_fill(voxelize_mesh(verts, faces, vert_off, face_off, tuple(a.shape[1:])), six_way)
+    if gt_solid == "winding":
+        solid = mesh_occupancy(verts, faces, vert_off, face_off, tuple(a.shape[1:]))
+    else:
+        solid = voxel_fill(voxelize_mesh(verts, faces, vert_off, face_off, tuple(a.shape[1:])), six_way)
     return _point_metrics(pp, fp, pg, fg, tau, voxel_iou(a, solid[:, 0].float(), level, 0.5)[0].double(),
                           emd_eps if emd else None)
 

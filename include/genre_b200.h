@@ -919,6 +919,41 @@ int genre_b200_mesh_voxelize(const float *verts, int64_t V, const int32_t *faces
                              size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Generalized winding numbers of batched triangle meshes (Jacobson, Kavan & Sorkine-Hornung 2013), the exact sum over every
+ * face: w(q) = sum_f Omega_f(q) / 4 pi, the signed solid angles of the faces seen from q.  1 inside and 0 outside a closed,
+ * consistently oriented mesh; across holes and self-intersections it changes smoothly, so |w| > 0.5 is the intended solid.
+ *   meshes  the packed format of genre_b200_isosurface_* / genre_b200_mesh_voxelize: verts [V, 3] fp32, faces [F, 3] int32
+ *           indexing the sample's own vertex block (trusted: in [0, V_n)), vert_off / face_off [N+1] int64 on the device.
+ *           F (the total) < 2^31, 1 <= N <= 65535.
+ *   queries points mode (points != NULL): points [N|1, P, 3] fp32, sample n's table at points + n pN, pN = 3P or 0 (one
+ *           table shared by the batch), 0 <= P < 2^31, D = H = W = 0; out [N, P].
+ *           grid mode (points == NULL): P = pN = 0, every dimension of the D x H x W grid in [1, 512]; the query of voxel
+ *           (i0, i1, i2) is its centre in genre_b200_mesh_voxelize's frame, c_a = fl(fl(i_a + 0.5) / n_a) - 0.5 in fp32
+ *           ((n0, n1, n2) = (D, H, W), axis 0 = vertex coordinate 0); out [N, D, H, W].  Points mode fed these fp32 centres
+ *           gives the same bits.
+ *   skip    a face with a non-finite vertex coordinate, or whose fp64 normal (b - a) x (c - a) from the fp32 vertices is
+ *           exactly 0 (genre_b200_mesh_voxelize's rule), contributes 0.
+ *   term    for a kept face (v0, v1, v2) and query q, in fp32, one rounding per operation, fma only where written:
+ *             n_x = fma(e1y, e2z, -(e1z*e2y)), n_y = fma(e1z, e2x, -(e1x*e2z)), n_z = fma(e1x, e2y, -(e1y*e2x)),
+ *                   e1 = v1 - v0, e2 = v2 - v0;
+ *             a = v0 - q, b = v1 - q, c = v2 - q;
+ *             det = fma(a_z, n_z, fma(a_y, n_y, a_x*n_x))          (= a . (b x c) in exact arithmetic);
+ *             la = sqrt(fma(a_z, a_z, fma(a_y, a_y, a_x*a_x))), lb, lc likewise (sqrt correctly rounded);
+ *             ab = fma(a_z, b_z, fma(a_y, b_y, a_x*b_x)), bc = (b, c), ca = (c, a) likewise;
+ *             den = fma(ca, lb, fma(bc, la, fma(ab, lc, (la*lb)*lc)));
+ *             term = 0 if det == 0 (q on the face's plane, an edge or a vertex), else atan2f(det, den) = Omega_f / 2.
+ *   sum     S = the fp64 sum of the terms, from 0, in face order on one thread; w = fl32(S * 0.15915494309189535) (the fp64
+ *           value nearest 1 / 2 pi).  A sample without faces gives 0.  So w is bitwise repeatable and does not depend on
+ *           the batch, on P, on the other samples or on the launch tiling.  tests/winding_ref.py restates the contract in
+ *           fp64 with a per-query bound on this fp32 order's error.
+ *   One launch (none when the query count is 0), no workspace, no host synchronisation: graph-capturable.  fp32 and int32
+ *   buffers 4-byte aligned, offsets 8-byte aligned (else GENRE_B200_EALIGN); arguments are checked before the launch.
+ * ------------------------------------------------------------------------------------------- */
+int genre_b200_winding_number(const float *verts, int64_t V, const int32_t *faces, int64_t F, const int64_t *vert_off,
+                              const int64_t *face_off, int64_t N, const float *points, int64_t P, int64_t pN, int D, int H,
+                              int W, float *out, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Input preprocessing: the test-time silhouette crop (util_img.get_bbox + util_img.crop of every preprocess_wrapper) and
  * MarrnetBaseModel.preprocess (models/marrnetbase.py:71-126), batched.  fp64 in the reference's operation order, one
  * rounding per operation, no FMA (fp32 only where stated); outputs rounded once to fp32, as convert_to_float32 does.

@@ -7,6 +7,8 @@
 //           p (value v0) to q (value v1) along axis a:  t = fl(fl(level - v0) / fl(v1 - v0)),
 //           x_a = fl(fl(fl(p_a + t) * spacing_a) - shift_a),  x_b = fl(fl(p_b * spacing_b) - shift_b) for the other axes.
 //           Every step rounds once (__fadd_rn / __fmul_rn / __fdiv_rn; no FMA contraction).  Axis 0 is the array's first axis.
+//           Non-finite voxels take the same formula: a finite p and an infinite q give t = +-0 (the vertex is p); a NaN end
+//           or an infinite p gives a NaN t and x_a.
 //           Order: by sample, grid point linear index (i*H + j)*W + k, then axis.
 //   cells   per-cell segment linking, no case table.  On each of the cell's 6 faces, walked counter-clockwise as seen from
 //           outside the cell, an edge is an ENTRY (outside -> inside corner) or an EXIT (inside -> outside); every entry is linked

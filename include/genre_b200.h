@@ -656,6 +656,8 @@ int genre_b200_voxel_surface(const float *vox, int64_t N, int res, int iteration
  *             (value v0) to q (value v1) along axis a: t = fl(fl(level - v0) / fl(v1 - v0)),
  *             x_a = fl(fl(fl(p_a + t) * spacing_a) - shift_a), x_b = fl(fl(p_b * spacing_b) - shift_b) for the other axes
  *             (one rounding per step, no FMA).  Axis 0 is the first array axis (skimage's convention).
+ *             Non-finite voxels follow the same formula: a crossing edge with a finite low end p and an infinite high end
+ *             has t = +-0, so its vertex is p; with a NaN end, or an infinite low end, t and x_a are NaN.
  *             Order: sample, point index (i*H + j)*W + k, axis.
  *   faces:    per-cell segment linking with the asymptotic decider on ambiguous faces (inside corners a, d on a diagonal
  *             are joined iff fl(a'*d') > fl(b'*c'), x' = fl(x - level)); loops fanned as (v0, v_i, v_{i+1}).  Interior
